@@ -1027,7 +1027,7 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums(const ui
 static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums16(const uint16_t *__restrict__ H, uint32_t tiles, uint32_t chunk_shift, uint32_t *__restrict__ C,
                                                                           uint32_t *__restrict__ ctl_counts = nullptr)
 {
-    // ctl_counts (optional): the global digit counts are accumulated there as well (callers that do not run k_wide_chunk_scan)
+    // ctl_counts (optional): the global digit counts are accumulated there as well (callers that do not run k_wide_tile_bases)
     const uint32_t chunk = blockIdx.x, tid = threadIdx.x;
     const uint32_t t0 = chunk << chunk_shift, t1 = min(tiles, t0 + (1u << chunk_shift));
     uint4 acc = make_uint4(0, 0, 0, 0);
@@ -1043,84 +1043,116 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums16(const 
     }
 }
 
-// C[chunk][digit] (chunk sums) -> first output position of (chunk, digit): exclusive scan over the digits of the totals + exclusive
-// scan over the chunks, in place; ctl_counts[digit] = total of the digit. One CTA, one thread per digit, every load independent.
-static __global__ void __launch_bounds__(OSW_DIGITS) k_wide_chunk_scan(uint32_t *__restrict__ C, uint32_t chunks, uint32_t *__restrict__ ctl_counts)
+// The first output position of every (wide tile, digit), in one launch, from the 16-bit rows the tile pass filed. CTA c adds the rows
+// of chunk c and files, for every tile of the chunk, the sum of the chunk's earlier rows (T[tile][digit], 32-bit). The last CTA to
+// finish turns the chunk sums C[chunk][digit] into the first output position of every (chunk, digit) -- exclusive scan over the digits
+// of the totals + exclusive scan over the chunks, in place -- and sets ctl_counts[digit] = total of the digit. A tile's first output
+// position of digit d is then C[chunk][d] + T[tile][d]: two rows per scatter CTA, whatever the tile's place in its chunk.
+// `done` (one word, zero between launches: the last CTA clears it) counts the finished chunks. T = nullptr: only the chunk rows
+// (k_wide_scatter, which adds the earlier rows of its chunk itself).
+static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const uint16_t *__restrict__ H, uint32_t tiles, uint32_t chunk_shift, uint32_t chunks,
+                                                                        uint32_t *__restrict__ C, uint32_t *__restrict__ T, uint32_t *__restrict__ ctl_counts,
+                                                                        uint32_t *__restrict__ done)
 {
-    __shared__ uint32_t wsum[32];
-    const uint32_t d = threadIdx.x, lane = d & 31, warp = d >> 5;
-    uint32_t total = 0;
-#pragma unroll 16
-    for (uint32_t c = 0; c < chunks; c++) total += C[static_cast<size_t>(c) * OSW_DIGITS + d];
-    ctl_counts[d] = total;
-    uint32_t incl = total;
+    static_assert(OSW_THREADS * 4 == OSW_DIGITS, "four digits per thread");
+    constexpr uint32_t NW = OSW_THREADS / 32;
+    __shared__ uint32_t wsum[NW];
+    __shared__ uint32_t s_last;
+    const uint32_t chunk = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t t0 = chunk << chunk_shift, t1 = min(tiles, t0 + (1u << chunk_shift));
+    uint4 acc = make_uint4(0, 0, 0, 0);
+    const ushort4 *row = reinterpret_cast<const ushort4 *>(H) + tid;
+    uint4 *trow = reinterpret_cast<uint4 *>(T) + tid;
+#pragma unroll 8
+    for (uint32_t t = t0; t < t1; t++) {
+        const ushort4 v = row[static_cast<size_t>(t) * (OSW_DIGITS / 4)];
+        if (T != nullptr) trow[static_cast<size_t>(t) * (OSW_DIGITS / 4)] = acc;
+        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+    uint4 *C4 = reinterpret_cast<uint4 *>(C);
+    C4[static_cast<size_t>(chunk) * (OSW_DIGITS / 4) + tid] = acc;
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(done, 1u) == chunks - 1u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    uint4 tot = make_uint4(0, 0, 0, 0);
+#pragma unroll 8
+    for (uint32_t c = 0; c < chunks; c++) { const uint4 v = __ldcg(C4 + static_cast<size_t>(c) * (OSW_DIGITS / 4) + tid); tot.x += v.x; tot.y += v.y; tot.z += v.z; tot.w += v.w; }
+    reinterpret_cast<uint4 *>(ctl_counts)[tid] = tot;
+    const uint32_t sum = tot.x + tot.y + tot.z + tot.w;
+    uint32_t incl = sum;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if (lane >= static_cast<uint32_t>(o)) incl += v; }
     if (lane == 31) wsum[warp] = incl;
     __syncthreads();
-    if (warp == 0) {
-        const uint32_t w = wsum[lane];
-        uint32_t wi = w;
+    uint32_t base = incl - sum;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, wi, o); if (lane >= static_cast<uint32_t>(o)) wi += v; }
-        wsum[lane] = wi - w;
+    for (uint32_t q = 0; q < NW; q++) if (q < warp) base += wsum[q];
+    uint4 run = make_uint4(base, base + tot.x, base + tot.x + tot.y, base + tot.x + tot.y + tot.z);
+#pragma unroll 8
+    for (uint32_t c = 0; c < chunks; c++) {
+        uint4 *p = C4 + static_cast<size_t>(c) * (OSW_DIGITS / 4) + tid;
+        const uint4 v = __ldcg(p);
+        *p = run;
+        run.x += v.x; run.y += v.y; run.z += v.z; run.w += v.w;
     }
-    __syncthreads();
-    uint32_t run = wsum[warp] + incl - total;
-#pragma unroll 16
-    for (uint32_t c = 0; c < chunks; c++) { uint32_t *p = C + static_cast<size_t>(c) * OSW_DIGITS + d; const uint32_t v = *p; *p = run; run += v; }
+    if (tid == 0) *done = 0;
 }
 
 // The scatter of the wide partition when the tile pass packed a rank with every slot (TileArgs::pack_rank): word = slot | rank << 16,
 // rank = any numbering 0 .. count-1 of the survivors of one (wide tile, digit) cell. One CTA per wide tile, everything on chip:
-//   1. first output position of every digit for this tile (chunk row of k_wide_chunk_scan + the rows of the earlier tiles of the chunk)
+//   1. the tile's words to shared memory; first output position of every digit for this tile (C[chunk] + T[tile] of k_wide_tile_bases)
 //      and the tile's own cells laid out back to back in shared memory (exclusive scan of the tile's digit counts),
 //   2. every item files its position within the tile at cell start + rank -- no ranking rounds, no per-warp counters,
-//   3. ARRIVAL order inside a cell (the count windows need every key's items in stream order, and two items of one key may share a
-//      cell): an item's place = number of the cell's entries with a smaller position; a cell holds a few entries, read from shared memory,
-//   4. one write of (slot, position) per item to its final place.
+//   3. a sweep over the laid-out cells, consecutive threads on consecutive entries of a cell: ARRIVAL order inside the cell (the count
+//      windows need every key's items in stream order, and two items of one key may share a cell) -- an entry's place is the number of
+//      the cell's entries with a smaller position -- and one write of (slot, position) to the final place. The stores of a warp land in
+//      the few cells it sweeps, and no per-thread array outlives a loop (nothing is indexed at run time: no local memory).
 // Output: keys_out[i] = slot, vals_out[i] = arrival position, stable by (digit, position) -- what k_wide_scatter produces.
-// RBYTES != 0: the records travel (payload_in at the arrival positions -> payload_out at the final places; keys_out gets the slots,
-// vals_out is not written): the source side of the bucketed multi-GPU exchange.
+// RBYTES != 0: the records travel as well (payload_in at the arrival positions -> payload_out at the final places; vals_out may be
+// null): the source side of the bucketed multi-GPU exchange, and WFB_BUCKET_MOVE=1, whose update reads the arrival position of a
+// group's triggering item from vals_out.
+// 34 KB of shared memory and at most 40 registers: 6 resident CTAs per SM, so the 2048 wide tiles of the bench step take 2.6 waves
+// on 132 SMs.
 #ifndef WFB_OSR_MINBLOCKS
-#define WFB_OSR_MINBLOCKS 1   // (resident CTAs per SM the pair version is compiled for: 2048 tiles of the bench step are 2 full waves at 7)
+#define WFB_OSR_MINBLOCKS 6
 #endif
 template <int RBYTES>
-static __global__ void __launch_bounds__(OSW_THREADS, RBYTES == 0 ? WFB_OSR_MINBLOCKS : 1) k_wide_scatter_ranked(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
+static __global__ void __launch_bounds__(OSW_THREADS, WFB_OSR_MINBLOCKS) k_wide_scatter_ranked(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
                                                                             uint32_t *__restrict__ vals_out, uint32_t n, uint32_t shift, uint32_t chunk_shift,
-                                                                            const uint16_t *__restrict__ H, const uint32_t *__restrict__ Cx,
+                                                                            const uint16_t *__restrict__ H, const uint32_t *__restrict__ Cx, const uint32_t *__restrict__ T,
                                                                             const unsigned char *__restrict__ payload_in, unsigned char *__restrict__ payload_out)
 {
     constexpr uint32_t NW = OSW_THREADS / 32;
+    constexpr uint32_t LPOS = OSW_TILE + OSW_DIGITS;  // every cell padded to an even number of entries (4-byte loads in the repair loop)
+    constexpr uint32_t LPAD = 0x0fffu;                // padding entry: never below a position of the tile (positions are < 4096)
+    static_assert(OSW_TILE <= 4096 && LPOS % (2 * OSW_THREADS) == 0, "16-bit packed position compare");
+    __shared__ __align__(16) uint32_t sw[OSW_TILE];   // the tile's words, arrival order
     __shared__ __align__(16) uint32_t bin_base[OSW_DIGITS];
     __shared__ __align__(8) uint16_t cnt_row[OSW_DIGITS], cell_start[OSW_DIGITS];
-    constexpr uint32_t LPOS = OSW_TILE + 3u * OSW_DIGITS;  // every cell padded to a multiple of four entries (8-byte loads in the repair loop)
-    constexpr uint32_t LPAD = 0x0fffu;                     // padding entry: never below a position of the tile (positions are < 4096)
-    static_assert(OSW_TILE <= 4096 && LPOS % (2 * OSW_THREADS) == 0, "16-bit packed position compare");
-    __shared__ __align__(8) uint16_t lpos[LPOS];
+    __shared__ __align__(4) uint16_t lpos[LPOS];
     __shared__ uint32_t wsum[NW];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, tile = blockIdx.x;
     const uint32_t start = tile * OSW_TILE;
     if (start >= n) return;
-    uint32_t w[OSW_ITEMS];
 #pragma unroll
-    for (uint32_t r = 0; r < OSW_ITEMS; r++) { const uint32_t idx = start + r * OSW_THREADS + tid; w[r] = idx < n ? packed[idx] : INVALID_SLOT; }
-    if constexpr (RBYTES != 0) { // the records this CTA will move: on their way to L2 while the offsets are worked out below
-#pragma unroll
-        for (uint32_t r = 0; r < OSW_ITEMS; r++)
-            if (w[r] != INVALID_SLOT) asm volatile("prefetch.global.L2 [%0];" ::"l"(payload_in + static_cast<size_t>(start + r * OSW_THREADS + tid) * RBYTES));
+    for (uint32_t r = 0; r < OSW_ITEMS; r++) {
+        const uint32_t i = r * OSW_THREADS + tid, idx = start + i;
+        const uint32_t w = idx < n ? packed[idx] : INVALID_SLOT;
+        sw[i] = w;
+        if constexpr (RBYTES != 0) // the records this CTA will move: on their way to L2 while the offsets are worked out below
+            if (w != INVALID_SLOT) asm volatile("prefetch.global.L2 [%0];" ::"l"(payload_in + static_cast<size_t>(idx) * RBYTES));
     }
     {
-        const uint32_t chunk = tile >> chunk_shift;
-        uint4 acc = reinterpret_cast<const uint4 *>(Cx)[static_cast<size_t>(chunk) * (OSW_DIGITS / 4) + tid];
-        const ushort4 *hrow = reinterpret_cast<const ushort4 *>(H) + tid;
-#pragma unroll 16
-        for (uint32_t t = chunk << chunk_shift; t < tile; t++) { const ushort4 v = hrow[static_cast<size_t>(t) * (OSW_DIGITS / 4)]; acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w; }
-        reinterpret_cast<uint4 *>(bin_base)[tid] = acc;
-        const ushort4 c = hrow[static_cast<size_t>(tile) * (OSW_DIGITS / 4)];
+        const uint4 cb = reinterpret_cast<const uint4 *>(Cx)[static_cast<size_t>(tile >> chunk_shift) * (OSW_DIGITS / 4) + tid];
+        const uint4 tb = reinterpret_cast<const uint4 *>(T)[static_cast<size_t>(tile) * (OSW_DIGITS / 4) + tid];
+        reinterpret_cast<uint4 *>(bin_base)[tid] = make_uint4(cb.x + tb.x, cb.y + tb.y, cb.z + tb.z, cb.w + tb.w);
+        const ushort4 c = reinterpret_cast<const ushort4 *>(H)[static_cast<size_t>(tile) * (OSW_DIGITS / 4) + tid];
         reinterpret_cast<ushort4 *>(cnt_row)[tid] = c;
         // the tile's cells back to back: exclusive scan of its 1024 digit counts (thread tid owns digits 4 tid .. 4 tid + 3)
-        const uint32_t p0 = (c.x + 3u) & ~3u, p1 = (c.y + 3u) & ~3u, p2 = (c.z + 3u) & ~3u, p3 = (c.w + 3u) & ~3u; // padded cell sizes
+        const uint32_t p0 = (c.x + 1u) & ~1u, p1 = (c.y + 1u) & ~1u, p2 = (c.z + 1u) & ~1u, p3 = (c.w + 1u) & ~1u; // padded cell sizes
         const uint32_t sum = p0 + p1 + p2 + p3;
         uint32_t incl = sum;
 #pragma unroll
@@ -1138,37 +1170,36 @@ static __global__ void __launch_bounds__(OSW_THREADS, RBYTES == 0 ? WFB_OSR_MINB
     __syncthreads();
 #pragma unroll
     for (uint32_t r = 0; r < OSW_ITEMS; r++) {
-        if (w[r] != INVALID_SLOT) {
-            const uint32_t d = ((w[r] & 0xffffu) >> shift) & (OSW_DIGITS - 1u);
-            lpos[cell_start[d] + (w[r] >> 16)] = static_cast<uint16_t>(r * OSW_THREADS + tid);
-        }
+        const uint32_t i = r * OSW_THREADS + tid, w = sw[i];
+        if (w != INVALID_SLOT) lpos[cell_start[((w & 0xffffu) >> shift) & (OSW_DIGITS - 1u)] + (w >> 16)] = static_cast<uint16_t>(i);
     }
     __syncthreads();
-#pragma unroll 4
-    for (uint32_t r = 0; r < OSW_ITEMS; r++) {
-        if (w[r] != INVALID_SLOT) {
-            const uint32_t slot = w[r] & 0xffffu, d = (slot >> shift) & (OSW_DIGITS - 1u);
-            const uint32_t cnt = cnt_row[d], cs = cell_start[d], mine = r * OSW_THREADS + tid;
-            // entries of the cell below `mine`, four per load: per 16-bit half, bit 15 of (0x8000 + mine - 1 - entry) says entry < mine
-            // (all values are < 4096, so the halves never borrow from each other; padding entries are never below)
-            const uint32_t mm = (mine | (mine << 16)) + 0x7fff7fffu;
-            const uint2 *cell = reinterpret_cast<const uint2 *>(lpos + cs);
-            uint32_t less = 0;
-            for (uint32_t e = 0; e < cnt; e += 4) { const uint2 v = cell[e >> 2]; less += __popc((mm - v.x) & 0x80008000u) + __popc((mm - v.y) & 0x80008000u); }
-            const uint32_t dst = bin_base[d] + less;
-            keys_out[dst] = slot;
-            if constexpr (RBYTES == 0) vals_out[dst] = start + mine;
-            else {
-                static_assert(RBYTES % 8 == 0, "record size");
-                using W = typename std::conditional<RBYTES % 16 == 0, uint4, uint2>::type;
-                const W *src = reinterpret_cast<const W *>(payload_in + static_cast<size_t>(start + mine) * RBYTES);
-                W *dstp = reinterpret_cast<W *>(payload_out + static_cast<size_t>(dst) * RBYTES);
-                W v[RBYTES / sizeof(W)];
+#pragma unroll 2
+    for (uint32_t e = tid; e < LPOS; e += OSW_THREADS) {
+        const uint32_t mine = lpos[e], w = sw[mine];
+        if (w == INVALID_SLOT) continue;
+        const uint32_t slot = w & 0xffffu, d = (slot >> shift) & (OSW_DIGITS - 1u);
+        const uint32_t cs = cell_start[d], cnt = cnt_row[d];
+        if (e - cs >= cnt) continue; // padding (it reads as position 4095, which lives in another cell or not at all)
+        // entries of the cell below `mine`, two per load: per 16-bit half, bit 15 of (0x8000 + mine - 1 - entry) says entry < mine
+        // (all values are < 4096, so the halves never borrow from each other; padding entries are never below)
+        const uint32_t mm = (mine | (mine << 16)) + 0x7fff7fffu;
+        const uint32_t *cell = reinterpret_cast<const uint32_t *>(lpos + cs);
+        uint32_t less = 0;
+        for (uint32_t j = 0; j < cnt; j += 2) less += __popc((mm - cell[j >> 1]) & 0x80008000u);
+        const uint32_t dst = bin_base[d] + less;
+        keys_out[dst] = slot;
+        if (RBYTES == 0 || vals_out != nullptr) vals_out[dst] = start + mine;
+        if constexpr (RBYTES != 0) {
+            static_assert(RBYTES % 8 == 0, "record size");
+            using W = typename std::conditional<RBYTES % 16 == 0, uint4, uint2>::type;
+            const W *src = reinterpret_cast<const W *>(payload_in + static_cast<size_t>(start + mine) * RBYTES);
+            W *dstp = reinterpret_cast<W *>(payload_out + static_cast<size_t>(dst) * RBYTES);
+            W v[RBYTES / sizeof(W)];
 #pragma unroll
-                for (uint32_t q = 0; q < RBYTES / sizeof(W); q++) v[q] = src[q];
+            for (uint32_t q = 0; q < RBYTES / sizeof(W); q++) v[q] = src[q];
 #pragma unroll
-                for (uint32_t q = 0; q < RBYTES / sizeof(W); q++) dstp[q] = v[q];
-            }
+            for (uint32_t q = 0; q < RBYTES / sizeof(W); q++) dstp[q] = v[q];
         }
     }
 }
@@ -1298,7 +1329,7 @@ __global__ void __launch_bounds__(OSW_THREADS, WFB_OSW_MINBLOCKS) k_wide_scatter
                                                               uint32_t payload_bytes, uint32_t skip_invalid, uint32_t region_stride,
                                                               const uint32_t *__restrict__ H32, uint32_t cx)
 {
-    // cx != 0: C holds the first output position of every (chunk, digit) already (k_wide_chunk_scan); ctl_counts is not read
+    // cx != 0: C holds the first output position of every (chunk, digit) already (k_wide_tile_bases); ctl_counts is not read
     // H32 != nullptr: the per-tile counts are 32-bit rows filled by the producer of the keys (the tile pass) instead of H
     // region_stride != 0: bin d starts at d * region_stride (fixed-capacity regions; elements beyond the capacity are dropped)
     constexpr uint32_t NW = OSW_THREADS / 32;

@@ -147,7 +147,7 @@ struct RadixSorter {
         }
         return 0;
     }
-    void destroy() { cudaFree(ctl); cudaFree(state); cudaFree(wideH); cudaFree(wideC); cudaFree(wideH32); }
+    void destroy() { cudaFree(ctl); cudaFree(state); cudaFree(wideH); cudaFree(wideC); cudaFree(wideT); cudaFree(wideDone); cudaFree(wideH32); }
 
     // stable sort of (kA[i], i) by the low 8*passes bits; n on the device (n_ptr) or the host (n_host), cap = upper bound
     template <class K, int ITEMS>
@@ -177,6 +177,8 @@ struct RadixSorter {
     // ONE stable partition pass of (kin[i], i) on the digit (key >> shift) & 1023 into (kout, vout): per-tile counts, then
     // the scatter (no chained scan). *counts = the 1024 digit counts (ready_ctl if the producer of the keys made them).
     uint16_t *wideH = nullptr; uint32_t *wideC = nullptr; uint32_t wide_tiles = 0, wide_chunks = 0;
+    uint32_t *wideT = nullptr;    // [tiles][1024]: sum of the earlier rows of the tile's chunk (k_wide_tile_bases)
+    uint32_t *wideDone = nullptr; // finished chunks of k_wide_tile_bases (zero between launches)
     uint32_t *wideH32 = nullptr; uint32_t wide32_tiles = 0; // per-tile counts filled by the producer of the keys (32-bit rows)
     // rows for `cap` positions, zeroed on stream s: the producer adds its digit counts, sort_wide(..., h32_ready) consumes them
     int prepare_h32(uint32_t cap, cudaStream_t s, uint32_t **rows)
@@ -193,28 +195,42 @@ struct RadixSorter {
         return 0;
     }
     // tiles of the wide pass over `cap` positions and their chunks. prefix = false: about sqrt(tiles) chunks of >= 16 tiles, every
-    // scatter CTA sums the rows of the earlier chunks itself; true (rows filed by the tile pass): chunks of 32 tiles whose first
-    // output positions one small kernel computes (k_wide_chunk_scan), so a scatter CTA reads one chunk row and < 32 tile rows
+    // scatter CTA sums the rows of the earlier chunks itself; true (rows filed by the tile pass): chunks of 32 tiles; one kernel
+    // (k_wide_tile_bases) computes the first output positions of every chunk and the in-chunk offsets of every tile, so a scatter
+    // CTA reads two rows
     static void wide_geometry(uint32_t cap, bool prefix, uint32_t *tiles, uint32_t *chunk_shift, uint32_t *chunks)
     {
         *tiles = std::max(1u, (cap + OSW_TILE - 1) / OSW_TILE);
-        uint32_t cs = prefix ? 5 : 4; // (prefix: 32 tiles per chunk -- the one-CTA scan over the chunks stays short, a scatter CTA adds < 32 rows)
+        uint32_t cs = prefix ? 5 : 4; // (prefix: 32 tiles per chunk -- the scan over the chunks, done by one CTA, stays short)
         if (!prefix) while ((1u << (2 * cs)) < *tiles) cs++;
         *chunk_shift = cs;
         *chunks = (*tiles + (1u << cs) - 1) >> cs;
+    }
+    // grows the rows and chunk rows of the wide pass; the chunk rows alone when only they are short, so that rows a producer has
+    // already filed (ensure_wide, whose chunks of 32 tiles may be fewer than sort_wide's without a prefix) survive
+    int ensure_wide_buffers(uint32_t tiles, uint32_t chunks, cudaStream_t s)
+    {
+        if (tiles <= wide_tiles && chunks <= wide_chunks) return 0;
+        CK(cudaStreamSynchronize(s));
+        if (tiles > wide_tiles) {
+            cudaFree(wideH); cudaFree(wideT);
+            wide_tiles = tiles;
+            CK(cudaMalloc(&wideH, sizeof(uint16_t) * OSW_DIGITS * wide_tiles));
+            CK(cudaMalloc(&wideT, sizeof(uint32_t) * OSW_DIGITS * wide_tiles));
+        }
+        if (chunks > wide_chunks) {
+            cudaFree(wideC);
+            wide_chunks = chunks;
+            CK(cudaMalloc(&wideC, sizeof(uint32_t) * OSW_DIGITS * wide_chunks));
+        }
+        return 0;
     }
     // rows of the wide partition for `cap` positions, allocated before the producer of the keys files them (TileArgs::wide_h16)
     int ensure_wide(uint32_t cap, cudaStream_t s, uint16_t **rows)
     {
         uint32_t tiles, chunk_shift, chunks;
         wide_geometry(cap, true, &tiles, &chunk_shift, &chunks);
-        if (tiles > wide_tiles || chunks > wide_chunks) {
-            CK(cudaStreamSynchronize(s));
-            cudaFree(wideH); cudaFree(wideC);
-            wide_tiles = std::max(tiles, wide_tiles); wide_chunks = std::max(chunks, wide_chunks);
-            CK(cudaMalloc(&wideH, sizeof(uint16_t) * OSW_DIGITS * wide_tiles));
-            CK(cudaMalloc(&wideC, sizeof(uint32_t) * OSW_DIGITS * wide_chunks));
-        }
+        { int rc = ensure_wide_buffers(tiles, chunks, s); if (rc) return rc; }
         *rows = wideH;
         return 0;
     }
@@ -242,22 +258,15 @@ struct RadixSorter {
         rows_override = prefix ? h16_rows : nullptr;
         uint32_t tiles, chunk_shift, chunks;
         wide_geometry(cap, prefix, &tiles, &chunk_shift, &chunks);
-        if (tiles > wide_tiles || chunks > wide_chunks) {
-            CK(cudaStreamSynchronize(s));
-            cudaFree(wideH); cudaFree(wideC);
-            wide_tiles = std::max(tiles, wide_tiles); wide_chunks = std::max(chunks, wide_chunks);
-            CK(cudaMalloc(&wideH, sizeof(uint16_t) * OSW_DIGITS * wide_tiles));
-            CK(cudaMalloc(&wideC, sizeof(uint32_t) * OSW_DIGITS * wide_chunks));
-        }
+        { int rc = ensure_wide_buffers(tiles, chunks, s); if (rc) return rc; }
         uint32_t *c = ready_ctl ? ready_ctl : ctl;
         if (!ready_ctl) { int rc = prepare_wide(c, s); if (rc) return rc; }
         const uint32_t *h32 = nullptr;
         if (h16_ready && ready_ctl && few_bins) { // a few bins (destinations), rows filed by the tile pass: chunk sums + the global counts (c was cleared by the caller)
             k_wide_chunk_sums16<<<chunks, OSW_THREADS, 0, s>>>(h16_rows ? h16_rows : wideH, tiles, chunk_shift, wideC, c);
-        } else if (prefix) { // the tile pass filed the 16-bit rows (wideH): chunk sums, then first output position of every (chunk, digit) + digit counts
-            k_wide_chunk_sums16<<<chunks, OSW_THREADS, 0, s>>>(h16_rows ? h16_rows : wideH, tiles, chunk_shift, wideC);
-            k_wide_chunk_scan<<<1, OSW_DIGITS, 0, s>>>(wideC, chunks, c);
-            launches++;
+        } else if (prefix) { // the tile pass filed the 16-bit rows (wideH): first output position of every (chunk, digit) and (tile, digit) + digit counts
+            if (!wideDone) { CK(cudaMalloc(&wideDone, sizeof(uint32_t))); CK(cudaMemsetAsync(wideDone, 0, sizeof(uint32_t), s)); }
+            k_wide_tile_bases<<<chunks, OSW_THREADS, 0, s>>>(h16_rows ? h16_rows : wideH, tiles, chunk_shift, chunks, wideC, ranked ? wideT : nullptr, c, wideDone);
         } else if (h32_ready && ready_ctl && !few_bins) { // the producer of the keys counted the digits per tile: only the chunk sums are missing
             k_wide_chunk_sums<<<chunks, OSW_THREADS, 0, s>>>(wideH32, tiles, chunk_shift, wideC);
             h32 = wideH32;
@@ -284,15 +293,15 @@ struct RadixSorter {
         }
         if (prefix && ranked && sizeof(K) == 4 && !payload_in && keys_out_ok(kout, vout)) {
             k_wide_scatter_ranked<0><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, chunk_shift,
-                                                                   h16_rows ? h16_rows : wideH, wideC, nullptr, nullptr);
+                                                                   h16_rows ? h16_rows : wideH, wideC, wideT, nullptr, nullptr);
             CK(cudaGetLastError());
             launches += 2;
             *counts = c;
             return 0;
         }
         if (prefix && ranked && sizeof(K) == 4 && payload_in && payload_out && kout && !region_stride) { // the records travel with their slots (bucketed exchange)
-#define WFB_WSR(RB_) k_wide_scatter_ranked<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), nullptr, n_host, shift, \
-                                                                             chunk_shift, h16_rows ? h16_rows : wideH, wideC, payload_in, payload_out)
+#define WFB_WSR(RB_) k_wide_scatter_ranked<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, \
+                                                                             chunk_shift, h16_rows ? h16_rows : wideH, wideC, wideT, payload_in, payload_out)
             switch (payload_bytes) {
                 case 16: WFB_WSR(16); break; case 24: WFB_WSR(24); break; case 32: WFB_WSR(32); break; case 48: WFB_WSR(48); break; case 64: WFB_WSR(64); break;
                 default: return WFB_E_UNSUPPORTED;
