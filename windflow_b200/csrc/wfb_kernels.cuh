@@ -1691,44 +1691,59 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
 // ------------------------------------------------------------------------------------------------------
 // k_ffat_update_buckets: the window update after ONE wide partition pass (k_wide_scatter) on the top 10 bits of the
 // slot. The pass leaves the segment's (slot, arrival position) pairs in 1024 buckets of at most BK_KEYS consecutive
-// slots, arrival order inside a bucket. One CTA per bucket, in chunks of at most BK_CAP items (arrival order is chunk
-// order). Every phase is built to need as few dependent memory round trips as possible -- the kernel is bound by
-// latency, not by bytes:
-//   1. every thread takes BK_IT consecutive items of the chunk; stable split by key through per-thread private key
-//      counts in shared memory (count, exclusive scan over the threads, place) -> per-key runs of record indices,
-//   2. the FlatFAT siblings of the leaf each key completes first in this chunk are copied to shared memory with cp.async
-//      while
-//   3. ONE THREAD per segment (the items of a run that fall into one pane) folds its items in arrival order straight
-//      from the lifted array, eight masked loads per round trip; then one thread per key walks its segments in order:
+// slots, arrival order inside a bucket. One CTA per bucket. The kernel's time is the random gather of the records and the
+// dependent round trips in front of it, so every phase issues all of its global loads before it uses the first one:
+//   0. the bucket's range (scan of the pass histogram), the keys' state, and the items of every key in the whole bucket
+//      (BK_CNT_U independent loads of the bucket list per thread and round trip): the deferral of fired groups needs them,
+// then per chunk of at most CAP items (arrival order is chunk order; CAP is sized so that the chunk's records take
+// BK_REC_BYTES of shared memory). The chunk's part of the bucket list is already in shared memory: it was copied with
+// cp.async while the previous chunk ran.
+//   1. stable split by key: item r * BK_THREADS + t is thread t's r-th; a warp ranks its items of a key with match_any and
+//      files their count per (round, warp) column; scans over the columns and over the keys give every item its place in
+//      the key-major order,
+//   2. every thread copies its items' records global -> shared in that order with cp.async (all of them in flight at once;
+//      16-byte copies bypass L1, where a copy in flight would hold a line); eager FlatFAT levels also stage the siblings of
+//      the first leaf each key completes,
+//   3. ONE THREAD per segment (the items of a run that fall into one pane) folds them in arrival order from shared memory
+//      and leaves the result in place of the segment's first record; then one thread per key walks its segments in order:
 //      completed panes become FlatFAT leaves, their root paths are recomputed (staged siblings for the first) and fired
 //      groups go to the deferred window list; the last partial segment is the new open pane,
 //   4. a chunk with more segments than threads (tiny panes) is folded one warp per key instead (ordered shuffle-tree
-//      fold, 32 records per load).
+//      fold of 32 staged records at a time).
 // Per-key bookkeeping (count, position in the open pane, next leaf, next trigger, open-pane accumulator) is computed
 // once per CTA by one thread per key and lives in shared memory across the chunks.
 // `moved` = 1: the partition pass also moved the records (bucket b's records are lifted[boff[b] ..)); 0: records are
 // gathered through the arrival positions.
 // ------------------------------------------------------------------------------------------------------
 #ifdef WFB_BK_TRACE
+// debug build only, per CTA: start time, time thread 0 spent in phases 1..6 (summed over the chunks), end time (globaltimer ns)
 __device__ unsigned long long g_bk_trace[1024 * 8];
-#define BK_MARK(i) do { if (threadIdx.x == 0) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); g_bk_trace[blockIdx.x * 8 + (i)] = t_; } } while (0)
+__device__ __forceinline__ unsigned long long bk_now() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+#define BK_TRACE_STATE unsigned long long bk_t = 0
+#define BK_MARK(i) do { if (threadIdx.x == 0) { const unsigned long long t_ = bk_now(); unsigned long long *r_ = g_bk_trace + blockIdx.x * 8; \
+    if ((i) == 0) { r_[0] = t_; for (int q_ = 1; q_ < 8; q_++) r_[q_] = 0; } else if ((i) == 7) r_[7] = t_; else r_[i] += t_ - bk_t; bk_t = t_; } } while (0)
 #else
+#define BK_TRACE_STATE do { } while (0)
 #define BK_MARK(i) do { } while (0)
 #endif
 constexpr uint32_t BK_KEYS = 64;      // keys per bucket (at most)
 constexpr uint32_t BK_THREADS = 128;
-constexpr uint32_t BK_IT = 18;        // consecutive items per thread and chunk
-constexpr uint32_t BK_CAP = BK_THREADS * BK_IT; // items per chunk
-#ifndef WFB_BK_U
-#define WFB_BK_U 4
+#ifndef WFB_BK_REC_BYTES
+#define WFB_BK_REC_BYTES 16384
 #endif
+constexpr uint32_t BK_REC_BYTES = WFB_BK_REC_BYTES; // shared memory for a chunk's records
+constexpr uint32_t BK_CNT_U = 16;     // bucket-list loads in flight per thread (key counts)
+// a copy of v the compiler cannot see through: keeps it from computing a shared-memory address from v before the chunk loop
+// and holding it (in local memory, under the launch bound) until the write-back
+__device__ __forceinline__ uint32_t bk_opaque(uint32_t v) { asm volatile("" : "+r"(v)); return v; }
+template <uint32_t RB>                // items per thread and chunk: BK_REC_BYTES of records, 1..8
+constexpr uint32_t bk_items_per_thread() { return BK_REC_BYTES / (BK_THREADS * RB) < 1 ? 1 : (BK_REC_BYTES / (BK_THREADS * RB) > 8 ? 8 : BK_REC_BYTES / (BK_THREADS * RB)); }
 #ifndef WFB_BK_MINBLOCKS
-#define WFB_BK_MINBLOCKS 4
+#define WFB_BK_MINBLOCKS 4        // eager FlatFAT levels (16 KB of staged siblings on top of the lazy footprint)
 #endif
 #ifndef WFB_BK_MINBLOCKS_LAZY
-#define WFB_BK_MINBLOCKS_LAZY 4   // lazy FlatFAT levels: no sibling staging (32 KB of shared memory instead of 48), no path code.
-#endif                            // (5 caps sm_90a at 96 registers, 272 B of spills; 4: 128, 132 B. Update 236 -> 193 us per bench step, H100 SXM 700 W)
-constexpr uint32_t BK_U = WFB_BK_U;   // record loads in flight per thread
+#define WFB_BK_MINBLOCKS_LAZY 4   // lazy FlatFAT levels. Update + queries per bench step at 4 CTAs per SM: 153 us; at 6: 167 us; at 7:
+#endif                            // 168 us (H100 SXM, 700 W): more resident CTAs only queue more gathers behind each other
 
 template <class P, bool LAZY>
 __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB_BK_MINBLOCKS) k_ffat_update_buckets(const FfatDev ff, const unsigned char *__restrict__ lifted,
@@ -1743,14 +1758,17 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
     constexpr uint32_t RB = sizeof(R);
     constexpr uint32_t NW = BK_THREADS / 32;
     constexpr uint32_t DPT = OSW_DIGITS / BK_THREADS;                  // digit counts per thread
-    constexpr uint32_t HS = BK_THREADS + 2;                            // row stride of the private counts (bank-conflict padding)
+    constexpr uint32_t IT = bk_items_per_thread<RB>();                 // items per thread and chunk
+    constexpr uint32_t CAP = BK_THREADS * IT;                          // items per chunk
+    constexpr uint32_t NCOL = IT * NW;                                 // (round, warp) columns of the split counts
+    constexpr uint32_t CS = NCOL + 2;                                  // row stride of the split counts (odd in words: no bank conflicts)
     constexpr uint32_t CPB = (RB % 16 == 0) ? 16 : 8;                  // cp.async granule of a record
-    constexpr uint32_t BK_SIBL = RB <= 32 ? 8 : (RB <= 48 ? 4 : (RB <= 128 ? 2 : 1)); // FlatFAT levels whose siblings are staged in shared memory (static shared memory <= 48 KB)
+    constexpr uint32_t BK_SIBL = RB <= 32 ? 8 : (RB <= 48 ? 4 : (RB <= 128 ? 2 : 1)); // FlatFAT levels whose siblings are staged in shared memory
     static_assert(DPT % 4 == 0 && BK_KEYS == 64 && BK_THREADS == 128 && RB % 8 == 0, "layout");
-    __shared__ uint32_t s_idx[BK_CAP];                 // record index of the items (into `lifted`), key-major
-    __shared__ __align__(16) uint16_t hist[BK_KEYS][HS]; // items of key k among thread t's items -> exclusive over the threads;
-                                                       // after the split: segment descriptors and segment results (fold phase)
-    __shared__ uint32_t htot[2][BK_KEYS];              // per key: items held by threads 0..63 / 64..127
+    __shared__ __align__(16) unsigned char s_rec[CAP * RB]; // the chunk's records, key-major; a segment's fold replaces its first record
+    __shared__ uint32_t s_idx[CAP];                    // record index of the items (into `lifted`), key-major
+    __shared__ uint32_t s_lslot[CAP], s_lpos[CAP];     // the bucket list of the next chunk (slots, arrival positions), prefetched
+    __shared__ __align__(16) uint16_t s_col[BK_KEYS][CS]; // items of key k in (round, warp) column c -> exclusive over the columns
     __shared__ uint32_t kcnt[BK_KEYS], koff[BK_KEYS];  // items / first index of key k in this chunk
     __shared__ uint32_t kleft[BK_KEYS];                // items of key k still to come in this segment
     __shared__ uint32_t kcp[BK_KEYS], kleaf[BK_KEYS];  // items in the open pane, leaf the open pane will be written to
@@ -1759,10 +1777,8 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
     __shared__ __align__(16) unsigned char s_sib[LAZY ? 16 : BK_KEYS * BK_SIBL * RB]; // siblings of the leaf key k completes in this chunk (lazy levels: none)
     __shared__ uint32_t s_heavy[BK_KEYS];              // keys folded by a warp in this chunk
     __shared__ uint32_t ksegb[BK_KEYS];                // first segment of key k (a segment = the items of a run that fall into one pane)
-    __shared__ uint32_t misc[NW], s_boff[2], s_nheavy, s_nseg;
-    constexpr bool SEG_OK = BK_THREADS * (RB + 4) <= sizeof(uint16_t) * BK_KEYS * HS; // segment results + descriptors alias the private counts
-    unsigned char *seg_res = reinterpret_cast<unsigned char *>(&hist[0][0]);                       // BK_THREADS x result_t
-    uint32_t *seg_desc = reinterpret_cast<uint32_t *>(seg_res + BK_THREADS * RB);                  // key | index of the segment in its run << 8
+    __shared__ uint32_t seg_desc[BK_THREADS];          // key | index of the segment in its run << 8
+    __shared__ uint32_t misc[NW], s_boff[2], s_nheavy, s_hnext, s_nseg;
 
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t bucket = blockIdx.x;
@@ -1772,17 +1788,18 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
     const uint32_t P32 = static_cast<uint32_t>(ff.pane);
     const uint64_t group_items = ff.slide * ff.nb;
     const size_t tree_stride = static_cast<size_t>(2 * n - 1) * RB;
+    BK_TRACE_STATE;
 
     BK_MARK(0);
-    // ---- per-key bookkeeping, one thread per key (loads first: they overlap the histogram scan below) ----------------------
+    // ---- 0. per-key bookkeeping, one thread per key (loads first: they overlap the histogram scan below) -----------------------
     uint32_t my_total = 0;
     uint64_t st_c = 0;
-    alignas(16) R st_acc;
     const bool has_key = tid < kpc && key_lo + tid < ff.max_keys;
-    if (has_key) {
+    if (has_key) { // the open-pane accumulator goes straight to shared memory (it has landed by the first fold's barrier)
         const uint32_t slot = key_lo + tid;
         st_c = ff.cnt[slot];
-        ld_rec<R>(ff.acc + static_cast<size_t>(slot) * RB, st_acc);
+#pragma unroll
+        for (uint32_t q = 0; q < RB / CPB; q++) cp_async<CPB>(kacc + tid * RB + q * CPB, ff.acc + static_cast<size_t>(slot) * RB + q * CPB);
     }
     if (tid < BK_KEYS) kleft[tid] = 0;
     // ---- bucket range = exclusive scan of the pass histogram --------------------------------------------------------------
@@ -1804,18 +1821,37 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
         if (tid == bucket / DPT) {
             uint32_t base = incl - sum;
             for (uint32_t w = 0; w < warp; w++) base += misc[w];
-            uint32_t own = 0;
-#pragma unroll
-            for (uint32_t q = 0; q < DPT; q++) { if (q < bucket % DPT) base += cc[q]; if (q == bucket % DPT) own = cc[q]; }
-            s_boff[0] = base; s_boff[1] = base + own;
+            for (uint32_t q = bucket - bucket % DPT; q < bucket; q++) base += digit_counts[q]; // (L1 hits; indexing cc would put it in local memory)
+            s_boff[0] = base; s_boff[1] = base + digit_counts[bucket];
         }
         __syncthreads();
     }
+    const uint32_t bbeg = s_boff[0], bend = s_boff[1];
+    // the bucket list of the chunk at `at` -> s_lslot / s_lpos, asynchronously. Item r * BK_THREADS + tid is copied and later read by
+    // thread tid alone: its own cp.async.wait_all makes it visible, no barrier is needed.
+    const auto fetch_list = [&](uint32_t at, uint32_t end) {
+#pragma unroll
+        for (uint32_t r = 0; r < IT; r++) {
+            const uint32_t i = r * BK_THREADS + tid;
+            if (at + i < end) {
+                cp_async<4>(s_lslot + i, bk_slots + at + i);
+                if (!moved) cp_async<4>(s_lpos + i, bk_pos + at + i);
+            }
+        }
+    };
+    fetch_list(bbeg, bend); // the first chunk's list: in flight during the key counts
     // items of every key in this stream segment (the whole bucket, all chunks): the deferral of fired groups needs them. Counting
     // them here instead of one global RED per survivor in the streaming pass is what that pass is sensitive to (+17 us per RED).
-    for (uint32_t i = s_boff[0] + tid; i < s_boff[1]; i += BK_THREADS) {
-        const uint32_t lk = bk_slots[i] - key_lo;
-        if (lk < kpc) atomicAdd(&kleft[lk], 1u);
+    // BK_CNT_U loads per thread are in flight before the first count: a bucket of 4096 items costs two round trips.
+    for (uint32_t base = bbeg; base < bend; base += BK_CNT_U * BK_THREADS) {
+        uint32_t lk[BK_CNT_U];
+#pragma unroll
+        for (uint32_t q = 0; q < BK_CNT_U; q++) {
+            const uint32_t i = base + q * BK_THREADS + tid;
+            lk[q] = i < bend ? bk_slots[i] - key_lo : 0xffffffffu;
+        }
+#pragma unroll
+        for (uint32_t q = 0; q < BK_CNT_U; q++) if (lk[q] < kpc) atomicAdd(&kleft[lk[q]], 1u);
     }
     __syncthreads();
     if (tid < BK_KEYS) {
@@ -1827,53 +1863,56 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
             cp = static_cast<uint32_t>(c % P32); leaf = static_cast<uint32_t>((c / P32) & (n - 1));
             if (c < ff.B) { g = 0; tt = ff.B - c; }
             else { g = 1 + (c - ff.B) / group_items; tt = ff.B + g * group_items - c; }
-            if (cp) st_rec<R>(kacc + tid * RB, st_acc);
         }
         kleft[tid] = m; kc[tid] = c; kg[tid] = g; ktt[tid] = tt; kcp[tid] = cp; kleaf[tid] = leaf;
     }
     const uint32_t any_items = __syncthreads_or(my_total != 0);
     BK_MARK(1);
-    if (!any_items) return;
-    uint32_t cursor = s_boff[0];
-    const uint32_t bend = s_boff[1];
+    if (!any_items) { cp_async_wait_all(); BK_MARK(7); return; }
     if (moved)
-        for (size_t o = static_cast<size_t>(tid) * 128; o < static_cast<size_t>(bend - cursor) * RB; o += BK_THREADS * 128) // the bucket's block -> L2
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(lifted + static_cast<size_t>(cursor) * RB + o));
+        for (size_t o = static_cast<size_t>(tid) * 128; o < static_cast<size_t>(bend - bbeg) * RB; o += BK_THREADS * 128) // the bucket's block -> L2
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(lifted + static_cast<size_t>(bbeg) * RB + o));
 
-    while (cursor < bend) {
-        const uint32_t nsel = min(BK_CAP, bend - cursor);
-        // ---- 1. stable split of the chunk's items by key: thread t owns items [t*BK_IT, +BK_IT) --------------------------------------
-        uint32_t ek[BK_IT], ep[BK_IT]; // local key (BK_KEYS = none), record index
+    // s_boff[0] is the chunk cursor: kept in shared memory, no register is held across the chunk
+    for (uint32_t cursor = s_boff[0]; cursor < s_boff[1]; cursor = s_boff[0]) {
+        const uint32_t nsel = min(CAP, s_boff[1] - cursor);
+        // ---- 1. stable split of the chunk's items by key: item r * BK_THREADS + tid is this thread's r-th -------------------------
+        uint32_t ek[IT], ep[IT]; // local key (BK_KEYS = none) | rank among the warp's items of the key << 8, record index
+        cp_async_wait_all();     // (the first chunk's list; the later ones landed with the previous chunk's gather)
 #pragma unroll
-        for (uint32_t r = 0; r < BK_IT; r++) {
-            const uint32_t i = tid * BK_IT + r;
+        for (uint32_t r = 0; r < IT; r++) {
+            const uint32_t i = r * BK_THREADS + tid;
             ek[r] = BK_KEYS; ep[r] = cursor + i;
             if (i < nsel) {
-                const uint32_t lk = bk_slots[cursor + i] - key_lo; // slots outside the bucket's keys (invalid slots) are dropped
-                if (!moved) ep[r] = bk_pos[cursor + i];             // records still in arrival order: the index is the position
+                const uint32_t lk = s_lslot[i] - key_lo; // slots outside the bucket's keys (invalid slots) are dropped
+                if (!moved) ep[r] = s_lpos[i];           // records still in arrival order: the index is the position
                 if (lk < kpc) ek[r] = lk;
             }
         }
         {
-            uint32_t *z = reinterpret_cast<uint32_t *>(&hist[0][0]);
-            for (uint32_t i = tid; i < BK_KEYS * HS / 2; i += BK_THREADS) z[i] = 0;
+            uint32_t *z = reinterpret_cast<uint32_t *>(&s_col[0][0]);
+            for (uint32_t i = tid; i < BK_KEYS * CS / 2; i += BK_THREADS) z[i] = 0;
         }
         __syncthreads();
+        fetch_list(cursor + CAP, s_boff[1]); // the next chunk's list, in flight with this chunk's gather (this thread's reads are done)
 #pragma unroll
-        for (uint32_t r = 0; r < BK_IT; r++) if (ek[r] < BK_KEYS) hist[ek[r]][tid]++; // column tid is private to this thread
-        __syncthreads();
-        { // key (tid & 63), threads [64*(tid >> 6), +64): exclusive scan of the private counts over the threads
-            const uint32_t k = tid & 63u, half = tid >> 6;
-            uint16_t *row = &hist[k][half * 64];
-            uint32_t run = 0;
-#pragma unroll 16
-            for (uint32_t i = 0; i < 64; i++) { const uint32_t c = row[i]; row[i] = static_cast<uint16_t>(run); run += c; }
-            htot[half][k] = run;
+        for (uint32_t r = 0; r < IT; r++) {
+            const uint32_t k = ek[r];
+            const uint32_t peers = __match_any_sync(FULL, k);
+            const uint32_t rank = __popc(peers & lanemask_lt());
+            if (k < BK_KEYS && rank == 0) s_col[k][r * NW + warp] = static_cast<uint16_t>(__popc(peers));
+            ek[r] = k | rank << 8;
         }
         __syncthreads();
         BK_MARK(2);
-        if (warp == 0) { // keys lane and lane+32: chunk totals, exclusive scan over the keys, keys with long runs
-            const uint32_t a0 = htot[0][lane] + htot[1][lane], a1 = htot[0][lane + 32] + htot[1][lane + 32];
+        if (warp == 0) { // keys lane and lane+32: exclusive scan over the columns, chunk totals, exclusive scan over the keys, long runs
+            uint32_t a0 = 0, a1 = 0;
+#pragma unroll
+            for (uint32_t c = 0; c < NCOL; c++) {
+                const uint32_t v0 = s_col[lane][c], v1 = s_col[lane + 32][c];
+                s_col[lane][c] = static_cast<uint16_t>(a0); s_col[lane + 32][c] = static_cast<uint16_t>(a1);
+                a0 += v0; a1 += v1;
+            }
             uint32_t i0 = a0, i1 = a1;
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) {
@@ -1896,28 +1935,30 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
             const uint32_t st0 = __shfl_sync(FULL, s0, 31), nseg = st0 + __shfl_sync(FULL, s1, 31);
             ksegb[lane] = s0 - n0; ksegb[lane + 32] = st0 + s1 - n1;
             // more segments than threads (tiny panes): every run of the chunk is folded by a warp instead
-            const bool fallback = !SEG_OK || nseg > BK_THREADS;
+            const bool fallback = nseg > BK_THREADS;
             const bool h0 = fallback && a0 != 0, h1 = fallback && a1 != 0;
             const uint32_t b0 = __ballot_sync(FULL, h0), b1 = __ballot_sync(FULL, h1);
             if (h0) s_heavy[__popc(b0 & lanemask_lt())] = lane;
             if (h1) s_heavy[__popc(b0) + __popc(b1 & lanemask_lt())] = lane + 32;
-            if (lane == 0) { s_nheavy = __popc(b0) + __popc(b1); s_nseg = fallback ? 0u : nseg; }
+            if (lane == 0) { s_nheavy = __popc(b0) + __popc(b1); s_hnext = 0; s_nseg = fallback ? 0u : nseg; }
         }
         __syncthreads();
-        {
-            const uint32_t hb = tid >> 6;
+        // ---- 2. every item's place in the key-major order; its record -> shared memory there (asynchronous) ------------------------
 #pragma unroll
-            for (uint32_t r = 0; r < BK_IT; r++) {
-                const uint32_t k = ek[r];
-                if (k < BK_KEYS) {
-                    const uint32_t rank = hist[k][tid];
-                    hist[k][tid] = static_cast<uint16_t>(rank + 1);
-                    s_idx[koff[k] + (hb ? htot[0][k] : 0u) + rank] = ep[r];
+        for (uint32_t r = 0; r < IT; r++) {
+            const uint32_t k = ek[r] & 255u;
+            if (k < BK_KEYS) {
+                const uint32_t at = koff[k] + s_col[k][r * NW + warp] + (ek[r] >> 8);
+                s_idx[at] = ep[r];
+                const unsigned char *src = lifted + static_cast<size_t>(ep[r]) * RB;
+#pragma unroll
+                for (uint32_t q = 0; q < RB / CPB; q++) { // (16-byte granules bypass L1: the records are read once)
+                    if constexpr (CPB == 16) cp_async_cg16(s_rec + at * RB + q * CPB, src + q * CPB);
+                    else cp_async<CPB>(s_rec + at * RB + q * CPB, src + q * CPB);
                 }
             }
         }
-        __syncthreads(); // the private counts are dead: their memory now holds the segment descriptors / results
-        // ---- 2. segment descriptors; siblings of the first leaf each key completes -> shared memory (asynchronous) -----------------
+        // segment descriptors; siblings of the first leaf each key completes -> shared memory
         const uint32_t nseg = s_nseg;
         bool sib_staged = false;
         if (tid < BK_KEYS && nseg != 0) {
@@ -1938,60 +1979,52 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                 }
             }
         }
+        cp_async_wait_all();
         __syncthreads();
         BK_MARK(3);
-        // ---- 3a. one thread per segment: plain ordered fold of at most one pane of items, BK_U masked loads per round trip ---------
+        // ---- 3a. one thread per segment: ordered fold of at most one pane of staged records ------------------------------------
         if (tid < nseg) {
             const uint32_t d = seg_desc[tid], k = d & 255u, j = d >> 8;
             const uint32_t m = kcnt[k], cp0 = kcp[k], first = min(m, P32 - cp0);
             const uint32_t start = j == 0 ? 0u : first + (j - 1) * P32;
-            uint32_t seg = j == 0 ? first : min(P32, m - start);
-            bool fresh = j != 0 || cp0 == 0;
-            const uint32_t *ip = s_idx + koff[k] + start;
+            const uint32_t seg = j == 0 ? first : min(P32, m - start);
+            unsigned char *rp = s_rec + (koff[k] + start) * RB;
             alignas(16) R acc;
-            if (!fresh) ld_rec<R>(kacc + k * RB, acc);
-            while (seg != 0) {
-                alignas(16) R it[BK_U];
-                const uint32_t kk = min(seg, BK_U);
-#pragma unroll
-                for (uint32_t q = 0; q < BK_U; q++) if (q < kk) ld_rec<R>(lifted + static_cast<size_t>(ip[q]) * RB, it[q]);
-                if (fresh) acc = it[0]; else P::comb(acc, it[0], acc, prm);
-                fresh = false;
-#pragma unroll
-                for (uint32_t q = 1; q < BK_U; q++) if (q < kk) P::comb(acc, it[q], acc, prm);
-                seg -= kk; ip += kk;
-            }
-            st_rec<R>(seg_res + tid * RB, acc);
+            uint32_t i = 1;
+            if (j == 0 && cp0 != 0) { ld_rec<R>(kacc + k * RB, acc); i = 0; } // the open pane continues
+            else ld_rec<R>(rp, acc);
+#pragma unroll 4
+            for (; i < seg; i++) { alignas(16) R it; ld_rec<R>(rp + i * RB, it); P::comb(acc, it, acc, prm); }
+            st_rec<R>(rp, acc);
         }
         __syncthreads();
+        BK_MARK(4);
         // ---- 3b. one thread per key, its segments in order: completed panes -> leaf + root path + fired group; the rest is the open
         // pane. The loop over the segments is warp-uniform: a group that cannot be deferred (another pane of the key completes
         // in this stream segment and would overwrite ring leaves the windows still need) is evaluated by the whole warp at once.
         if (tid < BK_KEYS && nseg != 0) { // warps 0 and 1, whole
-            const uint32_t k = tid, slot = key_lo + k, m = kcnt[k];
-            const uint32_t cp0 = kcp[k], first = min(m, P32 - cp0), ns = m ? 1u + (m - first + P32 - 1) / P32 : 0u, sb = ksegb[k];
+            const uint32_t k = bk_opaque(tid), m = kcnt[k]; // (the key's slot, key_lo + k, and tree are recomputed where they are used)
+            const uint32_t cp0 = kcp[k];
             uint32_t leafi = kleaf[k], new_cp = cp0, consumed = 0;
             uint64_t g = kg[k], tt = ktt[k]; // tt: index (1-based) of the run's item that fires the next group
-            const uint32_t left0 = kleft[k];
-            unsigned char *tree = ff.tree + static_cast<size_t>(slot) * tree_stride;
-            const uint64_t key = key_of_slot(ff, slot < ff.max_keys ? slot : 0u);
-            for (uint32_t j = 0; __any_sync(FULL, j < ns); j++) {
+            while (__any_sync(FULL, consumed < m)) {
                 bool eval_now = false;
                 uint32_t ev_obase = 0, ev_pos = 0;
                 uint64_t ev_g = 0;
-                if (j < ns) {
-                    const uint32_t len = j == 0 ? first : min(P32, m - consumed);
-                    consumed += len;
+                if (consumed < m) {
+                    const uint32_t open = consumed == 0 ? cp0 : 0u; // items already in the pane the segment continues
+                    const uint32_t len = min(m - consumed, P32 - open);
                     alignas(16) R cur;
-                    ld_rec<R>(seg_res + (sb + j) * RB, cur);
-                    const bool completes = (j == 0 ? cp0 + len : len) == P32;
-                    if (!completes) { st_rec<R>(kacc + k * RB, cur); new_cp = (j == 0 ? cp0 : 0u) + len; } // (only the last segment)
+                    ld_rec<R>(s_rec + (koff[k] + consumed) * RB, cur); // the segment's fold
+                    consumed += len;
+                    const bool completes = open + len == P32;
+                    if (!completes) { st_rec<R>(kacc + k * RB, cur); new_cp = open + len; } // (only the last segment)
                     else {
                         new_cp = 0;
-                        const uint32_t leaf = leafi;
+                        const uint32_t slot = key_lo + k, leaf = leafi;
+                        unsigned char *tree = ff.tree + static_cast<size_t>(slot) * tree_stride;
                         leafi = (leafi + 1) & (n - 1);
                         st_rec<R>(tree + static_cast<size_t>(leaf) * RB, cur);
-                        if (sib_staged) cp_async_wait_all();
                         for (uint32_t l0 = 0; l0 < (LAZY ? 0u : logn); l0 += 4) { // siblings of four levels per round trip (none of them is on the path)
                             alignas(16) R sbl[4];
 #pragma unroll
@@ -2018,10 +2051,10 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                             const uint32_t lp = s_idx[koff[k] + consumed - 1];
                             const uint32_t last_pos = moved ? bk_pos[lp] : lp; // arrival position of the triggering item
                             const uint32_t obase = atomicAdd(n_out, ff.nb);
-                            bool deferred = (left0 - consumed) < ff.defer_items; // the panes this key still completes in this segment fit the spare ring leaves
+                            bool deferred = (kleft[k] - consumed) < ff.defer_items; // the panes this key still completes in this segment fit the spare ring leaves
                             if (deferred) {
                                 const uint32_t ti = atomicAdd(ff.n_trig, 1u);
-                                if (ti < ff.trig_cap) { Trigger tr; tr.key = key; tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
+                                if (ti < ff.trig_cap) { Trigger tr; tr.key = key_of_slot(ff, slot); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
                                 else deferred = false;
                             }
                             if (!deferred) { eval_now = true; ev_obase = obase; ev_pos = last_pos; ev_g = g; }
@@ -2034,8 +2067,8 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                 while (pend) {
                     const int src = __ffs(pend) - 1;
                     pend &= pend - 1;
-                    const uint32_t e_slot = __shfl_sync(FULL, slot, src), e_obase = __shfl_sync(FULL, ev_obase, src), e_pos = __shfl_sync(FULL, ev_pos, src);
-                    const uint64_t e_key = __shfl_sync(FULL, key, src), e_g = __shfl_sync(FULL, ev_g, src);
+                    const uint32_t e_slot = key_lo + (warp << 5) + src, e_obase = __shfl_sync(FULL, ev_obase, src), e_pos = __shfl_sync(FULL, ev_pos, src);
+                    const uint64_t e_key = key_of_slot(ff, e_slot), e_g = __shfl_sync(FULL, ev_g, src);
                     const unsigned char *e_tree = ff.tree + static_cast<size_t>(e_slot) * tree_stride;
                     const uint64_t wm = batch_watermark(batch_off, batches, nbatches, e_pos);
                     for (uint32_t i = lane; i < ff.nb; i += 32)
@@ -2043,29 +2076,29 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                 }
                 __syncwarp(); // the evaluated windows read tree nodes another lane has just written, and it may overwrite them next
             }
-            if (sib_staged) cp_async_wait_all(); // (a staged key always completes its first segment: nothing is pending here)
-            if (m != 0) { kc[k] += m; kg[k] = g; ktt[k] = tt - m; kcp[k] = new_cp; kleaf[k] = leafi; kleft[k] = left0 - m; }
+            if (m != 0) { kc[k] += m; kg[k] = g; ktt[k] = tt - m; kcp[k] = new_cp; kleaf[k] = leafi; kleft[k] -= m; }
         }
-        BK_MARK(4);
-        // ---- 3. long runs: one warp per key, ordered shuffle-tree fold of 32 records per load ----------------------------------------
+        BK_MARK(5);
+        // ---- 4. tiny panes: one warp per key, ordered shuffle-tree fold of 32 staged records at a time -----------------------------
         if (s_nheavy != 0) { // (block-uniform: written before the last barrier)
             __syncthreads();
-            for (uint32_t h = warp; h < s_nheavy; h += NW) {
+            for (;;) { // a warp claims the next key (no loop counter is held across the fold)
+                uint32_t h = 0;
+                if (lane == 0) h = atomicAdd(&s_hnext, 1u);
+                h = __shfl_sync(FULL, h, 0);
+                if (h >= s_nheavy) break;
                 const uint32_t k = s_heavy[h];
                 const uint32_t m = kcnt[k], off = koff[k], slot = key_lo + k;
-                uint64_t c = kc[k], g = kg[k], tt = ktt[k];
+                uint64_t g = kg[k], tt = ktt[k];
                 uint32_t cp = kcp[k], leafi = kleaf[k], left = kleft[k];
-                const uint64_t key = key_of_slot(ff, slot);
                 unsigned char *tree = ff.tree + static_cast<size_t>(slot) * tree_stride;
                 alignas(16) R acc;
                 if (cp) ld_rec<R>(kacc + k * RB, acc);
-                alignas(16) R cur_rec;
-                if (lane < m) ld_rec<R>(lifted + static_cast<size_t>(s_idx[off + lane]) * RB, cur_rec);
                 uint32_t j = 0;
                 while (j < m) {
                     const uint32_t cnt = min(32u, m - j);
-                    alignas(16) R nxt_rec;
-                    if (j + 32 + lane < m) ld_rec<R>(lifted + static_cast<size_t>(s_idx[off + j + 32 + lane]) * RB, nxt_rec);
+                    alignas(16) R cur_rec;
+                    if (lane < cnt) ld_rec<R>(s_rec + (off + j + lane) * RB, cur_rec);
                     uint32_t lo = 0;
                     while (lo < cnt) { // sub-ranges of the 32 records that fall into one pane
                         const uint32_t hi = min(cnt, lo + (P32 - cp));
@@ -2078,7 +2111,7 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                         r = shfl_rec<R>(r, lo);
                         if (cp == 0) acc = r; else P::comb(acc, r, acc, prm);
                         const uint32_t take = hi - lo;
-                        cp += take; c += take; left -= take; tt -= take;
+                        cp += take; left -= take; tt -= take;
                         if (cp == P32) { // pane complete -> leaf + root path
                             cp = 0;
                             const uint32_t leaf = leafi;
@@ -2107,11 +2140,12 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                                     if (lane == 0) ti = atomicAdd(ff.n_trig, 1u);
                                     ti = __shfl_sync(FULL, ti, 0);
                                     if (ti < ff.trig_cap) {
-                                        if (lane == 0) { Trigger tr; tr.key = key; tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
+                                        if (lane == 0) { Trigger tr; tr.key = key_of_slot(ff, slot); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
                                     } else deferred = false;
                                 }
                                 if (!deferred) {
                                     const uint64_t wm = batch_watermark(batch_off, batches, nbatches, last_pos);
+                                    const uint64_t key = key_of_slot(ff, slot);
                                     for (uint32_t i = lane; i < ff.nb; i += 32)
                                         ffat_eval_window<P>(ff, tree, key, g * ff.nb + i, wm, obase + i, out_res, out_ts, out_cap, prm);
                                 }
@@ -2122,25 +2156,24 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                         lo = hi;
                     }
                     j += cnt;
-                    cur_rec = nxt_rec;
                 }
                 if (lane == 0) {
-                    kc[k] = c; kg[k] = g; ktt[k] = tt; kcp[k] = cp; kleaf[k] = leafi; kleft[k] = left;
+                    kc[k] += m; kg[k] = g; ktt[k] = tt; kcp[k] = cp; kleaf[k] = leafi; kleft[k] = left;
                     if (cp) st_rec<R>(kacc + k * RB, acc);
                 }
             }
         }
-        cursor += nsel;
+        if (tid == 0) s_boff[0] += CAP; // (every thread has read it before the chunk's first barrier)
         __syncthreads(); // the next chunk overwrites the shared buffers
+        BK_MARK(6);
     }
-    BK_MARK(5);
-    // ---- keys' state back as contiguous blocks -----------------------------------------------------------------------------------
-    if (tid < kpc && my_total) {
-        const uint32_t slot = key_lo + tid;
-        ff.cnt[slot] = kc[tid];
-        if (kcp[tid]) { alignas(16) R a; ld_rec<R>(kacc + tid * RB, a); st_rec<R>(ff.acc + static_cast<size_t>(slot) * RB, a); }
+    // ---- keys' state back as contiguous blocks (a key without items rewrites its count; its cp is 0: no accumulator) ------------
+    if (tid < kpc && key_lo + tid < ff.max_keys) {
+        const uint32_t k = bk_opaque(tid), slot = key_lo + k;
+        ff.cnt[slot] = kc[k];
+        if (kcp[k]) { alignas(16) R a; ld_rec<R>(kacc + k * RB, a); st_rec<R>(ff.acc + static_cast<size_t>(slot) * RB, a); }
     }
-    BK_MARK(6);
+    BK_MARK(7);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -53,6 +53,11 @@ __device__ __forceinline__ void cp_async(void *smem_dst, const void *gmem_src)
     static_assert(BYTES == 4 || BYTES == 8 || BYTES == 16, "cp.async copies 4, 8 or 16 bytes");
     asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "n"(BYTES) : "memory");
 }
+// the same, 16 bytes, bypassing L1: a copy in flight holds no L1 line (random gathers with many copies in flight per SM)
+__device__ __forceinline__ void cp_async_cg16(void *smem_dst, const void *gmem_src)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait_group() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); } // at most N groups of this thread pending
