@@ -140,11 +140,18 @@ template <class T, class R> struct NoLift { __host__ __device__ void operator()(
 template <class R> struct NoComb { __host__ __device__ void operator()(const R &, const R &, R &) const {} };
 template <class T> struct NoReduce { __host__ __device__ T operator()(const T &a, const T &) const { return a; } };
 
+// The key type of an operator is what its key extractor returns (as in the reference, wf/keyby_emitter_gpu.hpp:108): an integral or
+// enum type, float, double, or a trivially copyable type of at most 16 bytes without padding or floating-point members (such as a
+// struct { uint32_t src, dst; }). windflow_b200/csrc/wfb_keys.cuh maps it to the words the device key table stores; any other type
+// fails to compile there.
+template <class KeyF> using key_of_t = std::decay_t<fn_ret_t<KeyF>>;
+template <class KeyF> constexpr bool integral_key_v = wfb::KeyCodec<key_of_t<KeyF>>::kind == wfb::KEY_KIND_INTEGRAL;
+
 // The program the kernels are instantiated for: the user's functor objects travel by value in params_t; the map / filter slots
 // hold the fused chain that runs in front of the operator.
 template <class T, class R, class KeyF, class LiftF, class CombF, class RedF, bool KEYED, class PreF = ChainStages<T>>
 struct FacadeProgram {
-    using tuple_t = T; using result_t = R; using key_t = uint64_t;
+    using tuple_t = T; using result_t = R; using key_t = key_of_t<KeyF>;
     // (a typed run leaves no stage that is called through a pointer: the tuple then stays in registers)
     using map_slot_t = std::conditional_t<is_chain<PreF>::value, ChainStages<T>, TypedChain<T>>;
     struct params_t { map_slot_t map; PreF filt; KeyF key; LiftF lift; CombF comb; RedF red; };
@@ -152,12 +159,12 @@ struct FacadeProgram {
     static_assert(sizeof(T) % 8 == 0 && sizeof(R) % 8 == 0, "tuple_t / result_t sizes must be multiples of 8 bytes");
     __host__ __device__ static void map(tuple_t &t, const params_t &p) { p.map(t); }
     __host__ __device__ static bool filter(tuple_t &t, const params_t &p) { return p.filt(t); }
-    __host__ __device__ static key_t key(const tuple_t &t, const params_t &p) { KeyF f = p.key; return static_cast<key_t>(f(t)); }
+    __host__ __device__ static key_t key(const tuple_t &t, const params_t &p) { KeyF f = p.key; return f(t); }
     __host__ __device__ static void lift(const tuple_t &t, result_t &r, const params_t &p) { LiftF f = p.lift; f(t, r); }
     __host__ __device__ static void comb(const result_t &a, const result_t &b, result_t &o, const params_t &p) { CombF f = p.comb; f(a, b, o); }
     __host__ __device__ static result_t make_result(key_t k, uint64_t gwid, const params_t &)
     {   // create_win_result_t_gpu, wf/basic_gpu.hpp:236-247: result_t(key, gwid) when keyed, result_t(gwid) otherwise
-        if constexpr (KEYED && std::is_constructible<result_t, fn_ret_t<KeyF>, uint64_t>::value) { result_t r(static_cast<fn_ret_t<KeyF>>(k), gwid); return r; }
+        if constexpr (KEYED && std::is_constructible<result_t, key_t, uint64_t>::value) { result_t r(k, gwid); return r; }
         else if constexpr (!KEYED && std::is_constructible<result_t, uint64_t>::value) { result_t r(gwid); return r; }
         else { (void) k; (void) gwid; return result_t(); } // programs of operators without windows never call this
     }
@@ -169,13 +176,13 @@ template <class T> using ChainProgram = FacadeProgram<T, T, NoKey<T>, NoLift<T, 
 // (API: __host__ __device__ void(tuple_t &, state_t &) / bool(tuple_t &, state_t &), wf/map_gpu.hpp:104-310, wf/filter_gpu.hpp:120-399).
 template <class T, class S, class MapF2, class FiltF2, class KeyF>
 struct FacadeStatefulProgram {
-    using tuple_t = T; using result_t = T; using key_t = uint64_t; using state_t = S;
+    using tuple_t = T; using result_t = T; using key_t = key_of_t<KeyF>; using state_t = S;
     struct params_t { MapF2 map; FiltF2 filt; KeyF key; };
     static_assert(std::is_trivially_copyable<T>::value && std::is_trivially_copyable<S>::value, "tuple_t / state_t must be trivially copyable");
     static_assert(sizeof(T) % 8 == 0, "tuple_t size must be a multiple of 8 bytes");
     __host__ __device__ static void map(tuple_t &, const params_t &) {}
     __host__ __device__ static bool filter(tuple_t &, const params_t &) { return true; }
-    __host__ __device__ static key_t key(const tuple_t &t, const params_t &p) { KeyF f = p.key; return static_cast<key_t>(f(t)); }
+    __host__ __device__ static key_t key(const tuple_t &t, const params_t &p) { KeyF f = p.key; return f(t); }
     __host__ __device__ static void lift(const tuple_t &t, result_t &r, const params_t &) { r = t; }
     __host__ __device__ static void comb(const result_t &, const result_t &, result_t &, const params_t &) {}
     __host__ __device__ static result_t make_result(key_t, uint64_t, const params_t &) { return result_t(); }
@@ -763,7 +770,7 @@ public:
             Basic_Replica::svc_init();
             wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
             wfbErrChk(wfb_engine_set_params(eng, &prm, sizeof(prm)));
-            wfbErrChk(wfb_engine_set_key_bits(eng, key_bits));
+            if (key_bits != 64) wfbErrChk(wfb_engine_set_key_bits(eng, key_bits)); // (integral keys: ReduceGPU_Builder::build checks)
             gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING));
             return 0;
         }
@@ -794,7 +801,8 @@ public:
                 outs[i] = o;
             }
             if constexpr (isKeyed) {
-                if (k > 1 && key_bits + kbits <= 64) { wfbErrChk(wfb_reduce_by_key_batches(eng, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d + ring, stream)); }
+                const uint32_t sort_bits = integral_key_v<keyextr_func_gpu_t> ? key_bits : 32u; // other keys are sorted by their 32-bit rank
+                if (k > 1 && sort_bits + kbits <= 64) { wfbErrChk(wfb_reduce_by_key_batches(eng, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d + ring, stream)); }
                 else for (size_t i = 0; i < k; i++)
                     wfbErrChk(wfb_reduce_by_key(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), counts_d + ring + i, stream));
                 gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
@@ -1007,14 +1015,18 @@ public:
     explicit ReduceGPU_Builder(reduce_func_gpu_t f): func(f), key_extr() {}
     auto &withName(std::string n) { name = std::move(n); return *this; }
     auto &withParallelism(size_t p) { parallelism = p; return *this; }
-    auto &withKeyBits(uint32_t b) { key_bits = b; return *this; } // extension: significant low bits of the key (fewer radix passes)
+    auto &withKeyBits(uint32_t b) { key_bits = b; return *this; } // extension: significant low bits of an integral key (fewer radix passes)
     template <class new_keyextr_t> auto withKeyBy(new_keyextr_t k)
     {
         ReduceGPU_Builder<reduce_func_gpu_t, new_keyextr_t> nb(func, k);
         nb.name = name; nb.parallelism = parallelism; nb.mode = Routing_Mode_t::KEYBY; nb.key_bits = key_bits;
         return nb;
     }
-    auto build() { Reduce_GPU<reduce_func_gpu_t, keyextr_func_gpu_t> r(func, key_extr, parallelism, name, mode); r.key_bits = key_bits; return r; }
+    auto build()
+    {   // (withKeyBits may precede withKeyBy: the key type is known here)
+        if (key_bits != 64 && !integral_key_v<keyextr_func_gpu_t>) wf_fatal("ReduceGPU_Builder: withKeyBits() needs an integral or enum key type");
+        Reduce_GPU<reduce_func_gpu_t, keyextr_func_gpu_t> r(func, key_extr, parallelism, name, mode); r.key_bits = key_bits; return r;
+    }
 };
 
 template <class lift_func_gpu_t, class comb_func_gpu_t, class keyextr_func_gpu_t = NoKey<fn_arg_t<lift_func_gpu_t, 0>>>
@@ -1039,9 +1051,17 @@ public:
     auto &withLateness(std::chrono::microseconds l) { lateness = l.count(); return *this; }
     auto &withNumWinPerBatch(size_t n) { numWinPerBatch = n; return *this; }
     auto &withMaxKeys(uint32_t n) { max_keys = n; return *this; }       // extension: capacity of the device-resident key table
-    auto &withDenseKeys() { dense = true; return *this; }               // extension: keys are 0 .. max_keys-1 (slot = key, no hash probe)
+    auto &withDenseKeys()                                               // extension: keys are 0 .. max_keys-1 (slot = key, no hash probe)
+    {
+        static_assert(integral_key_v<keyextr_func_gpu_t>, "WindFlow Compilation Error - Ffat_WindowsGPU_Builder: withDenseKeys() needs an integral or enum key type:\n");
+        dense = true; return *this;
+    }
     auto &withMaxBatchesPerCall(size_t k) { max_batches = k; return *this; } // extension: queued batches one svc() hands to one launch sequence
-    auto build() { return Ffat_Windows_GPU<lift_func_gpu_t, comb_func_gpu_t, keyextr_func_gpu_t>(lift, comb, key_extr, name, win_len, slide_len, lateness, winType, numWinPerBatch, max_keys, dense, max_batches); }
+    auto build()
+    {   // (withDenseKeys before withKeyBy: the key type is known here)
+        if (dense && !integral_key_v<keyextr_func_gpu_t>) wf_fatal("Ffat_WindowsGPU_Builder: withDenseKeys() needs an integral or enum key type");
+        return Ffat_Windows_GPU<lift_func_gpu_t, comb_func_gpu_t, keyextr_func_gpu_t>(lift, comb, key_extr, name, win_len, slide_len, lateness, winType, numWinPerBatch, max_keys, dense, max_batches);
+    }
 };
 
 // ---- MultiPipe / PipeGraph (wf/multipipe.hpp, wf/pipegraph.hpp) ------------------------------------------------------------------------

@@ -43,11 +43,16 @@ extern "C" {
 #define WFB_PROG_WFTEST16 1   /* reference tests/graph_tests_gpu/graph_common_gpu.hpp:40-49 {key,value}  */
 #define WFB_PROG_WFWIN24  2   /* reference tests/win_tests_gpu/win_common_gpu.hpp:40-80 {key,id,value}   */
 #define WFB_PROG_LIFTED32 3   /* already-lifted wfb_result32_t records (destination side of the multi-GPU keyby) */
+#define WFB_PROG_TUPLE64_FKEY 4 /* wfb_tuple64_t keyed by the double whose bits are pad[0] -> wfb_result32d_t (a floating-point key) */
+#define WFB_PROG_TUPLE64_K16  5 /* wfb_tuple64_t keyed by wfb_key16_t {key, low and high half of pad[0]} -> wfb_result48k_t (a 16-byte key) */
 
 typedef struct { uint64_t key; uint64_t id; int64_t ivalue; double fvalue; uint64_t pad[4]; } wfb_tuple64_t;
 typedef struct { uint64_t key; uint64_t id; int64_t isum; double fsum; } wfb_result32_t;
 typedef struct { uint64_t key; int64_t value; } wfb_wftest16_t;
 typedef struct { uint64_t key; uint64_t id; int64_t value; } wfb_wfwin24_t; /* tuple_t and result_t */
+typedef struct { double key; uint64_t id; int64_t isum; double fsum; } wfb_result32d_t;
+typedef struct { uint64_t key; uint32_t a, b; } wfb_key16_t;
+typedef struct { wfb_key16_t key; uint64_t id; int64_t isum; double fsum; uint64_t pad; } wfb_result48k_t;
 typedef struct { int64_t counter; } wfb_state8_t; /* per-key state of the built-in stateful functors (map_state_t / filter_state_t of the reference's tests) */
 
 /* Parameters of the built-in functors (a user program carries its own functor objects instead).
@@ -66,8 +71,8 @@ typedef struct {
 typedef struct {
     uint32_t tuple_bytes;   /* sizeof(tuple_t) */
     uint32_t result_bytes;  /* sizeof(result_t) of the window operators */
-    uint32_t key_bytes;     /* sizeof(key_t) (8 for all built-ins) */
-    uint32_t reserved;
+    uint32_t key_bytes;     /* bytes of the key's canonical words: 8 (key_t of at most 8 bytes) or 16 (9-16 bytes) */
+    uint32_t key_kind;      /* 0 integral or enum, 1 float / double, 2 other bytes (windflow_b200/csrc/wfb_keys.cuh) */
 } wfb_program_info_t;
 
 /* One input batch of a multi-batch call (host-side descriptor array). */
@@ -89,7 +94,7 @@ int         wfb_device_count(void);                    /* 0 => every compute ent
 int         wfb_program_info(int prog, wfb_program_info_t *info);
 /* Adds an application-defined program (record schema + functors compiled in the application's own .cu): `ops` is the
  * launch table built by wfb::register_program<P>() of windflow_b200/csrc/wfb_launch.cuh. Returns the new program id
- * (>= 4) or a negative error. For such programs every `const wfb_functors_t *` parameter below points to the program's
+ * (>= 6) or a negative error. For such programs every `const wfb_functors_t *` parameter below points to the program's
  * own params_t (its functor objects) instead. */
 int         wfb_program_register(const void *ops, size_t ops_bytes);
 
@@ -105,7 +110,7 @@ uint64_t wfb_engine_launches(const wfb_engine_t *e);
 int wfb_engine_set_params(wfb_engine_t *e, const void *params, size_t bytes);
 
 /* number of significant low bits of key_t for the per-batch keyed operators below (default 64): the stable LSD
- * radix sort that replaces thrust::sort_by_key runs ceil(bits/8) passes. */
+ * radix sort that replaces thrust::sort_by_key runs ceil(bits/8) passes. Integral keys only (WFB_E_BADARG otherwise). */
 int wfb_engine_set_key_bits(wfb_engine_t *e, uint32_t bits);
 
 /* ---- Map_GPU, stateless: in-place func(tuple) over a batch --------------------------------------
@@ -144,7 +149,8 @@ int wfb_filter_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batc
                         uint32_t *n_out_dev, void *stream);
 
 /* ---- Reduce_GPU, per batch -------------------------------------------------------------------------
- * keyed: one output item per distinct key, ascending key order, tuple = fold of the program's reduce functor
+ * keyed: one output item per distinct key, ascending key order (floating-point keys: numeric, NaN last; other keys that are not
+ * integers: their bytes read as a little-endian unsigned integer), tuple = fold of the program's reduce functor
  * over the key's items, ts = max ts. replaces Extract_Keys_Kernel + sort_by_key + reduce_by_key + D2D,
  * wf/reduce_gpu.hpp:75-105, :226-262. */
 int wfb_reduce_by_key(wfb_engine_t *e, const void *tuples, const uint64_t *ts, uint32_t n,
@@ -163,6 +169,7 @@ int wfb_reduce_all(wfb_engine_t *e, const void *tuples, const uint64_t *ts, uint
  * the same key or -1, dist_keys[k] = the key; *n_keys_dev = number of distinct keys.
  * replaces Extract_Dests_Kernel + sort_by_key + Compute_Mapping_Kernel + unique_by_key_copy,
  * wf/keyby_emitter_gpu.hpp:68-100, :519-583. */
+/* integral keys only (WFB_E_UNSUPPORTED otherwise), as for wfb_shard_by_key, wfb_shard_lift and wfb_mg_create */
 int wfb_keyby_group(wfb_engine_t *e, const void *tuples, uint32_t n,
                     int32_t *start_idxs, int32_t *map_idxs, uint64_t *dist_keys, uint32_t *n_keys_dev,
                     void *stream);
@@ -186,7 +193,7 @@ int wfb_shard_lift(wfb_engine_t *e, const wfb_functors_t *pre, const wfb_batch_t
  * wf/ffat_replica_gpu.hpp:438-506, wf/flatfat_gpu.hpp:165-192.
  *   win_type: 0 count-based (win/slide in tuples, wfb_ffat_process_cb), 1 time-based (win/slide/lateness in timestamp
  *             units, wfb_ffat_process_tb)
- *   flags   : WFB_FFAT_DENSE_KEYS => keys are known to be < max_keys (slot = key, no hash probe) */
+ *   flags   : WFB_FFAT_DENSE_KEYS => keys are known to be < max_keys (slot = key, no hash probe); integral keys only (WFB_E_BADARG) */
 #define WFB_FFAT_DENSE_KEYS 1u
 /*   WFB_FFAT_PIPELINED  => results are delivered one call late: wfb_ffat_process_cb(segment k) returns the results of
  *                          segment k-1 (none on the first call) while sort + update of segment k run on an internal stream and

@@ -15,7 +15,7 @@ class Functors(C.Structure):
 
 
 class ProgramInfo(C.Structure):
-    _fields_ = [("tuple_bytes", u32), ("result_bytes", u32), ("key_bytes", u32), ("reserved", u32)]
+    _fields_ = [("tuple_bytes", u32), ("result_bytes", u32), ("key_bytes", u32), ("key_kind", u32)]
 
 
 class Batch(C.Structure):

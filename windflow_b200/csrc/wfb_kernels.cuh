@@ -25,8 +25,18 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include "wfb_ptx.cuh"
+#include "wfb_keys.cuh"
 
 namespace wfb {
+
+// the canonical words of a program's key (wfb_keys.cuh): uint64_t for keys of at most 8 bytes, Key128 for 9-16 bytes
+template <class P> using key_codec = KeyCodec<typename P::key_t>;
+template <class P> using key_words_t = typename key_codec<P>::words_t;
+template <class P>
+__host__ __device__ __forceinline__ key_words_t<P> key_words(const typename P::tuple_t &t, const typename P::params_t &prm)
+{
+    return key_codec<P>::encode(P::key(t, prm));
+}
 
 constexpr int TILE = 256;    // tuples per tile == threads per CTA of k_tile_pass
 constexpr uint32_t OSW_TILE_POS = 4096; // positions per tile of the wide partition pass (== OSW_TILE below)
@@ -58,12 +68,13 @@ struct DevBatch {
     uint32_t tile_begin;       // first global tile index of this batch
 };
 
-// one fired window group whose Nb window queries are evaluated after the update kernel
+// one fired window group whose Nb window queries are evaluated after the update kernel. `key` holds the key of a one-word program;
+// a group of a two-word program reads its key from FfatDev::slot_key[slot] (trig_key below).
 struct Trigger { uint64_t key; uint64_t g; uint32_t slot; uint32_t last_pos; uint32_t obase; uint32_t pad; };
 
 // key -> slot table (open addressing, linear probing) + per-key window state of one Ffat_Windows_GPU
 struct FfatDev {
-    // key table
+    // key table (entries and slot keys are key_codec<P>::words words wide: one 8-byte word, or two for a 16-byte key)
     uint64_t *ht_keys;         // capacity entries, EMPTY_KEY when free
     uint32_t *ht_slots;        // capacity entries, INVALID_SLOT until published
     uint32_t ht_mask;          // capacity - 1
@@ -237,9 +248,52 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x)
     return x;
 }
 
-__device__ __forceinline__ uint64_t key_of_slot(const FfatDev &ff, uint32_t slot)
+template <class P>
+__device__ __forceinline__ key_words_t<P> key_of_slot(const FfatDev &ff, uint32_t slot)
 {
-    return ff.dense ? (ff.key_div > 1 ? static_cast<uint64_t>(slot) * ff.key_div + ff.key_rem : static_cast<uint64_t>(slot)) : ff.slot_key[slot];
+    if constexpr (key_codec<P>::words == 2) return reinterpret_cast<const Key128 *>(ff.slot_key)[slot]; // (never dense)
+    else return ff.dense ? (ff.key_div > 1 ? static_cast<uint64_t>(slot) * ff.key_div + ff.key_rem : static_cast<uint64_t>(slot)) : ff.slot_key[slot];
+}
+// the key a Trigger carries (one-word keys only) and the key of a fired group
+__device__ __forceinline__ uint64_t trig_word(uint64_t key) { return key; }
+__device__ __forceinline__ uint64_t trig_word(const Key128 &) { return 0; }
+template <class P>
+__device__ __forceinline__ key_words_t<P> trig_key(const FfatDev &ff, const Trigger &tr)
+{
+    if constexpr (key_codec<P>::words == 2) return key_of_slot<P>(ff, tr.slot); else return tr.key;
+}
+
+// 16-byte keys: one 16-byte load per probe. The load may see an entry that a concurrent 16-byte CAS is writing half done, so an entry
+// with an all-ones half -- free, half written, or a key with such a half -- is settled with the CAS (which returns the whole entry)
+// before it is compared: a torn read never counts as a hit. The all-ones key itself marks a free entry: it is refused with the key
+// table's capacity flag.
+__device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, const Key128 &key)
+{
+    if (key.lo == EMPTY_KEY && key.hi == EMPTY_KEY) { atomicOr(ff.err_flags, 1u); return INVALID_SLOT; }
+    uint32_t h = static_cast<uint32_t>(mix64(key.lo ^ mix64(key.hi))) & ff.ht_mask;
+    for (uint32_t probe = 0; probe <= ff.ht_mask; probe++) {
+        uint64_t *e = ff.ht_keys + 2 * static_cast<size_t>(h);
+        Key128 k;
+        ld_relaxed_v2u64(e, k.lo, k.hi);
+        if (k.lo == EMPTY_KEY || k.hi == EMPTY_KEY) {
+            atom_cas_b128(e, EMPTY_KEY, EMPTY_KEY, key.lo, key.hi, k.lo, k.hi);
+            if (k.lo == EMPTY_KEY && k.hi == EMPTY_KEY) { // we own the entry: allocate the slot and publish it
+                uint32_t s = atomicAdd(ff.n_slots, 1u);
+                if (s >= ff.max_keys) { atomicOr(ff.err_flags, 1u); s = INVALID_SLOT - 1; }
+                else reinterpret_cast<Key128 *>(ff.slot_key)[s] = key;
+                st_release_u32(&ff.ht_slots[h], s);
+                return s >= ff.max_keys ? INVALID_SLOT : s;
+            }
+        }
+        if (k == key) {
+            uint32_t s;
+            while ((s = ld_acquire_u32(&ff.ht_slots[h])) == INVALID_SLOT) { }
+            return s >= ff.max_keys ? INVALID_SLOT : s;
+        }
+        h = (h + 1) & ff.ht_mask;
+    }
+    atomicOr(ff.err_flags, 1u);
+    return INVALID_SLOT;
 }
 
 __device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, uint64_t key)
@@ -476,13 +530,14 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
                 if (keep) {
                     P::lift(tup, res, prm);
                     if (a.nshards && a.shard_slots) { // keyby across GPUs, bucketed: destination-major virtual slot
-                        const uint64_t key = P::key(tup, prm), q = key / a.nshards;
+                        // (integer keys only: the shard paths refuse other key types)
+                        const uint64_t key = key_word0(key_words<P>(tup, prm)), q = key / a.nshards;
                         if (q < a.shard_keys) slot = static_cast<uint32_t>(key - q * a.nshards) * a.shard_slots + static_cast<uint32_t>(q);
                         else atomicOr(a.shard_err, 2u); // (a key outside the declared key space: the record is dropped, the step fails)
-                    } else if (a.nshards) slot = static_cast<uint32_t>(P::key(tup, prm) % a.nshards); // keyby across GPUs: the "slot" is the destination
+                    } else if (a.nshards) slot = static_cast<uint32_t>(key_word0(key_words<P>(tup, prm)) % a.nshards); // keyby across GPUs: the "slot" is the destination
                     else {
                         if (a.ext_slots != nullptr) { slot = a.ext_slots[m.tile * TILE + ctid]; if (slot >= a.ff.max_keys) slot = INVALID_SLOT; }
-                        else slot = slot_of_key(a.ff, P::key(tup, prm));
+                        else slot = slot_of_key(a.ff, key_words<P>(tup, prm));
                         if (slot != INVALID_SLOT && a.count_keys) atomicAdd(&a.ff.seg_cnt[slot], 1u); // (full-sort path only)
                     }
                     if (a.wide_h16 != nullptr) { // digit counts of this wide tile (the CTA owns all of its tiles)
@@ -912,7 +967,7 @@ __global__ void __launch_bounds__(256) k_slots_inplace(const TileArgs a, const t
             if (a.ext_slots != nullptr) { slot = a.ext_slots[p]; if (slot >= a.ff.max_keys) slot = INVALID_SLOT; }
             else {
                 const T *rec = reinterpret_cast<const T *>(b.tuples + static_cast<size_t>(local) * sizeof(T));
-                slot = slot_of_key(a.ff, P::key(*rec, prm));
+                slot = slot_of_key(a.ff, key_words<P>(*rec, prm));
             }
             if (slot != INVALID_SLOT && a.count_keys) atomicAdd(&a.ff.seg_cnt[slot], 1u);
         }
@@ -1584,7 +1639,7 @@ __device__ __forceinline__ uint32_t level_off(uint32_t n_leaves, uint32_t level)
 __device__ __forceinline__ uint64_t batch_watermark(const uint32_t *__restrict__ batch_off, const DevBatch *__restrict__ batches,
                                                     uint32_t nbatches, uint32_t pos);
 template <class P>
-__device__ __forceinline__ void ffat_eval_window(const FfatDev &ff, const unsigned char *tree, uint64_t key, uint64_t gwid, uint64_t wm,
+__device__ __forceinline__ void ffat_eval_window(const FfatDev &ff, const unsigned char *tree, key_words_t<P> key, uint64_t gwid, uint64_t wm,
                                                  uint32_t opos, unsigned char *__restrict__ out_res, uint64_t *__restrict__ out_ts,
                                                  uint32_t out_cap, const typename P::params_t &prm);
 
@@ -1614,12 +1669,13 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
             m = 0;
         }
         const bool act = m > 0;
-        uint32_t off = 0; uint64_t c = 0, key = 0, g = 0, trig = 0;
+        uint32_t off = 0; uint64_t c = 0, g = 0, trig = 0;
+        key_words_t<P> key{};
         alignas(16) R acc;
         unsigned char *tree = ff.tree + static_cast<size_t>(slot) * tree_stride;
         if (act) {
             off = ff.seg_off[slot]; c = ff.cnt[slot];
-            key = key_of_slot(ff, slot);
+            key = key_of_slot<P>(ff, slot);
             if (c % P_ != 0) ld_rec<R>(ff.acc + static_cast<size_t>(slot) * RB, acc);
             g = (c < ff.B) ? 0 : 1 + (c - ff.B) / group_items;
             trig = ff.B + g * group_items;
@@ -1667,7 +1723,7 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
                     bool deferred = (m - j) < ff.defer_items; // the panes this key still completes in this segment fit the spare ring leaves
                     if (deferred) {
                         const uint32_t ti = atomicAdd(ff.n_trig, 1u);
-                        if (ti < ff.trig_cap) { Trigger tr; tr.key = key; tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
+                        if (ti < ff.trig_cap) { Trigger tr; tr.key = trig_word(key); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
                         else deferred = false;
                     }
                     if (!deferred) {
@@ -2054,7 +2110,7 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                             bool deferred = (kleft[k] - consumed) < ff.defer_items; // the panes this key still completes in this segment fit the spare ring leaves
                             if (deferred) {
                                 const uint32_t ti = atomicAdd(ff.n_trig, 1u);
-                                if (ti < ff.trig_cap) { Trigger tr; tr.key = key_of_slot(ff, slot); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
+                                if (ti < ff.trig_cap) { Trigger tr; tr.key = trig_word(key_of_slot<P>(ff, slot)); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
                                 else deferred = false;
                             }
                             if (!deferred) { eval_now = true; ev_obase = obase; ev_pos = last_pos; ev_g = g; }
@@ -2068,7 +2124,8 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                     const int src = __ffs(pend) - 1;
                     pend &= pend - 1;
                     const uint32_t e_slot = key_lo + (warp << 5) + src, e_obase = __shfl_sync(FULL, ev_obase, src), e_pos = __shfl_sync(FULL, ev_pos, src);
-                    const uint64_t e_key = key_of_slot(ff, e_slot), e_g = __shfl_sync(FULL, ev_g, src);
+                    const key_words_t<P> e_key = key_of_slot<P>(ff, e_slot);
+                    const uint64_t e_g = __shfl_sync(FULL, ev_g, src);
                     const unsigned char *e_tree = ff.tree + static_cast<size_t>(e_slot) * tree_stride;
                     const uint64_t wm = batch_watermark(batch_off, batches, nbatches, e_pos);
                     for (uint32_t i = lane; i < ff.nb; i += 32)
@@ -2140,12 +2197,12 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                                     if (lane == 0) ti = atomicAdd(ff.n_trig, 1u);
                                     ti = __shfl_sync(FULL, ti, 0);
                                     if (ti < ff.trig_cap) {
-                                        if (lane == 0) { Trigger tr; tr.key = key_of_slot(ff, slot); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
+                                        if (lane == 0) { Trigger tr; tr.key = trig_word(key_of_slot<P>(ff, slot)); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
                                     } else deferred = false;
                                 }
                                 if (!deferred) {
                                     const uint64_t wm = batch_watermark(batch_off, batches, nbatches, last_pos);
-                                    const uint64_t key = key_of_slot(ff, slot);
+                                    const key_words_t<P> key = key_of_slot<P>(ff, slot);
                                     for (uint32_t i = lane; i < ff.nb; i += 32)
                                         ffat_eval_window<P>(ff, tree, key, g * ff.nb + i, wm, obase + i, out_res, out_ts, out_cap, prm);
                                 }
@@ -2294,7 +2351,7 @@ __global__ void __launch_bounds__(ST_THREADS, WFB_ST_MINBLOCKS) k_ffat_update_st
     if (b0 == b1) return;
 
     // the whole warp evaluates the Nb windows of one fired group
-    auto eval_group = [&](uint32_t e_slot, uint64_t e_key, uint64_t e_g, uint32_t e_pos, uint32_t e_obase) {
+    auto eval_group = [&](uint32_t e_slot, key_words_t<P> e_key, uint64_t e_g, uint32_t e_pos, uint32_t e_obase) {
         const unsigned char *e_tree = ff.tree + static_cast<size_t>(e_slot) * tree_stride;
         const uint64_t wm = batch_watermark(batch_off, batches, nbatches, e_pos);
         for (uint32_t i = lane; i < ff.nb; i += 32)
@@ -2344,7 +2401,7 @@ __global__ void __launch_bounds__(ST_THREADS, WFB_ST_MINBLOCKS) k_ffat_update_st
             ev &= ev - 1;
             const uint32_t ti = __shfl_sync(FULL, pend, src);
             const Trigger tr = ff.trig[ti];
-            eval_group(tr.slot, tr.key, tr.g, tr.last_pos, tr.obase);
+            eval_group(tr.slot, trig_key<P>(ff, tr), tr.g, tr.last_pos, tr.obase);
             if (lane == static_cast<uint32_t>(src)) { ff.trig[ti].slot = INVALID_SLOT; pend = ST_NONE; } // k_ffat_windows skips voided entries
             __syncwarp();
         }
@@ -2370,7 +2427,7 @@ __global__ void __launch_bounds__(ST_THREADS, WFB_ST_MINBLOCKS) k_ffat_update_st
                 const uint32_t obase = atomicAdd(n_out, ff.nb);
                 const uint32_t ti = atomicAdd(ff.n_trig, 1u);
                 if (ti < ff.trig_cap) {
-                    Trigger tr; tr.key = key_of_slot(ff, my_slot); tr.g = g; tr.slot = my_slot; tr.last_pos = it_pos; tr.obase = obase; tr.pad = 0;
+                    Trigger tr; tr.key = trig_word(key_of_slot<P>(ff, my_slot)); tr.g = g; tr.slot = my_slot; tr.last_pos = it_pos; tr.obase = obase; tr.pad = 0;
                     ff.trig[ti] = tr;
                     pend = ti;
                 } else { eval_now = true; ev_obase = obase; ev_g = g; } // list full: evaluate here
@@ -2385,7 +2442,7 @@ __global__ void __launch_bounds__(ST_THREADS, WFB_ST_MINBLOCKS) k_ffat_update_st
             const uint64_t e_g = __shfl_sync(FULL, ev_g, src);
             const uint32_t e_slot = key_lo + warp * 32u + static_cast<uint32_t>(src);
             __syncwarp(); // the path nodes the source lane has just written
-            eval_group(e_slot, key_of_slot(ff, e_slot), e_g, e_pos, e_obase);
+            eval_group(e_slot, key_of_slot<P>(ff, e_slot), e_g, e_pos, e_obase);
             __syncwarp();
         }
     };
@@ -2478,14 +2535,14 @@ __device__ __forceinline__ uint64_t batch_watermark(const uint32_t *__restrict__
 // one window: result_t(key, gwid) folded left to right over the largest aligned FlatFAT nodes covering panes
 // [gwid*sp, gwid*sp + wp) of the key's ring (the walk of Compute_Results_Kernel, wf/flatfat_gpu.hpp:109-136)
 template <class P>
-__device__ __forceinline__ void ffat_eval_window(const FfatDev &ff, const unsigned char *tree, uint64_t key, uint64_t gwid, uint64_t wm,
+__device__ __forceinline__ void ffat_eval_window(const FfatDev &ff, const unsigned char *tree, key_words_t<P> key, uint64_t gwid, uint64_t wm,
                                                  uint32_t opos, unsigned char *__restrict__ out_res, uint64_t *__restrict__ out_ts,
                                                  uint32_t out_cap, const typename P::params_t &prm)
 {
     using R = typename P::result_t;
     constexpr uint32_t RB = sizeof(R);
     const uint32_t n = ff.n_leaves;
-    alignas(16) R res = P::make_result(key, gwid, prm);
+    alignas(16) R res = P::make_result(key_codec<P>::decode(key), gwid, prm);
     uint32_t ws = static_cast<uint32_t>((gwid * ff.sp) & (n - 1));
     uint32_t remaining = ff.wp;
     if (ff.lazy) { // only the leaves are kept in global memory: fold them in order (the rare in-kernel evaluations; the deferred groups go
@@ -2536,7 +2593,7 @@ __global__ void __launch_bounds__(256) k_ffat_windows(const FfatDev ff, const ui
         const Trigger tr = ff.trig[ti];
         if (tr.slot == INVALID_SLOT) continue; // evaluated inside the update kernel (k_ffat_update_stream)
         const uint64_t wm = batch_watermark(batch_off, batches, nbatches, tr.last_pos);
-        ffat_eval_window<P>(ff, ff.tree + static_cast<size_t>(tr.slot) * tree_stride, tr.key, tr.g * ff.nb + i, wm, tr.obase + i,
+        ffat_eval_window<P>(ff, ff.tree + static_cast<size_t>(tr.slot) * tree_stride, trig_key<P>(ff, tr), tr.g * ff.nb + i, wm, tr.obase + i,
                             out_res, out_ts, out_cap, prm);
     }
 }
@@ -2584,7 +2641,7 @@ __global__ void __launch_bounds__(128) k_ffat_windows_lazy(const FfatDev ff, con
         }
         const uint64_t wm = batch_watermark(batch_off, batches, nbatches, tr.last_pos);
         for (uint32_t i = lane; i < ff.nb; i += 32)
-            ffat_eval_window<P>(fs, t, tr.key, tr.g * ff.nb + i, wm, tr.obase + i, out_res, out_ts, out_cap, prm);
+            ffat_eval_window<P>(fs, t, trig_key<P>(ff, tr), tr.g * ff.nb + i, wm, tr.obase + i, out_res, out_ts, out_cap, prm);
         __syncwarp(); // the next group overwrites the on-chip tree
     }
 }
@@ -2616,7 +2673,7 @@ __global__ void __launch_bounds__(256) k_ffat_update(const FfatDev ff, const uns
         if (m == 0) continue;
         const uint32_t off = ff.seg_off[slot];
         uint64_t c = ff.cnt[slot];
-        const uint64_t key = key_of_slot(ff, slot);
+        const key_words_t<P> key = key_of_slot<P>(ff, slot);
         unsigned char *tree = ff.tree + static_cast<size_t>(slot) * tree_stride;
         alignas(16) R acc;
         if (c % P_ != 0) ld_rec<R>(ff.acc + static_cast<size_t>(slot) * RB, acc); // every lane keeps a copy
@@ -2679,7 +2736,7 @@ __global__ void __launch_bounds__(256) k_ffat_update(const FfatDev ff, const uns
                         if (lane == 0) ti = atomicAdd(ff.n_trig, 1u);
                         ti = __shfl_sync(FULL, ti, 0);
                         if (ti < ff.trig_cap) {
-                            if (lane == 0) { Trigger tr; tr.key = key; tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
+                            if (lane == 0) { Trigger tr; tr.key = trig_word(key); tr.g = g; tr.slot = slot; tr.last_pos = last_pos; tr.obase = obase; tr.pad = 0; ff.trig[ti] = tr; }
                         } else deferred = false;
                     }
                     if (!deferred) {
@@ -2712,7 +2769,7 @@ __global__ void k_extract_keys(const unsigned char *__restrict__ tuples, uint32_
     using T = typename P::tuple_t;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const T *t = reinterpret_cast<const T *>(tuples + static_cast<size_t>(i) * sizeof(T));
-        const uint64_t k = P::key(*t, prm);
+        const uint64_t k = key_word0(key_words<P>(*t, prm)); // (integer keys: other key types go through k_key_order_words)
         if (keys) keys[i] = k;
         if (dest) dest[i] = static_cast<uint32_t>(k % num_shards); // wf/keyby_emitter.hpp:215-217
     }
@@ -2810,7 +2867,58 @@ __global__ void k_extract_keys_batches(const DevBatch *__restrict__ batches, con
     for (uint32_t gi = blockIdx.x * blockDim.x + threadIdx.x; gi < total; gi += gridDim.x * blockDim.x) {
         const uint32_t b = batch_of(boff, nb, gi);
         const T *t = reinterpret_cast<const T *>(batches[b].tuples + static_cast<size_t>(gi - boff[b]) * sizeof(T));
-        keys[gi] = (key_bits >= 64 ? 0ull : (static_cast<uint64_t>(b) << key_bits)) | (P::key(*t, prm) & mask);
+        keys[gi] = (key_bits >= 64 ? 0ull : (static_cast<uint64_t>(b) << key_bits)) | (key_word0(key_words<P>(*t, prm)) & mask);
+    }
+}
+
+// ---- Reduce_GPU over keys that are not integers: the keys are first replaced by their dense rank in the sort order ----------------
+// lo[gi] / hi[gi] = the order words (KeyCodec::order) of element gi's key; hi only for two-word keys. `tuples` is the one batch when
+// `batches` is null.
+template <class P>
+__global__ void k_key_order_words(const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff, uint32_t nb,
+                                  const unsigned char *__restrict__ tuples, uint32_t total, uint64_t *__restrict__ lo, uint64_t *__restrict__ hi,
+                                  const typename P::params_t prm)
+{
+    using T = typename P::tuple_t;
+    for (uint32_t gi = blockIdx.x * blockDim.x + threadIdx.x; gi < total; gi += gridDim.x * blockDim.x) {
+        const unsigned char *src = tuples + static_cast<size_t>(gi) * sizeof(T);
+        if (batches != nullptr) { const uint32_t b = batch_of(boff, nb, gi); src = batches[b].tuples + static_cast<size_t>(gi - boff[b]) * sizeof(T); }
+        const key_words_t<P> w = key_codec<P>::order(key_words<P>(*reinterpret_cast<const T *>(src), prm));
+        if constexpr (key_codec<P>::words == 2) { lo[gi] = w.lo; hi[gi] = w.hi; } else lo[gi] = w;
+    }
+}
+
+// out[i] = in[perm[i]]
+static __global__ void k_gather_u64(const uint64_t *__restrict__ in, const uint32_t *__restrict__ perm, uint32_t n, uint64_t *__restrict__ out)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = in[perm[i]];
+}
+// out[i] = a[b[i]]
+static __global__ void k_compose_perm(const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, uint32_t n, uint32_t *__restrict__ out)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = a[b[i]];
+}
+// head[i] = 1 when sorted position i (element perm[i]) has other order words than its predecessor (hi may be null: one word)
+__device__ __forceinline__ bool rank_head(const uint64_t *__restrict__ lo, const uint64_t *__restrict__ hi, const uint32_t *__restrict__ perm, uint32_t i)
+{
+    if (i == 0) return true;
+    const uint32_t a = perm[i], b = perm[i - 1];
+    return lo[a] != lo[b] || (hi != nullptr && hi[a] != hi[b]);
+}
+static __global__ void k_rank_heads(const uint64_t *__restrict__ lo, const uint64_t *__restrict__ hi, const uint32_t *__restrict__ perm, uint32_t n,
+                                    uint32_t *__restrict__ head)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) head[i] = rank_head(lo, hi, perm, i) ? 1u : 0u;
+}
+// after the exclusive scan of head[]: keys[e] = (batch of e << 32) | dense rank of e's key (boff null: the rank alone)
+static __global__ void k_rank_scatter(const uint64_t *__restrict__ lo, const uint64_t *__restrict__ hi, const uint32_t *__restrict__ perm,
+                                      const uint32_t *__restrict__ head_scan, uint32_t n, const uint32_t *__restrict__ boff, uint32_t nb,
+                                      uint64_t *__restrict__ keys)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t e = perm[i];
+        const uint64_t rank = head_scan[i] - (rank_head(lo, hi, perm, i) ? 0u : 1u);
+        keys[e] = (boff != nullptr ? (static_cast<uint64_t>(batch_of(boff, nb, e)) << 32) : 0ull) | rank;
     }
 }
 
@@ -3016,7 +3124,7 @@ __global__ void k_tb_lift(const unsigned char *__restrict__ tuples, const uint64
             alignas(16) R r;
             P::lift(t, r, prm);
             st_rec<R>(lifted + static_cast<size_t>(i) * sizeof(R), r);
-            const uint32_t slot = slot_of_key(ff, P::key(t, prm));
+            const uint32_t slot = slot_of_key(ff, key_words<P>(t, prm));
             const uint64_t pane = ts[i] / tb.pane_len;                 // Lifting_Kernel_TB_Keyed :164
             if (pane < first_incomplete) atomicAdd(tb.ignored, 1u);    // :165-167
             if (slot != INVALID_SLOT) { // raw key: slot, pane relative to the key's first pending pane (0xffffffff: older = late)
@@ -3103,7 +3211,7 @@ __global__ void k_tb_merge(const uint64_t *__restrict__ skeys, const uint32_t *_
                         const uint64_t ckp = skeys[seg_begin[k - 1]];
                         if ((ckp >> tb.kbits) == slot && first_id + (ckp & relmask) + 1 > lower) lower = first_id + (ckp & relmask) + 1;
                     }
-                    const uint64_t key = key_of_slot(ff, slot);
+                    const typename P::key_t key = key_codec<P>::decode(key_of_slot<P>(ff, slot));
                     for (uint64_t m = lower; m < pane; m++) {
                         alignas(16) R e = P::make_result(key, 0, prm);
                         st_rec<R>(ring + (m % tb.capq) * sizeof(R), e);
@@ -3189,7 +3297,7 @@ __global__ void k_tb_pop_write(const FfatDev ff, const TbDev tb, uint64_t first_
         uint64_t trig = tb.trig[slot], first_id = tb.first[slot];
         uint32_t num = tb.num_new[slot];
         bool done = tb.done[slot] != 0;
-        const uint64_t key = key_of_slot(ff, slot);
+        const typename P::key_t key = key_codec<P>::decode(key_of_slot<P>(ff, slot));
         const unsigned char *ring = tb.ring + static_cast<size_t>(slot) * tb.capq * sizeof(R);
         uint32_t w = offs[i];
         while (trig < first_incomplete) {
@@ -3221,7 +3329,7 @@ __global__ void k_ks_slots(const DevBatch *__restrict__ batches, const uint32_t 
     for (uint32_t gi = blockIdx.x * blockDim.x + threadIdx.x; gi < total; gi += gridDim.x * blockDim.x) {
         const uint32_t b = batch_of(boff, nb, gi);
         const T *t = reinterpret_cast<const T *>(batches[b].tuples + static_cast<size_t>(gi - boff[b]) * sizeof(T));
-        slots[gi] = slot_of_key(ff, P::key(*t, prm));
+        slots[gi] = slot_of_key(ff, key_words<P>(*t, prm));
     }
 }
 

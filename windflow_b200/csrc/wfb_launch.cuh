@@ -113,6 +113,12 @@ struct ProgramOps {
                        const uint32_t *digit_counts, uint32_t shift, const uint32_t *batch_off, const DevBatch *batches,
                        uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts, uint32_t out_cap, uint32_t *n_out, cudaStream_t s,
                        const void *params);
+    // key_t (wfb_keys.cuh): bytes of its canonical words (8 or 16), KEY_KIND_* and sizeof(key_t) (the order words of a key that is not
+    // an integer have no bits above 8 * key_size: a float's fit in 32)
+    uint32_t key_bytes, key_kind, key_size;
+    // Reduce_GPU over keys that are not integers: the order words of every element (k_key_order_words; batches null: `tuples` is the batch)
+    int (*key_order_words)(const DevBatch *batches, const uint32_t *boff, uint32_t nb, const unsigned char *tuples, uint32_t total, uint64_t *lo,
+                           uint64_t *hi, cudaStream_t s, const void *params);
 };
 
 // P::passthrough (optional): map is a no-op and lift the identity (tuple_t == result_t)
@@ -326,6 +332,14 @@ int extract_keys_batches_dispatch(const DevBatch *batches, const uint32_t *boff,
     return 0;
 }
 template <class P>
+int key_order_words_dispatch(const DevBatch *batches, const uint32_t *boff, uint32_t nb, const unsigned char *tuples, uint32_t total, uint64_t *lo,
+                             uint64_t *hi, cudaStream_t s, const void *params)
+{
+    k_key_order_words<P><<<grid_for(total, 256), 256, 0, s>>>(batches, boff, nb, tuples, total, lo, hi, load_params<P>(params));
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+template <class P>
 int reduce_segments_batches_dispatch(const DevBatch *batches, const uint32_t *boff, const uint64_t *skeys, const uint32_t *sidx,
                                      const uint32_t *seg_begin, const uint32_t *first_seg, const uint32_t *n_segs, uint32_t key_bits,
                                      uint32_t total, uint32_t *long_list, uint32_t *n_long, cudaStream_t s, const void *params)
@@ -362,7 +376,7 @@ template <class P> struct program_has_result_key<P, std::void_t<decltype(P::resu
 
 template <class P>
 struct LiftedOf {
-    using tuple_t = typename P::result_t; using result_t = typename P::result_t; using key_t = uint64_t; using params_t = typename P::params_t;
+    using tuple_t = typename P::result_t; using result_t = typename P::result_t; using key_t = typename P::key_t; using params_t = typename P::params_t;
     static constexpr bool passthrough = true;
     static constexpr bool is_lifted = true;
     __host__ __device__ static void map(tuple_t &, const params_t &) {}
@@ -371,7 +385,7 @@ struct LiftedOf {
     // the time-based front end hands the slots over itself (TileArgs::ext_slots) and never asks
     __host__ __device__ static key_t key(const tuple_t &t, const params_t &p)
     {
-        if constexpr (program_has_result_key<P>::value) return P::result_key(t, p); else return 0;
+        if constexpr (program_has_result_key<P>::value) return P::result_key(t, p); else return key_t{};
     }
     __host__ __device__ static void lift(const tuple_t &t, result_t &r, const params_t &) { r = t; }
     __host__ __device__ static void comb(const result_t &a, const result_t &b, result_t &o, const params_t &p) { P::comb(a, b, o, p); }
@@ -399,6 +413,7 @@ const void *lifted_ops_of()
         t.tile_pass = &tile_pass_ingest_dispatch<L>; t.slots_inplace = &slots_inplace_dispatch<L>;
         t.ffat_update = &ffat_update_dispatch<L>; t.ffat_buckets = &ffat_buckets_dispatch<L>; t.ffat_windows = &ffat_windows_dispatch<L>;
         t.ffat_stream = &ffat_stream_dispatch<L>;
+        t.key_bytes = 8u * key_codec<L>::words; t.key_kind = key_codec<L>::kind; t.key_size = sizeof(typename L::key_t);
         t.reserved2 = program_has_result_key<P>::value ? 1u : 0u; // bit 0: the lifted records carry their key (usable behind an exchange)
         return t;
     }();
@@ -427,12 +442,14 @@ ProgramOps make_ops()
     o.tb_lift = &tb_lift_dispatch<P>; o.tb_reduce = &tb_reduce_dispatch<P>; o.tb_merge = &tb_merge_dispatch<P>; o.tb_pop_write = &tb_pop_write_dispatch<P>;
     o.extract_keys_batches = &extract_keys_batches_dispatch<P>;
     o.reduce_segments_batches = &reduce_segments_batches_dispatch<P>;
+    o.key_bytes = 8u * key_codec<P>::words; o.key_kind = key_codec<P>::kind; o.key_size = sizeof(typename P::key_t);
+    o.key_order_words = &key_order_words_dispatch<P>;
     if constexpr (program_is_lifted<P>::value) o.lifted_ops = nullptr; else o.lifted_ops = &lifted_ops_of<P>;
     return o;
 }
 
 
-// registers the launch table of program P with libwfb200 and returns its program id (>= 4), or a negative error
+// registers the launch table of program P with libwfb200 and returns its program id (>= 6), or a negative error
 template <class P>
 int register_program()
 {

@@ -40,7 +40,8 @@ std::mutex &registry_mutex() { static std::mutex m; return m; } // replicas of d
 
 std::vector<ProgramOps> &registry()
 {
-    static std::vector<ProgramOps> table; if (table.empty()) { table.reserve(4096); table = { make_ops<ProgTuple64>(), make_ops<ProgWfTest16>(), make_ops<ProgWfWin24>(), make_ops<ProgLifted32>() }; table.reserve(4096); }
+    static std::vector<ProgramOps> table; if (table.empty()) { table.reserve(4096); table = { make_ops<ProgTuple64>(), make_ops<ProgWfTest16>(), make_ops<ProgWfWin24>(), make_ops<ProgLifted32>(),
+                                                                 make_ops<ProgTuple64FKey>(), make_ops<ProgTuple64K16>() }; table.reserve(4096); }
     return table;
 }
 
@@ -394,6 +395,8 @@ struct wfb_engine {
     uint32_t *rb_off = nullptr, *rb_first = nullptr, *rb_total = nullptr; uint32_t rb_cap = 0;
     uint32_t *rb_long = nullptr; uint32_t rb_long_cap = 0; // segments folded by a warp; rb_total[1] = their number
     RadixSorter sorter;
+    // Reduce_GPU over keys that are not integers: the order words of the keys (whi: two-word keys) and the permutation of the first sort
+    uint64_t *wlo = nullptr, *whi = nullptr; uint32_t *wperm = nullptr; uint32_t wcap = 0;
 
     int ensure_sort(uint32_t n, cudaStream_t s)
     {
@@ -408,13 +411,49 @@ struct wfb_engine {
         CK(cudaMalloc(&head, sizeof(uint32_t) * cap)); CK(cudaMalloc(&seg_begin, sizeof(uint32_t) * (static_cast<size_t>(cap) + 1)));
         return 0;
     }
-    // stable LSD radix sort of (keysA[i], i) by key over `key_bits` bits; returns the buffers holding the result
-    int sort64(uint32_t n, cudaStream_t s, const uint64_t **skeys, const uint32_t **sidx)
+    // stable LSD radix sort of (keysA[i], i) by key over `bits` bits; returns the buffers holding the result
+    int sort64(uint32_t n, uint32_t bits, cudaStream_t s, const uint64_t **skeys, const uint32_t **sidx)
     {
         const uint64_t before = sorter.launches;
-        int rc = sorter.sort<uint64_t>(keysA, keysB, idxA, idxB, nullptr, n, n, (key_bits + 7) / 8, s, skeys, sidx);
+        int rc = sorter.sort<uint64_t>(keysA, keysB, idxA, idxB, nullptr, n, n, (bits + 7) / 8, s, skeys, sidx);
         launches += sorter.launches - before;
         return rc;
+    }
+    // Keys that are not integers (after ensure_sort(n)): keysA[i] = (batch of i << 32) | dense rank of element i's key in the key order
+    // (the rank alone when boff is null), so that the integer path that follows sorts 32 (+ batch) bits. The order words are sorted
+    // LSD over the bits the key type has (8 * sizeof(key_t)), low word first, then the high word of a two-word key; equal neighbours
+    // share a rank. `tuples` is the batch when `batches` is null.
+    int rank_keys(const DevBatch *batches, const uint32_t *boff, uint32_t nb, const void *tuples, uint32_t n, cudaStream_t s)
+    {
+        const bool two = ops->key_bytes == 16;
+        const uint32_t bits = 8u * ops->key_size, lo_bits = std::min(bits, 64u), hi_bits = two ? bits - 64u : 0u;
+        if (n > wcap) {
+            CK(cudaStreamSynchronize(s));
+            cudaFree(wlo); cudaFree(whi); cudaFree(wperm); wlo = whi = nullptr; wperm = nullptr;
+            wcap = std::max(n, cap);
+            CK(cudaMalloc(&wlo, sizeof(uint64_t) * wcap));
+            if (two) { CK(cudaMalloc(&whi, sizeof(uint64_t) * wcap)); CK(cudaMalloc(&wperm, sizeof(uint32_t) * wcap)); }
+        }
+        int rc = ops->key_order_words(batches, boff, nb, static_cast<const unsigned char *>(tuples), n, wlo, whi, s, pp()); if (rc) return rc;
+        CK(cudaMemcpyAsync(keysA, wlo, sizeof(uint64_t) * n, cudaMemcpyDeviceToDevice, s));
+        const uint64_t *sk; const uint32_t *perm;
+        rc = sort64(n, lo_bits, s, &sk, &perm); if (rc) return rc;
+        const uint32_t g = grid_for(n, 256);
+        if (two) { // sort the high words in the order of the low words, then compose the two permutations
+            CK(cudaMemcpyAsync(wperm, perm, sizeof(uint32_t) * n, cudaMemcpyDeviceToDevice, s));
+            k_gather_u64<<<g, 256, 0, s>>>(whi, wperm, n, keysA);
+            const uint32_t *p2;
+            rc = sort64(n, hi_bits, s, &sk, &p2); if (rc) return rc;
+            k_compose_perm<<<g, 256, 0, s>>>(wperm, p2, n, destA);
+            perm = destA;
+            launches += 2;
+        }
+        k_rank_heads<<<g, 256, 0, s>>>(wlo, whi, perm, n, head);
+        k_scan_u32<<<1, 1024, 0, s>>>(head, head, n, nullptr);
+        k_rank_scatter<<<g, 256, 0, s>>>(wlo, whi, perm, head, n, boff, nb, keysA);
+        CK(cudaGetLastError());
+        launches += 4;
+        return 0;
     }
     void free_sort()
     {
@@ -422,6 +461,7 @@ struct wfb_engine {
         cudaFree(head); cudaFree(seg_begin);
         cudaFree(sh_lifted); cudaFree(sh_dest); cudaFree(sh_ctl);
         cudaFree(rb_off); cudaFree(rb_first); cudaFree(rb_total); cudaFree(rb_long);
+        cudaFree(wlo); cudaFree(whi); cudaFree(wperm);
         sorter.destroy();
     }
 };
@@ -560,7 +600,7 @@ int wfb_program_info(int prog, wfb_program_info_t *info)
     const ProgramOps *o = program(prog);
     if (!o) return WFB_E_NOPROG;
     if (!info) return WFB_E_BADARG;
-    info->tuple_bytes = o->tuple_bytes; info->result_bytes = o->result_bytes; info->key_bytes = 8; info->reserved = 0;
+    info->tuple_bytes = o->tuple_bytes; info->result_bytes = o->result_bytes; info->key_bytes = o->key_bytes; info->key_kind = o->key_kind;
     return 0;
 }
 
@@ -674,7 +714,7 @@ int wfb_map_filter_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_b
 
 int wfb_engine_set_key_bits(wfb_engine_t *e, uint32_t bits)
 {
-    if (!e || bits == 0 || bits > 64) return WFB_E_BADARG;
+    if (!e || bits == 0 || bits > 64 || e->ops->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG;
     e->key_bits = bits;
     return 0;
 }
@@ -685,10 +725,12 @@ static int keyed_prepare(wfb_engine_t *e, const void *tuples, uint32_t n, int32_
 {
     int rc = e->ts.enter(s); if (rc) return rc;
     rc = e->ensure_sort(n, s); if (rc) return rc;
-    rc = e->ops->extract_keys(static_cast<const unsigned char *>(tuples), n, e->keysA, nullptr, 1, s, e->pp()); if (rc) return rc;
-    e->launches++;
+    const bool ranked = e->ops->key_kind != KEY_KIND_INTEGRAL; // (reduce_by_key only: keyby_group refuses such keys)
+    if (ranked) rc = e->rank_keys(nullptr, nullptr, 1, tuples, n, s);
+    else { rc = e->ops->extract_keys(static_cast<const unsigned char *>(tuples), n, e->keysA, nullptr, 1, s, e->pp()); e->launches++; }
+    if (rc) return rc;
     const uint64_t *skeys; const uint32_t *sidx;
-    rc = e->sort64(n, s, &skeys, &sidx); if (rc) return rc;
+    rc = e->sort64(n, ranked ? 32u : e->key_bits, s, &skeys, &sidx); if (rc) return rc;
     const uint32_t g = grid_for(n, 256);
     k_seg_heads<<<g, 256, 0, s>>>(skeys, sidx, n, e->head, map_idxs);
     k_scan_u32<<<1, 1024, 0, s>>>(e->head, e->head, n, nullptr);
@@ -721,7 +763,9 @@ int wfb_reduce_by_key_batches(wfb_engine_t *e, const wfb_batch_t *in_h, const wf
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (nbatches == 0) return 0;
     uint32_t bbits = 0; while ((1ull << bbits) < nbatches) bbits++;
-    if (e->key_bits + bbits > 64) return WFB_E_BADARG;
+    const bool ranked = e->ops->key_kind != KEY_KIND_INTEGRAL; // keys replaced by their 32-bit rank (wfb_engine::rank_keys)
+    const uint32_t key_bits = ranked ? 32u : e->key_bits;
+    if (key_bits + bbits > 64) return WFB_E_BADARG;
     int rc = e->ts.enter(s); if (rc) return rc;
     CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t) * nbatches, s));
     std::vector<DevBatch> hb(nbatches);
@@ -760,11 +804,13 @@ int wfb_reduce_by_key_batches(wfb_engine_t *e, const wfb_batch_t *in_h, const wf
         e->rb_long_cap = std::max(n / RB_LONG + 1, 2 * e->rb_long_cap);
         CK(cudaMalloc(&e->rb_long, sizeof(uint32_t) * e->rb_long_cap));
     }
-    const uint32_t kb = nbatches == 1 ? 64u : e->key_bits; // a single batch needs no composite key
-    rc = e->ops->extract_keys_batches(e->ts.d_batches, e->rb_off, nbatches, n, kb, e->keysA, s, e->pp()); if (rc) return rc;
+    const uint32_t kb = nbatches == 1 ? 64u : key_bits; // a single batch needs no composite key
+    if (ranked) rc = e->rank_keys(e->ts.d_batches, e->rb_off, nbatches, nullptr, n, s);
+    else rc = e->ops->extract_keys_batches(e->ts.d_batches, e->rb_off, nbatches, n, kb, e->keysA, s, e->pp());
+    if (rc) return rc;
     const uint64_t *skeys; const uint32_t *sidx;
     const uint64_t before = e->sorter.launches;
-    const uint32_t sort_bits = nbatches == 1 ? e->key_bits : e->key_bits + bbits;
+    const uint32_t sort_bits = nbatches == 1 ? key_bits : key_bits + bbits;
     rc = e->sorter.sort<uint64_t>(e->keysA, e->keysB, e->idxA, e->idxB, nullptr, n, n, (sort_bits + 7) / 8, s, &skeys, &sidx); if (rc) return rc;
     const uint32_t tiles = (n + SEGT - 1) / SEGT;
     k_head_tile_counts<<<tiles, 256, 0, s>>>(skeys, n, e->head);
@@ -794,6 +840,7 @@ int wfb_keyby_group(wfb_engine_t *e, const void *tuples, uint32_t n, int32_t *st
                     uint32_t *n_keys_dev, void *stream)
 {
     if (!e || !n_keys_dev || (n && (!tuples || !start_idxs || !map_idxs || !dist_keys))) return WFB_E_BADARG;
+    if (e->ops->key_kind != KEY_KIND_INTEGRAL) return WFB_E_UNSUPPORTED; // dist_keys holds 8-byte integer keys
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (n == 0) { CK(cudaMemsetAsync(n_keys_dev, 0, sizeof(uint32_t), s)); return 0; }
     const uint32_t *sidx;
@@ -804,6 +851,7 @@ int wfb_shard_by_key(wfb_engine_t *e, const void *tuples, const uint64_t *ts, ui
                      void *out_tuples, uint64_t *out_ts, uint32_t *seg_off_dev, void *stream)
 {
     if (!e || !seg_off_dev || num_shards == 0 || num_shards > 256 || (n && (!tuples || !out_tuples))) return WFB_E_BADARG;
+    if (e->ops->key_kind != KEY_KIND_INTEGRAL) return WFB_E_UNSUPPORTED; // shard = key % num_shards
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (n == 0) { CK(cudaMemsetAsync(seg_off_dev, 0, sizeof(uint32_t) * (num_shards + 1), s)); return 0; }
     int rc = e->ts.enter(s); if (rc) return rc;
@@ -843,6 +891,7 @@ static int shard_lift_impl(wfb_engine_t *e, const wfb_functors_t *pre, const wfb
     // Map -> Filter -> lift in one streaming pass (no compaction chain: tile t owns positions [t*TILE, +TILE)), then one
     // stable partition pass on the destination (key % num_shards) that moves the lifted records into the shard regions.
     if (!e || !counts_dev || !out_regions || num_shards == 0 || num_shards > MAX_SHARDS || (nbatches && !batches_h)) return WFB_E_BADARG;
+    if (e->ops->key_kind != KEY_KIND_INTEGRAL) return WFB_E_UNSUPPORTED; // shard = key % num_shards
     const bool bucketed = shard_slots != 0;
     if (bucketed && (!out_slots || !bins_ctl || (shard_slots & (shard_slots - 1)) || static_cast<uint64_t>(num_shards) * shard_slots > 65536u ||
                      shard_keys > shard_slots || (shard_slots >> shift) == 0)) return WFB_E_BADARG;
@@ -946,6 +995,7 @@ int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t f
     const ProgramOps *o = program(prog);
     if (!o) return WFB_E_NOPROG;
     if (o->state_bytes == 0) return WFB_E_UNSUPPORTED; // the program has no state_t / stateful functors
+    if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
     uint32_t bits = 0; while ((1ull << bits) < max_keys) bits++;
     if (bits > OSW_BITS + 6) return WFB_E_UNSUPPORTED;  // 1024 buckets of at most 64 keys
     int rc = device_ready(); if (rc) return rc;
@@ -958,12 +1008,12 @@ int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t f
     ff.ht_mask = cap - 1;
 #define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc(reinterpret_cast<void **>(&(ptr)), (bytes)); if (e_ != cudaSuccess) { wfb_kstate_destroy(h); return static_cast<int>(e_); } } while (0)
     if (!ff.dense) {
-        ALLOC(ff.ht_keys, sizeof(uint64_t) * cap); ALLOC(ff.ht_slots, sizeof(uint32_t) * cap);
-        CK(cudaMemset(ff.ht_keys, 0xff, sizeof(uint64_t) * cap)); CK(cudaMemset(ff.ht_slots, 0xff, sizeof(uint32_t) * cap));
+        ALLOC(ff.ht_keys, static_cast<size_t>(o->key_bytes) * cap); ALLOC(ff.ht_slots, sizeof(uint32_t) * cap);
+        CK(cudaMemset(ff.ht_keys, 0xff, static_cast<size_t>(o->key_bytes) * cap)); CK(cudaMemset(ff.ht_slots, 0xff, sizeof(uint32_t) * cap));
     }
     ALLOC(ff.n_slots, sizeof(uint32_t) * 4); ff.err_flags = ff.n_slots + 1;
     CK(cudaMemset(ff.n_slots, 0, sizeof(uint32_t) * 4));
-    ALLOC(ff.slot_key, sizeof(uint64_t) * max_keys);
+    ALLOC(ff.slot_key, static_cast<size_t>(o->key_bytes) * max_keys);
     ALLOC(h->states, static_cast<size_t>(o->state_bytes) * max_keys);
     CK(cudaMemset(h->states, 0, static_cast<size_t>(o->state_bytes) * max_keys)); // state_t(): zero-initialised
 #undef ALLOC
@@ -1086,6 +1136,7 @@ static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, ui
     if (!o) return WFB_E_NOPROG;
     const int lp = lifted_program_of(prog);
     if (lp < 0 || (flags & WFB_FFAT_PIPELINED)) return WFB_E_UNSUPPORTED;
+    if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
     int rc = device_ready(); if (rc) return rc;
     const uint64_t pane_len = gcd_u64(win, slide);                   // wf/ffat_replica_gpu.hpp:639-642
     const uint64_t win_p = win / pane_len, slide_p = slide / pane_len;
@@ -1103,16 +1154,16 @@ static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, ui
     size_t total = 0;
 #define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc(reinterpret_cast<void **>(&(ptr)), (bytes)); if (e_ != cudaSuccess) { wfb_ffat_destroy(h); return static_cast<int>(e_); } total += (bytes); } while (0)
     if (!ff.dense) {
-        ALLOC(ff.ht_keys, sizeof(uint64_t) * cap);
+        ALLOC(ff.ht_keys, static_cast<size_t>(o->key_bytes) * cap);
         ALLOC(ff.ht_slots, sizeof(uint32_t) * cap);
-        CK(cudaMemset(ff.ht_keys, 0xff, sizeof(uint64_t) * cap));
+        CK(cudaMemset(ff.ht_keys, 0xff, static_cast<size_t>(o->key_bytes) * cap));
         CK(cudaMemset(ff.ht_slots, 0xff, sizeof(uint32_t) * cap));
     }
     ALLOC(ff.n_slots, sizeof(uint32_t) * 4);
     h->own_n_slots = ff.n_slots;
     ff.err_flags = ff.n_slots + 1;
     CK(cudaMemset(ff.n_slots, 0, sizeof(uint32_t) * 4));
-    ALLOC(ff.slot_key, sizeof(uint64_t) * max_keys);
+    ALLOC(ff.slot_key, static_cast<size_t>(o->key_bytes) * max_keys);
     TbDev &tb = h->tb;
     tb.pane_len = pane_len; tb.Bp = Bp; tb.group = group; tb.capq = static_cast<uint32_t>(capq);
     ALLOC(tb.first, sizeof(uint64_t) * max_keys); CK(cudaMemset(tb.first, 0, sizeof(uint64_t) * max_keys));
@@ -1254,6 +1305,7 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
     if (win_type != 0) return WFB_E_UNSUPPORTED;
     const ProgramOps *o = program(prog);
     if (!o) return WFB_E_NOPROG;
+    if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
     int rc = device_ready(); if (rc) return rc;
     wfb_ffat *h = new (std::nothrow) wfb_ffat();
     if (!h) return WFB_E_BADARG;
@@ -1283,9 +1335,9 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
     size_t total = 0;
 #define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc(reinterpret_cast<void **>(&(ptr)), (bytes)); if (e_ != cudaSuccess) { wfb_ffat_destroy(h); return static_cast<int>(e_); } total += (bytes); } while (0)
     if (!ff.dense) {
-        ALLOC(ff.ht_keys, sizeof(uint64_t) * cap);
+        ALLOC(ff.ht_keys, static_cast<size_t>(o->key_bytes) * cap);
         ALLOC(ff.ht_slots, sizeof(uint32_t) * cap);
-        CK(cudaMemset(ff.ht_keys, 0xff, sizeof(uint64_t) * cap));
+        CK(cudaMemset(ff.ht_keys, 0xff, static_cast<size_t>(o->key_bytes) * cap));
         CK(cudaMemset(ff.ht_slots, 0xff, sizeof(uint32_t) * cap));
     }
     ALLOC(ff.n_slots, sizeof(uint32_t) * 4);
@@ -1293,7 +1345,7 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
     ff.err_flags = ff.n_slots + 1;
     ff.results_total = reinterpret_cast<unsigned long long *>(ff.n_slots + 2);
     CK(cudaMemset(ff.n_slots, 0, sizeof(uint32_t) * 4));
-    ALLOC(ff.slot_key, sizeof(uint64_t) * max_keys);
+    ALLOC(ff.slot_key, static_cast<size_t>(o->key_bytes) * max_keys);
     ALLOC(ff.cnt, sizeof(uint64_t) * max_keys);
     CK(cudaMemset(ff.cnt, 0, sizeof(uint64_t) * max_keys));
     ALLOC(ff.acc, RB * max_keys);
@@ -1942,6 +1994,7 @@ int wfb_mg_create(wfb_mg_t **hh, int prog, int nranks, int rank, const void *id1
     if (!o) return WFB_E_NOPROG;
     const int lp = lifted_program_of(prog);
     if (lp < 0 || !(program(lp)->reserved2 & 1u)) return WFB_E_UNSUPPORTED; // the lifted records must carry their key (Program::result_key)
+    if (o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_UNSUPPORTED;            // shards are key % nranks: integer keys only
     int rc = device_ready(); if (rc) return rc;
     if (nranks > 1 && !nccl().ok) return WFB_E_UNSUPPORTED;
     wfb_mg *h = new (std::nothrow) wfb_mg();

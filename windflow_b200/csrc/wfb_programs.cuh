@@ -1,7 +1,9 @@
 // wfb_programs.cuh -- the built-in "programs": record schemas + functors compiled into libwfb200.so.
 //
 // A program is a traits struct with
-//   tuple_t, result_t, key_t (uint64_t), params_t (functor objects / parameters, passed by value to kernels)
+//   tuple_t, result_t, key_t, params_t (functor objects / parameters, passed by value to kernels)
+//   (key_t: an integral or enum type, float, double, or a trivially copyable type of at most 16 bytes without padding or
+//    floating-point members; wfb_keys.cuh maps it to the words the key table stores)
 //   map(tuple_t&, params)            Map_GPU functor      __host__ __device__ void(tuple_t &)           (API:50-52)
 //   filter(tuple_t&, params)->bool   Filter_GPU functor   __host__ __device__ bool(tuple_t &)           (API:34-36)
 //   key(const tuple_t&, params)->key_t       key extractor    __host__ __device__ key_t(const tuple_t &)    (API:213)
@@ -14,6 +16,7 @@
 // WFB_DEFINE_PROGRAM (wfb_kernels.cuh); see INTEGRATION.md.
 #pragma once
 #include <cstdint>
+#include <cstring>
 #include "../../include/wfb200.h"
 
 namespace wfb {
@@ -167,5 +170,46 @@ struct ProgLifted32 {
         tuple_t r; r.key = a.key; r.id = 0; r.isum = a.isum + b.isum; r.fsum = a.fsum + b.fsum; return r;
     }
 };
+
+// ---- programs 4 and 5: the bench stream keyed by a double / by a 16-byte struct -------------------------------------------------
+// The functors of ProgTuple64 over the same tuples; only the key extractor and the result record differ (and reduce keeps pad[0],
+// which holds part of the key).
+template <class K, class R, int ID>
+struct ProgTuple64Keyed {
+    using tuple_t = wfb_tuple64_t;
+    using result_t = R;
+    using key_t = K;
+    using params_t = wfb_functors_t;
+    using state_t = wfb_state8_t;
+    static constexpr int id = ID;
+    __host__ __device__ static void map(tuple_t &t, const params_t &p) { ProgTuple64::map(t, p); }
+    __host__ __device__ static bool filter(tuple_t &t, const params_t &p) { return ProgTuple64::filter(t, p); }
+    __host__ __device__ static key_t key(const tuple_t &t, const params_t &)
+    {
+        if constexpr (sizeof(K) == 8) { K k; std::memcpy(&k, &t.pad[0], sizeof(k)); return k; } // the double whose bits are pad[0]
+        else { K k; k.key = t.key; k.a = static_cast<uint32_t>(t.pad[0]); k.b = static_cast<uint32_t>(t.pad[0] >> 32); return k; }
+    }
+    __host__ __device__ static void lift(const tuple_t &t, result_t &r, const params_t &p)
+    {
+        r.key = key(t, p); r.id = 0; r.isum = t.ivalue; r.fsum = t.fvalue;
+    }
+    __host__ __device__ static void comb(const result_t &a, const result_t &b, result_t &out, const params_t &)
+    {
+        int64_t is = a.isum + b.isum; double fs = a.fsum + b.fsum;
+        out.isum = is; out.fsum = fs;
+    }
+    __host__ __device__ static result_t make_result(key_t k, uint64_t gwid, const params_t &)
+    {
+        result_t r{}; r.key = k; r.id = gwid; r.isum = 0; r.fsum = 0.0; return r;
+    }
+    __host__ __device__ static tuple_t reduce(const tuple_t &a, const tuple_t &b, const params_t &p)
+    {
+        tuple_t r = ProgTuple64::reduce(a, b, p); r.pad[0] = a.pad[0]; return r;
+    }
+    __host__ __device__ static void map_stateful(tuple_t &t, state_t &st, const params_t &p) { ProgTuple64::map_stateful(t, st, p); }
+    __host__ __device__ static bool filter_stateful(tuple_t &t, state_t &st, const params_t &p) { return ProgTuple64::filter_stateful(t, st, p); }
+};
+using ProgTuple64FKey = ProgTuple64Keyed<double, wfb_result32d_t, WFB_PROG_TUPLE64_FKEY>;
+using ProgTuple64K16 = ProgTuple64Keyed<wfb_key16_t, wfb_result48k_t, WFB_PROG_TUPLE64_K16>;
 
 } // namespace wfb

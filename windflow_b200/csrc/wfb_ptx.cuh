@@ -122,6 +122,24 @@ __device__ __forceinline__ void st_release_u32(uint32_t *p, uint32_t v)
 {
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+// one 16-byte load of two words (not guaranteed single-copy atomic: a concurrent 16-byte CAS may be seen half written)
+__device__ __forceinline__ void ld_relaxed_v2u64(const uint64_t *p, uint64_t &lo, uint64_t &hi)
+{
+    asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(lo), "=l"(hi) : "l"(p) : "memory");
+}
+// 16-byte compare-and-swap (sm_90): returns the words found at p
+__device__ __forceinline__ void atom_cas_b128(uint64_t *p, uint64_t cmp_lo, uint64_t cmp_hi, uint64_t val_lo, uint64_t val_hi,
+                                              uint64_t &old_lo, uint64_t &old_hi)
+{
+    asm volatile("{\n\t.reg .b128 c, v, d;\n\t"
+                 "mov.b128 c, {%2, %3};\n\t"
+                 "mov.b128 v, {%4, %5};\n\t"
+                 "atom.relaxed.gpu.global.cas.b128 d, [%6], c, v;\n\t"
+                 "mov.b128 {%0, %1}, d;\n\t}"
+                 : "=l"(old_lo), "=l"(old_hi)
+                 : "l"(cmp_lo), "l"(cmp_hi), "l"(val_lo), "l"(val_hi), "l"(p)
+                 : "memory");
+}
 
 // streaming (read-once) 128-bit global load / store
 __device__ __forceinline__ uint4 ld_stream_u4(const void *p)

@@ -17,14 +17,21 @@ from ._lib import WfbError, Batch as CBatch
 from ._lib import Functors, check
 
 PROG_TUPLE64, PROG_WFTEST16, PROG_WFWIN24, PROG_LIFTED32 = 0, 1, 2, 3
+# the bench stream keyed by the double whose bits are pad[0] / by the 16-byte struct KEY16 {key, low and high half of pad[0]}
+PROG_TUPLE64_FKEY, PROG_TUPLE64_K16 = 4, 5
 
 TUPLE64 = np.dtype([("key", "<u8"), ("id", "<u8"), ("ivalue", "<i8"), ("fvalue", "<f8"), ("pad", "<u8", (4,))])
 RESULT32 = np.dtype([("key", "<u8"), ("id", "<u8"), ("isum", "<i8"), ("fsum", "<f8")])
 WFTEST16 = np.dtype([("key", "<u8"), ("value", "<i8")])
 WFWIN24 = np.dtype([("key", "<u8"), ("id", "<u8"), ("value", "<i8")])
+RESULT32D = np.dtype([("key", "<f8"), ("id", "<u8"), ("isum", "<i8"), ("fsum", "<f8")])
+KEY16 = np.dtype([("key", "<u8"), ("a", "<u4"), ("b", "<u4")])
+RESULT48K = np.dtype([("key", KEY16), ("id", "<u8"), ("isum", "<i8"), ("fsum", "<f8"), ("pad", "<u8")])
 
-TUPLE_DTYPE = {PROG_TUPLE64: TUPLE64, PROG_WFTEST16: WFTEST16, PROG_WFWIN24: WFWIN24, PROG_LIFTED32: RESULT32}
-RESULT_DTYPE = {PROG_TUPLE64: RESULT32, PROG_WFTEST16: WFWIN24, PROG_WFWIN24: WFWIN24, PROG_LIFTED32: RESULT32}
+TUPLE_DTYPE = {PROG_TUPLE64: TUPLE64, PROG_WFTEST16: WFTEST16, PROG_WFWIN24: WFWIN24, PROG_LIFTED32: RESULT32,
+               PROG_TUPLE64_FKEY: TUPLE64, PROG_TUPLE64_K16: TUPLE64}
+RESULT_DTYPE = {PROG_TUPLE64: RESULT32, PROG_WFTEST16: WFWIN24, PROG_WFWIN24: WFWIN24, PROG_LIFTED32: RESULT32,
+                PROG_TUPLE64_FKEY: RESULT32D, PROG_TUPLE64_K16: RESULT48K}
 
 KEY_RR, KEY_UNIFORM, KEY_ZIPF = 0, 1, 2
 SEED = 0x5EED5EED
