@@ -656,6 +656,7 @@ public:
                                       FacadeStatefulProgram<tuple_t, state_t, func_t, StatefulKeepAll<tuple_t, state_t>, keyextr_func_gpu_t>>;
     static constexpr op_type_t op_type = op_type_t::BASIC_GPU;
     func_t func; keyextr_func_gpu_t key_extr; uint32_t max_keys; size_t maxk = WF_MAX_BATCHES_PER_CALL;
+    bool grow_keys = false; // withKeyGrowth(): max_keys is the initial capacity of the table (WFB_KEYS_GROW), which grows under the replicas' mutex
     Stateful_GPU(func_t f, keyextr_func_gpu_t k, size_t p, std::string n, uint32_t mk): Basic_Operator(std::move(n), p, Routing_Mode_t::KEYBY, 1), func(f), key_extr(k), max_keys(mk) {}
     std::string getType() const override { return IS_FILTER ? "Filter_GPU" : "Map_GPU"; }
     keyextr_func_gpu_t getKeyExtractor() const { return key_extr; }
@@ -735,7 +736,7 @@ public:
     std::shared_ptr<SharedKState> kstate;
     Replica *make_replica()
     {
-        if (!kstate) { kstate = std::make_shared<SharedKState>(); wfbErrChk(wfb_kstate_create(&kstate->h, wfb::register_program<prog_t>(), max_keys, 0)); }
+        if (!kstate) { kstate = std::make_shared<SharedKState>(); wfbErrChk(wfb_kstate_create(&kstate->h, wfb::register_program<prog_t>(), max_keys, grow_keys ? WFB_KEYS_GROW : 0u)); }
         return new Replica(name, kstate, func, key_extr, parallelism > 1 ? 1 : maxk);
     }
 };
@@ -840,13 +841,14 @@ public:
     lift_func_gpu_t lift; comb_func_gpu_t comb; keyextr_func_gpu_t key_extr;
     uint64_t win_len, slide_len, lateness; Win_Type_t winType; size_t numWinPerBatch; uint32_t max_keys; bool dense_keys;
     size_t maxk = WF_MAX_BATCHES_PER_CALL;
+    bool grow_keys = false; // withKeyGrowth(): max_keys is the initial capacity of the key table (WFB_KEYS_GROW)
     pre_t pre{}; // the fused run of stateless operators chained in front of this operator (MultiPipe / FusedPipe fill it)
     bool has_pre() const { if constexpr (typed_pre) return true; else return pre.c.n != 0; }
     // the same operator with the typed run `p` in front (FusedPipe)
     template <class other_pre_t>
     Ffat_Windows_GPU(const Ffat_Windows_GPU<lift_func_gpu_t, comb_func_gpu_t, keyextr_func_gpu_t, other_pre_t> &o, pre_t p):
         Basic_Operator(o), lift(o.lift), comb(o.comb), key_extr(o.key_extr), win_len(o.win_len), slide_len(o.slide_len), lateness(o.lateness), winType(o.winType),
-        numWinPerBatch(o.numWinPerBatch), max_keys(o.max_keys), dense_keys(o.dense_keys), maxk(o.maxk), pre(p) {}
+        numWinPerBatch(o.numWinPerBatch), max_keys(o.max_keys), dense_keys(o.dense_keys), maxk(o.maxk), grow_keys(o.grow_keys), pre(p) {}
     Ffat_Windows_GPU(lift_func_gpu_t l, comb_func_gpu_t c, keyextr_func_gpu_t k, std::string n, uint64_t w, uint64_t s, uint64_t late,
                      Win_Type_t wt, size_t nwb, uint32_t mk, bool dense, size_t mbpc):
         Basic_Operator(std::move(n), 1 /* forced to 1, wf/ffat_windows_gpu.hpp:197 */, isKeyed ? Routing_Mode_t::KEYBY : Routing_Mode_t::FORWARD, nwb), lift(l), comb(c), key_extr(k),
@@ -874,7 +876,7 @@ public:
         {
             Basic_Replica::svc_init();
             wfbErrChk(wfb_ffat_create(&ffat, wfb::register_program<prog_t>(), op.win_len, op.slide_len, static_cast<uint32_t>(op.numWinPerBatch),
-                                      op.max_keys, tb ? 1 : 0, op.lateness, op.dense_keys ? WFB_FFAT_DENSE_KEYS : 0u));
+                                      op.max_keys, tb ? 1 : 0, op.lateness, (op.dense_keys ? WFB_FFAT_DENSE_KEYS : 0u) | (op.grow_keys ? WFB_KEYS_GROW : 0u)));
             wfbErrChk(wfb_ffat_set_params(ffat, &prm, sizeof(prm)));
             gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING));
             return 0;
@@ -891,11 +893,14 @@ public:
             uint64_t total = 0;
             for (size_t i = 0; i < k; i++) { bi[i] = wfb_batch_t{work[i]->tuples_gpu, work[i]->ts_gpu, work[i]->getWatermark(), static_cast<uint32_t>(work[i]->size), 0}; total += work[i]->size; }
             // every group that can fire in this call: per key, count-based one per slide*Nb items (+1: the first group); time-based one
-            // per slide*Nb time units the watermark advanced since the key was last seen -- bounded here by the whole advance
+            // per slide*Nb time units the watermark advanced since the key was last seen -- bounded here by the whole advance. A growing
+            // key table may take new keys in the call: count-based, a new key fires its first group after B = (Nb-1)*slide+win of its
+            // items; time-based, one item may be enough, so every item counts as a key
             const uint64_t wm = work.back()->getWatermark();
-            const uint64_t nb = op.numWinPerBatch, per = op.slide_len * nb;
-            const uint64_t groups = tb ? static_cast<uint64_t>(op.max_keys) * ((wm > last_wm ? wm - last_wm : 0) / per + 2) + (wm / per + 2)
-                                       : total / per + op.max_keys + 1;
+            const uint64_t nb = op.numWinPerBatch, per = op.slide_len * nb, B = (nb - 1) * op.slide_len + op.win_len;
+            const uint64_t keys = wfb_ffat_key_capacity(ffat) + (op.grow_keys ? (tb ? total : total / B) : 0);
+            const uint64_t groups = tb ? keys * ((wm > last_wm ? wm - last_wm : 0) / per + 2) + (wm / per + 2)
+                                       : total / per + keys + 1;
             if (tb && last_wm == 0) last_wm = wm; // (the bound above for the first batch: wm / per groups of one key)
             cap_hint = std::max(cap_hint, static_cast<size_t>(std::min<uint64_t>(groups * nb, 0x7fffffffull))); // (never shrinks: recycled batches keep fitting)
             const size_t cap = cap_hint;
@@ -935,13 +940,14 @@ public:
 // ---- builders (wf/builders_gpu.hpp) ----------------------------------------------------------------------------------------
 template <class map_func_gpu_t, class keyextr_func_gpu_t>
 class MapGPU_KB_Builder { // MapGPU_Builder(func).withKeyBy(key_extr): the keyed-stateful operator
-    map_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16;
+    map_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
 public:
     MapGPU_KB_Builder(map_func_gpu_t f, keyextr_func_gpu_t k, std::string n, size_t p): func(f), key(k), name(std::move(n)), parallelism(p) {}
     auto &withName(std::string n) { name = std::move(n); return *this; }
     auto &withParallelism(size_t p) { parallelism = p; return *this; }
-    auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; } // capacity of the device key -> state table (not in the reference: its map grows on the host)
-    auto build() { return Map_GPU_KB<map_func_gpu_t, keyextr_func_gpu_t>(func, key, parallelism, name, max_keys); }
+    auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; } // capacity of the device key -> state table (the initial one withKeyGrowth())
+    auto &withKeyGrowth() { grow = true; return *this; } // extension: the table grows with the keys, as the reference's map does on the host
+    auto build() { Map_GPU_KB<map_func_gpu_t, keyextr_func_gpu_t> m(func, key, parallelism, name, max_keys); m.grow_keys = grow; return m; }
 };
 
 template <class map_func_gpu_t>
@@ -971,13 +977,14 @@ public:
 
 template <class filter_func_gpu_t, class keyextr_func_gpu_t>
 class FilterGPU_KB_Builder {
-    filter_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16;
+    filter_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
 public:
     FilterGPU_KB_Builder(filter_func_gpu_t f, keyextr_func_gpu_t k, std::string n, size_t p): func(f), key(k), name(std::move(n)), parallelism(p) {}
     auto &withName(std::string n) { name = std::move(n); return *this; }
     auto &withParallelism(size_t p) { parallelism = p; return *this; }
     auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; }
-    auto build() { return Filter_GPU_KB<filter_func_gpu_t, keyextr_func_gpu_t>(func, key, parallelism, name, max_keys); }
+    auto &withKeyGrowth() { grow = true; return *this; } // extension: the key -> state table grows with the keys
+    auto build() { Filter_GPU_KB<filter_func_gpu_t, keyextr_func_gpu_t> m(func, key, parallelism, name, max_keys); m.grow_keys = grow; return m; }
 };
 
 template <class filter_func_gpu_t>
@@ -1034,7 +1041,7 @@ class Ffat_WindowsGPU_Builder {
     template <class A, class B, class C> friend class Ffat_WindowsGPU_Builder;
     lift_func_gpu_t lift; comb_func_gpu_t comb; keyextr_func_gpu_t key_extr; std::string name = "ffat_windows_gpu";
     size_t numWinPerBatch = 0, max_batches = WF_MAX_BATCHES_PER_CALL; uint64_t win_len = 0, slide_len = 0, lateness = 0; Win_Type_t winType = Win_Type_t::CB;
-    uint32_t max_keys = 65536; bool dense = false;
+    uint32_t max_keys = 65536; bool dense = false, grow = false;
     Ffat_WindowsGPU_Builder(lift_func_gpu_t l, comb_func_gpu_t c, keyextr_func_gpu_t k): lift(l), comb(c), key_extr(k) {}
 public:
     Ffat_WindowsGPU_Builder(lift_func_gpu_t l, comb_func_gpu_t c): lift(l), comb(c), key_extr() {}
@@ -1043,14 +1050,15 @@ public:
     {
         Ffat_WindowsGPU_Builder<lift_func_gpu_t, comb_func_gpu_t, new_keyextr_t> nb(lift, comb, k);
         nb.name = name; nb.numWinPerBatch = numWinPerBatch; nb.win_len = win_len; nb.slide_len = slide_len; nb.lateness = lateness;
-        nb.winType = winType; nb.max_keys = max_keys; nb.dense = dense; nb.max_batches = max_batches;
+        nb.winType = winType; nb.max_keys = max_keys; nb.dense = dense; nb.grow = grow; nb.max_batches = max_batches;
         return nb;
     }
     auto &withCBWindows(uint64_t w, uint64_t s) { win_len = w; slide_len = s; winType = Win_Type_t::CB; lateness = 0; return *this; }
     auto &withTBWindows(std::chrono::microseconds w, std::chrono::microseconds s) { win_len = w.count(); slide_len = s.count(); winType = Win_Type_t::TB; return *this; }
     auto &withLateness(std::chrono::microseconds l) { lateness = l.count(); return *this; }
     auto &withNumWinPerBatch(size_t n) { numWinPerBatch = n; return *this; }
-    auto &withMaxKeys(uint32_t n) { max_keys = n; return *this; }       // extension: capacity of the device-resident key table
+    auto &withMaxKeys(uint32_t n) { max_keys = n; return *this; }       // extension: capacity of the device-resident key table (the initial one withKeyGrowth())
+    auto &withKeyGrowth() { grow = true; return *this; }                // extension: the key table grows with the keys (not with withDenseKeys)
     auto &withDenseKeys()                                               // extension: keys are 0 .. max_keys-1 (slot = key, no hash probe)
     {
         static_assert(integral_key_v<keyextr_func_gpu_t>, "WindFlow Compilation Error - Ffat_WindowsGPU_Builder: withDenseKeys() needs an integral or enum key type:\n");
@@ -1060,7 +1068,10 @@ public:
     auto build()
     {   // (withDenseKeys before withKeyBy: the key type is known here)
         if (dense && !integral_key_v<keyextr_func_gpu_t>) wf_fatal("Ffat_WindowsGPU_Builder: withDenseKeys() needs an integral or enum key type");
-        return Ffat_Windows_GPU<lift_func_gpu_t, comb_func_gpu_t, keyextr_func_gpu_t>(lift, comb, key_extr, name, win_len, slide_len, lateness, winType, numWinPerBatch, max_keys, dense, max_batches);
+        if (dense && grow) wf_fatal("Ffat_WindowsGPU_Builder: withKeyGrowth() cannot be combined with withDenseKeys()");
+        Ffat_Windows_GPU<lift_func_gpu_t, comb_func_gpu_t, keyextr_func_gpu_t> w(lift, comb, key_extr, name, win_len, slide_len, lateness, winType, numWinPerBatch, max_keys, dense, max_batches);
+        w.grow_keys = grow;
+        return w;
     }
 };
 

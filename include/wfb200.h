@@ -139,8 +139,10 @@ int wfb_map_filter_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_b
  * order = batch order, then index order. replaces Stateful_MAPGPU_Kernel / Stateful_FILTERGPU_Kernel + the TBB key map,
  * spinlock and per-key state allocation, wf/map_gpu.hpp:80-102, :212-299, wf/filter_gpu.hpp:91-117, :247-355. */
 typedef struct wfb_kstate wfb_kstate_t;
-int wfb_kstate_create(wfb_kstate_t **h, int prog, uint32_t max_keys, uint32_t flags /* WFB_FFAT_DENSE_KEYS */);
+int wfb_kstate_create(wfb_kstate_t **h, int prog, uint32_t max_keys, uint32_t flags /* WFB_FFAT_DENSE_KEYS or WFB_KEYS_GROW */);
 int wfb_kstate_destroy(wfb_kstate_t *h);
+/* Current key capacity (max_keys, or what a WFB_KEYS_GROW handle has grown to). Host-side: does not synchronise. */
+uint32_t wfb_kstate_key_capacity(const wfb_kstate_t *h);
 /* Map_GPU: in place. */
 int wfb_map_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *batches_h, uint32_t nbatches, void *stream);
 /* Filter_GPU: the functor may modify the tuple; survivors of batch i are compacted (stable) into (out[i].tuples, out[i].ts),
@@ -200,6 +202,16 @@ int wfb_shard_lift(wfb_engine_t *e, const wfb_functors_t *pre, const wfb_batch_t
  *                          overlap the ingest pass of segment k+1; wfb_ffat_flush returns the last segment's results. The
  *                          set of results over the whole stream is identical to the non-pipelined mode. */
 #define WFB_FFAT_PIPELINED 2u
+/*   WFB_KEYS_GROW       => max_keys is the initial capacity: the key table and every per-key array grow on demand (the reference's
+ *                          key maps grow on the host, wf/ffat_replica_gpu.hpp:783-790, wf/map_gpu.hpp:236-240). A call that meets more
+ *                          keys than the capacity grows it to a power of two >= 2 * max(keys, capacity) and reruns its key lookup; slots
+ *                          are kept, so every key's state survives. The only cost on calls that do not grow is one 8-byte device-to-host
+ *                          copy the host waits for. A growth that cannot allocate returns WFB_E_CAPACITY and leaves the handle as it was.
+ *                          Also accepted by wfb_kstate_create. Not with WFB_FFAT_DENSE_KEYS, WFB_FFAT_PIPELINED or a key shard
+ *                          (WFB_E_BADARG). The doubling stops at 65536 keys while the keys fit: time-based and keyed-stateful handles
+ *                          grow up to 65536 keys, count-based ones then double again up to 2^30. On a growing handle the integer key
+ *                          2^64-1 (the free-entry marker) is refused with error bit 0, as the all-ones 16-byte key is. */
+#define WFB_KEYS_GROW 4u
 int wfb_ffat_create(wfb_ffat_t **h, int prog, uint64_t win, uint64_t slide, uint32_t wins_per_batch,
                     uint32_t max_keys, int win_type, uint64_t lateness, uint32_t flags);
 int wfb_ffat_destroy(wfb_ffat_t *h);
@@ -244,8 +256,12 @@ int wfb_ffat_flush(wfb_ffat_t *h, void *out_results, uint64_t *out_ts, uint32_t 
  * call, and *calls_h = number of calls summed. Synchronises on the last recorded event. */
 int wfb_ffat_timing(wfb_ffat_t *h, int enable, float *ms_h, uint32_t *calls_h);
 
-/* Number of distinct keys seen so far / error flags raised on the device (synchronises the stream). */
+/* Number of distinct keys seen so far / error flags raised on the device (synchronises the stream). Flags: bit 0 more keys than the
+ * capacity (fixed handles), bit 1 more results than out_capacity, bit 2 pane id out of range (time-based), bit 3 the key table must
+ * grow (growing handles: set only while a growth that returned WFB_E_CAPACITY is pending). */
 int wfb_ffat_stats(wfb_ffat_t *h, uint32_t *n_keys_h, uint32_t *err_flags_h, void *stream);
+/* Current key capacity (max_keys, or what a WFB_KEYS_GROW handle has grown to). Host-side: does not synchronise. */
+uint32_t wfb_ffat_key_capacity(const wfb_ffat_t *h);
 /* Window results delivered by the handle since it was created (summed on the device by the last kernel of every call; synchronises
  * the stream). Lets a caller account for results without reading *n_out_dev back after every call (the role of the
  * outputs_sent counter of wf/stats_record.hpp:80-82). */

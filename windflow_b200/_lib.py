@@ -49,6 +49,7 @@ SYMBOLS = {
     "wfb_map_filter": (C.c_int, [vp, C.POINTER(Functors), vp, vp, u32, vp, vp, vp, vp]),
     "wfb_kstate_create": (C.c_int, [C.POINTER(vp), C.c_int, u32, u32]),
     "wfb_kstate_destroy": (C.c_int, [vp]),
+    "wfb_kstate_key_capacity": (u32, [vp]),
     "wfb_map_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), u32, vp]),
     "wfb_filter_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_reduce_by_key_batches": (C.c_int, [vp, C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
@@ -67,6 +68,7 @@ SYMBOLS = {
     "wfb_ffat_flush": (C.c_int, [vp, vp, vp, u32, vp, vp]),
     "wfb_ffat_timing": (C.c_int, [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(u32)]),
     "wfb_ffat_stats": (C.c_int, [vp, C.POINTER(u32), C.POINTER(u32), vp]),
+    "wfb_ffat_key_capacity": (u32, [vp]),
     "wfb_ffat_results_total": (C.c_int, [vp, C.POINTER(C.c_uint64), vp]),
     "wfb_gen_tuple64": (C.c_int, [u64, u64, u32, C.c_int, u64, vp, vp, vp, vp]),
     "wfb_mg_unique_id": (C.c_int, [vp]),

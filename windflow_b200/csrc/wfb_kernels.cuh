@@ -80,11 +80,12 @@ struct FfatDev {
     uint32_t ht_mask;          // capacity - 1
     uint32_t max_keys;
     uint32_t *n_slots;         // number of keys inserted so far
-    uint32_t *err_flags;       // bit0: key table full, bit1: output capacity exceeded
+    uint32_t *err_flags;       // bit0: key table full, bit1: output capacity exceeded, bit2: pane ring overflow (time-based), bit3: KEYS_GROW_FLAG
     unsigned long long *results_total; // window results delivered so far (added by the last kernel of every call)
     uint64_t defer_items;              // a fired group may wait for the deferred pass (k_ffat_windows*) while fewer than this many further items of
                                        // its key follow in the call: (spare ring leaves + 1) panes -- later panes then do not overwrite leaves it reads
     uint32_t dense;            // 1: slot = key (keys < max_keys), or key / key_div for one shard of a keyby
+    uint32_t grow;             // 1: the key table grows (WFB_KEYS_GROW): a key beyond max_keys keeps its slot and raises KEYS_GROW_FLAG
     uint32_t key_div, key_rem; // dense: the handle owns the keys with key % key_div == key_rem (key_div <= 1: all keys)
     // per-slot state
     uint64_t *slot_key;        // key of each slot
@@ -114,6 +115,9 @@ struct FfatDev {
 };
 constexpr uint64_t EMPTY_KEY = 0xffffffffffffffffull;
 constexpr uint32_t INVALID_SLOT = 0xffffffffu;
+// error flag of a growing handle: a key got a slot at or beyond max_keys, or found the key table full. Its items were not taken
+// (INVALID_SLOT); the host grows the table and reruns the pass that inserts the keys (wfb_lib.cu, grow_keys). Cleared by the rebuild.
+constexpr uint32_t KEYS_GROW_FLAG = 8u;
 
 struct TileArgs {
     const DevBatch *batches;   // device array (nbatches entries) or null => use `one`
@@ -279,8 +283,9 @@ __device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, const Key128 
             atom_cas_b128(e, EMPTY_KEY, EMPTY_KEY, key.lo, key.hi, k.lo, k.hi);
             if (k.lo == EMPTY_KEY && k.hi == EMPTY_KEY) { // we own the entry: allocate the slot and publish it
                 uint32_t s = atomicAdd(ff.n_slots, 1u);
-                if (s >= ff.max_keys) { atomicOr(ff.err_flags, 1u); s = INVALID_SLOT - 1; }
-                else reinterpret_cast<Key128 *>(ff.slot_key)[s] = key;
+                if (s < ff.max_keys) reinterpret_cast<Key128 *>(ff.slot_key)[s] = key;
+                else if (ff.grow) atomicOr(ff.err_flags, KEYS_GROW_FLAG); // (the rebuild at the new capacity writes slot_key[s])
+                else { atomicOr(ff.err_flags, 1u); s = INVALID_SLOT - 1; }
                 st_release_u32(&ff.ht_slots[h], s);
                 return s >= ff.max_keys ? INVALID_SLOT : s;
             }
@@ -288,11 +293,12 @@ __device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, const Key128 
         if (k == key) {
             uint32_t s;
             while ((s = ld_acquire_u32(&ff.ht_slots[h])) == INVALID_SLOT) { }
-            return s >= ff.max_keys ? INVALID_SLOT : s;
+            if (s >= ff.max_keys) { if (ff.grow) atomicOr(ff.err_flags, KEYS_GROW_FLAG); return INVALID_SLOT; }
+            return s;
         }
         h = (h + 1) & ff.ht_mask;
     }
-    atomicOr(ff.err_flags, 1u);
+    atomicOr(ff.err_flags, ff.grow ? KEYS_GROW_FLAG : 1u);
     return INVALID_SLOT;
 }
 
@@ -306,6 +312,9 @@ __device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, uint64_t key)
         if (key >= ff.max_keys) { atomicOr(ff.err_flags, 1u); return INVALID_SLOT; }
         return static_cast<uint32_t>(key);
     }
+    // the all-ones key marks a free entry: every insert of it would take a new slot. A growing table refuses it with the capacity flag
+    // (as the 16-byte path does), so that it never grows the table
+    if (ff.grow && key == EMPTY_KEY) { atomicOr(ff.err_flags, 1u); return INVALID_SLOT; }
     uint32_t h = static_cast<uint32_t>(mix64(key)) & ff.ht_mask;
     for (uint32_t probe = 0; probe <= ff.ht_mask; probe++) {
         uint64_t k = ld_relaxed_u64(&ff.ht_keys[h]);
@@ -315,8 +324,9 @@ __device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, uint64_t key)
                                                static_cast<unsigned long long>(key));
             if (old == EMPTY_KEY) { // we own the entry: allocate the slot and publish it
                 uint32_t s = atomicAdd(ff.n_slots, 1u);
-                if (s >= ff.max_keys) { atomicOr(ff.err_flags, 1u); s = INVALID_SLOT - 1; }
-                else ff.slot_key[s] = key;
+                if (s < ff.max_keys) ff.slot_key[s] = key;
+                else if (ff.grow) atomicOr(ff.err_flags, KEYS_GROW_FLAG); // (the rebuild at the new capacity writes slot_key[s])
+                else { atomicOr(ff.err_flags, 1u); s = INVALID_SLOT - 1; }
                 st_release_u32(&ff.ht_slots[h], s);
                 return s >= ff.max_keys ? INVALID_SLOT : s;
             }
@@ -325,12 +335,48 @@ __device__ __forceinline__ uint32_t slot_of_key(const FfatDev &ff, uint64_t key)
         if (k == key) {
             uint32_t s;
             while ((s = ld_acquire_u32(&ff.ht_slots[h])) == INVALID_SLOT) { }
-            return s >= ff.max_keys ? INVALID_SLOT : s;
+            if (s >= ff.max_keys) { if (ff.grow) atomicOr(ff.err_flags, KEYS_GROW_FLAG); return INVALID_SLOT; }
+            return s;
         }
         h = (h + 1) & ff.ht_mask;
     }
-    atomicOr(ff.err_flags, 1u);
+    atomicOr(ff.err_flags, ff.grow ? KEYS_GROW_FLAG : 1u);
     return INVALID_SLOT;
+}
+
+// Rebuilds the key table of a growing handle at a new capacity (new_keys / new_slots all free, new_mask + 1 entries): every
+// entry of the old table is inserted again with its slot -- slots are never renumbered, so the per-slot state moves with a prefix
+// copy -- and slot_key (already the new, larger array) gets the keys of the slots at or beyond old_max_keys, which the old array
+// had no room for. Keys are distinct: an insert claims the first free entry of its probe (16-byte entries with the 16-byte CAS,
+// as slot_of_key does). Clears KEYS_GROW_FLAG.
+static __global__ void __launch_bounds__(256) k_key_table_rebuild(const uint64_t *__restrict__ old_keys, const uint32_t *__restrict__ old_slots,
+                                                           uint32_t old_mask, uint64_t *new_keys, uint32_t *__restrict__ new_slots, uint32_t new_mask,
+                                                           uint64_t *__restrict__ slot_key, uint32_t old_max_keys, uint32_t words, uint32_t *err_flags)
+{
+    if (blockIdx.x == 0 && threadIdx.x == 0) atomicAnd(err_flags, ~KEYS_GROW_FLAG);
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= old_mask; i += gridDim.x * blockDim.x) {
+        uint32_t h;
+        const uint32_t s = old_slots[i];
+        if (words == 2) {
+            const Key128 k = reinterpret_cast<const Key128 *>(old_keys)[i];
+            if (k.lo == EMPTY_KEY && k.hi == EMPTY_KEY) continue;
+            h = static_cast<uint32_t>(mix64(k.lo ^ mix64(k.hi))) & new_mask;
+            for (;; h = (h + 1) & new_mask) {
+                uint64_t lo, hi;
+                atom_cas_b128(new_keys + 2 * static_cast<size_t>(h), EMPTY_KEY, EMPTY_KEY, k.lo, k.hi, lo, hi);
+                if (lo == EMPTY_KEY && hi == EMPTY_KEY) break;
+            }
+            if (s >= old_max_keys) reinterpret_cast<Key128 *>(slot_key)[s] = k;
+        } else {
+            const uint64_t k = old_keys[i];
+            if (k == EMPTY_KEY) continue;
+            h = static_cast<uint32_t>(mix64(k)) & new_mask;
+            while (atomicCAS(reinterpret_cast<unsigned long long *>(&new_keys[h]), static_cast<unsigned long long>(EMPTY_KEY),
+                             static_cast<unsigned long long>(k)) != EMPTY_KEY) h = (h + 1) & new_mask;
+            if (s >= old_max_keys) slot_key[s] = k;
+        }
+        new_slots[h] = s;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------

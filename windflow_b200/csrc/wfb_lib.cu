@@ -374,6 +374,93 @@ struct RadixSorter {
     }
 };
 
+// ---- key tables that grow (WFB_KEYS_GROW) -----------------------------------------------------------------------------------
+// The arrays one growth replaces. Every new array is allocated before any old one is freed, so that a failed allocation leaves the
+// handle as it was.
+struct GrowPlan {
+    struct Array { void **ptr; size_t old_bytes, bytes; bool copy; int fill; bool counted; void *fresh; };
+    std::vector<Array> arrays;
+    // *p (old_bytes) becomes `bytes` bytes: the old ones copied when `copy`, the rest set to the byte `fill` (-1: uninitialised, as
+    // create leaves it). counted: part of wfb_ffat_state_bytes
+    template <class T> void add(T *&p, size_t old_bytes, size_t bytes, bool copy, int fill, bool counted = true)
+    {
+        arrays.push_back({reinterpret_cast<void **>(&p), old_bytes, bytes, copy, fill, counted, nullptr});
+    }
+    template <class T> T *fresh(T *const &p) const
+    {
+        for (const Array &a : arrays) if (a.ptr == reinterpret_cast<void *const *>(&p)) return static_cast<T *>(a.fresh);
+        return nullptr;
+    }
+    int64_t grown_bytes() const { int64_t d = 0; for (const Array &a : arrays) if (a.counted) d += static_cast<int64_t>(a.bytes) - static_cast<int64_t>(a.old_bytes); return d; }
+    int alloc()
+    {
+        for (Array &a : arrays)
+            if (cudaMalloc(&a.fresh, a.bytes) != cudaSuccess) { cudaGetLastError(); release(); return WFB_E_CAPACITY; }
+        return 0;
+    }
+    void release() { for (Array &a : arrays) { cudaFree(a.fresh); a.fresh = nullptr; } }
+    int fill(cudaStream_t s)
+    {
+        for (Array &a : arrays) {
+            const size_t keep = a.copy ? a.old_bytes : 0;
+            if (keep) CK(cudaMemcpyAsync(a.fresh, *a.ptr, keep, cudaMemcpyDeviceToDevice, s));
+            if (a.fill >= 0 && a.bytes > keep) CK(cudaMemsetAsync(static_cast<unsigned char *>(a.fresh) + keep, a.fill, a.bytes - keep, s));
+        }
+        return 0;
+    }
+    void commit() { for (Array &a : arrays) { cudaFree(*a.ptr); *a.ptr = a.fresh; a.fresh = nullptr; } }
+};
+
+// pinned words the growth check reads the key count and the error flags into, and the event it waits on
+struct GrowCheck {
+    uint32_t *host = nullptr; cudaEvent_t ev = nullptr;
+    int init() { CK(cudaMallocHost(reinterpret_cast<void **>(&host), 2 * sizeof(uint32_t))); CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); return 0; }
+    void destroy() { if (host) cudaFreeHost(host); if (ev) cudaEventDestroy(ev); host = nullptr; ev = nullptr; }
+};
+
+// The growth step of every handle kind, run after the pass that inserts the keys of a call. It reads the key count and the error
+// flags (the one synchronisation growth adds, on growing handles only). When the pass raised KEYS_GROW_FLAG, the capacity becomes a
+// power of two >= 2 * max(keys, capacity), but not beyond `ceiling` (a power of two) while the capacity is below it and the keys fit it:
+// the largest capacity that keeps the handle's path (time-based and keyed-stateful handles: their only path; count-based: the bucket
+// path). It is at most `limit` (else WFB_E_CAPACITY). add_state(plan, cap) lists the handle's own arrays sized by the capacity, the key
+// table is rebuilt at the new size, and derive(cap, plan) recomputes what create derived from the capacity. *grew = true: the caller
+// reruns its key-inserting pass (it has no other state than the inserts, which are idempotent), and so on until a pass raises no flag;
+// every growth but the one that stops at the ceiling at least doubles the capacity.
+template <class AddState, class Derive>
+int grow_keys(FfatDev &ff, uint32_t key_bytes, GrowCheck &gc, uint32_t ceiling, uint32_t limit, cudaStream_t s, bool *grew, AddState add_state,
+              Derive derive)
+{
+    *grew = false;
+    CK(cudaMemcpyAsync(gc.host, ff.n_slots, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s)); // n_slots, err_flags (adjacent)
+    CK(cudaEventRecord(gc.ev, s));
+    CK(cudaEventSynchronize(gc.ev));
+    if (!(gc.host[1] & KEYS_GROW_FLAG)) return 0;
+    const uint32_t old = ff.max_keys;
+    uint64_t cap = 1; while (cap < 2ull * std::max(gc.host[0], old)) cap <<= 1;
+    if (cap > ceiling && old < ceiling && gc.host[0] <= ceiling) cap = ceiling; // (every slot handed out so far, < n_slots, fits)
+    if (cap > limit) return WFB_E_CAPACITY;
+    uint64_t entries = 1; while (entries < 2 * cap) entries <<= 1;
+    GrowPlan plan;
+    plan.add(ff.ht_keys, static_cast<size_t>(key_bytes) * (ff.ht_mask + 1ull), key_bytes * entries, false, 0xff);
+    plan.add(ff.ht_slots, sizeof(uint32_t) * (ff.ht_mask + 1ull), sizeof(uint32_t) * entries, false, 0xff);
+    plan.add(ff.slot_key, static_cast<size_t>(key_bytes) * old, static_cast<size_t>(key_bytes) * cap, true, -1);
+    int rc = add_state(plan, static_cast<uint32_t>(cap)); if (rc) return rc;
+    rc = plan.alloc(); if (rc) return rc;
+    rc = plan.fill(s);
+    if (!rc) {
+        k_key_table_rebuild<<<grid_for(ff.ht_mask + 1, 256), 256, 0, s>>>(ff.ht_keys, ff.ht_slots, ff.ht_mask, plan.fresh(ff.ht_keys), plan.fresh(ff.ht_slots),
+                                                                        static_cast<uint32_t>(entries - 1), plan.fresh(ff.slot_key), old, key_bytes / 8, ff.err_flags);
+        rc = static_cast<int>(cudaGetLastError());
+    }
+    if (!rc) rc = static_cast<int>(cudaStreamSynchronize(s)); // (the old arrays are read until here)
+    if (rc) { cudaStreamSynchronize(s); plan.release(); return rc; }
+    plan.commit();
+    ff.ht_mask = static_cast<uint32_t>(entries - 1); ff.max_keys = static_cast<uint32_t>(cap);
+    rc = derive(static_cast<uint32_t>(cap), plan); if (rc) return rc;
+    *grew = true;
+    return 0;
+}
+
 } // namespace
 
 struct wfb_engine {
@@ -529,7 +616,8 @@ struct wfb_ffat {
     uint32_t *tb_popped_slots = nullptr;
     bool shares_slot_key = false;                   // back end of a time-based handle: ff.slot_key / ff.n_slots belong to the front end
     uint32_t *own_n_slots = nullptr;                // the allocation behind ff.n_slots / ff.err_flags of this handle
-    uint32_t *tb_head = nullptr, *tb_seg = nullptr, *tb_misc = nullptr; // misc: [0] n_segs [1] first_seg dummy [2] n_present [3] popped total [4] ignored [5] ring capacity needed
+    uint32_t *tb_head = nullptr, *tb_seg = nullptr, *tb_misc = nullptr; // misc: [0] n_segs [1] first_seg dummy [2] n_present [3] popped total [4] ignored [5] ring capacity needed [6] ignored before the batch (growing handles)
+    GrowCheck growc;                // WFB_KEYS_GROW (ff.grow): the growth check after the key-inserting pass
     uint32_t *mg_scratch = nullptr; // (internal, ffat_process_prebucketed) per-(bucket, sub-bucket, source) counts, their scan, run starts
     bool append_results = false;  // (internal, wfb_mg_flush) the next call's results follow the ones already in the output buffer
     bool buckets = true;          // one wide radix pass + per-bucket CTAs (<= 65536 keys); WFB_UPDATE=lanes selects the
@@ -986,6 +1074,7 @@ struct wfb_kstate {
     unsigned char *keep = nullptr;
     uint64_t launches = 0;
     PinnedStage stage;
+    GrowCheck growc;              // WFB_KEYS_GROW (ff.grow)
 };
 extern "C" {
 
@@ -996,6 +1085,7 @@ int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t f
     if (!o) return WFB_E_NOPROG;
     if (o->state_bytes == 0) return WFB_E_UNSUPPORTED; // the program has no state_t / stateful functors
     if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
+    if ((flags & WFB_KEYS_GROW) && (flags & WFB_FFAT_DENSE_KEYS)) return WFB_E_BADARG;       // (slot = key: nothing to grow)
     uint32_t bits = 0; while ((1ull << bits) < max_keys) bits++;
     if (bits > OSW_BITS + 6) return WFB_E_UNSUPPORTED;  // 1024 buckets of at most 64 keys
     int rc = device_ready(); if (rc) return rc;
@@ -1004,6 +1094,7 @@ int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t f
     h->prog = prog; h->ops = o; h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
     FfatDev &ff = h->ff;
     ff.max_keys = max_keys; ff.dense = (flags & WFB_FFAT_DENSE_KEYS) ? 1u : 0u;
+    if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_kstate_destroy(h); return rc; } }
     uint32_t cap = 1; while (cap < 2ull * max_keys) cap <<= 1;
     ff.ht_mask = cap - 1;
 #define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc(reinterpret_cast<void **>(&(ptr)), (bytes)); if (e_ != cudaSuccess) { wfb_kstate_destroy(h); return static_cast<int>(e_); } } while (0)
@@ -1028,11 +1119,13 @@ int wfb_kstate_destroy(wfb_kstate_t *h)
     cudaFree(h->ff.ht_keys); cudaFree(h->ff.ht_slots); cudaFree(h->ff.n_slots); cudaFree(h->ff.slot_key); cudaFree(h->states);
     cudaFree(h->d_batches); cudaFree(h->d_boff); cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posB); cudaFree(h->tile_cnt);
     cudaFree(h->rank_start); cudaFree(h->keep);
-    h->sorter.destroy(); h->stage.destroy();
+    h->sorter.destroy(); h->stage.destroy(); h->growc.destroy();
     delete h;
     cudaGetLastError();
     return 0;
 }
+
+uint32_t wfb_kstate_key_capacity(const wfb_kstate_t *h) { return h ? h->ff.max_keys : 0; }
 
 static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
                       uint32_t *n_out_dev, bool filter, cudaStream_t s)
@@ -1078,6 +1171,21 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
     { int rc_ = h->stage.h2d(h->d_boff, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
     // 1. slots; 2. one wide partition pass into 1024 buckets of consecutive slots; 3. per-bucket CTAs, one thread per key
     int rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc;
+    for (bool grew = h->ff.grow != 0; grew; ) { // (a growing handle: the buckets hold 64 keys at most, as at create)
+        rc = grow_keys(h->ff, h->ops->key_bytes, h->growc, 1u << (OSW_BITS + 6), 1u << (OSW_BITS + 6), s, &grew,
+                       [h](GrowPlan &plan, uint32_t cap) {
+                           const size_t sb = h->ops->state_bytes;
+                           plan.add(h->states, sb * h->ff.max_keys, sb * cap, true, 0); // state_t(): zero-initialised
+                           return 0;
+                       },
+                       [h](uint32_t cap, const GrowPlan &) {
+                           uint32_t bits = 0; while ((1ull << bits) < cap) bits++;
+                           h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
+                           return 0;
+                       });
+        if (rc) return rc;
+        if (grew) { rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc; h->launches += 2; }
+    }
     const uint32_t *counts = nullptr;
     const uint64_t before = h->sorter.launches;
     rc = h->sorter.sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, &counts, nullptr, nullptr, 0, true);
@@ -1130,6 +1238,89 @@ static int lifted_program_of(int prog)
     return id;
 }
 
+// what create derives from the key capacity and the tuning knobs: the sort passes over the slots and the bucket / onesweep path
+static void ffat_derive_paths(wfb_ffat *h)
+{
+    uint32_t bits = 0; while ((1ull << bits) < h->ff.max_keys) bits++;
+    h->sort_passes = std::max(1u, (bits + 7) / 8);
+    h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
+    // bucket path: every bucket holds at most BK_KEYS keys and the pane length fits 32 bits
+    const char *e = std::getenv("WFB_UPDATE");
+    h->buckets = !(e && std::strcmp(e, "lanes") == 0) && (1u << h->bucket_shift) <= BK_KEYS && h->ff.pane < (1ull << 32);
+    // streaming update: one path update per completed pane inside the item loop, so panes of a few items at least
+    h->stream_update = h->buckets && !h->bucket_move && e && std::strcmp(e, "stream") == 0; // (measured: 173 us against 153 us for the bucket kernel at the bench configuration)
+    const char *t = std::getenv("WFB_TILE_H16");
+    h->tile_h16 = h->buckets && !(t && std::atoi(t) == 0);
+}
+
+// deferred window groups a segment of seg_cap records can fire: one per slide * Nb records, and one more per key
+static uint32_t ffat_trig_cap(const wfb_ffat *h, uint32_t seg_cap, uint32_t keys)
+{
+    const uint64_t per_group = std::max<uint64_t>(1, h->ff.slide * h->ff.nb);
+    return static_cast<uint32_t>(std::min<uint64_t>(seg_cap / per_group + keys + 1, 0x7fffffffull));
+}
+
+// growth of a count-based handle (also the back end of a time-based one) to `cap` keys: its per-key arrays, tails as create leaves
+// them (slot-major: the state of slot s stays at s), then what create derives from the capacity
+static void ffat_plan_state(wfb_ffat *h, GrowPlan &plan, uint32_t cap)
+{
+    FfatDev &ff = h->ff;
+    const size_t old = ff.max_keys, RB = h->ops->result_bytes, tree = (2ull * ff.n_leaves - 1) * RB;
+    plan.add(ff.cnt, sizeof(uint64_t) * old, sizeof(uint64_t) * cap, true, 0);
+    plan.add(ff.acc, RB * old, RB * cap, true, 0);
+    plan.add(ff.tree, tree * old, tree * cap, true, 0);
+    plan.add(ff.seg_off, sizeof(uint32_t) * (old + 1), sizeof(uint32_t) * (cap + 1ull), true, 0xff);
+    plan.add(ff.heavy, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, false, -1);
+    SegScratch &g = h->seg[0]; // (growing handles are not pipelined: one segment scratch)
+    plan.add(g.seg_cnt, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, false, 0); // (a rerun pass counts the segment's items again)
+    if (g.trig) plan.add(g.trig, sizeof(Trigger) * g.trig_cap, sizeof(Trigger) * ffat_trig_cap(h, g.cap, cap), false, -1, false);
+}
+static void ffat_derive(wfb_ffat *h, uint32_t cap)
+{
+    h->ff.max_keys = cap;
+    SegScratch &g = h->seg[0];
+    if (g.trig) g.trig_cap = ffat_trig_cap(h, g.cap, cap);
+    ffat_derive_paths(h);
+}
+static int ffat_grow(wfb_ffat *h, cudaStream_t s, bool *grew)
+{
+    return grow_keys(h->ff, h->ops->key_bytes, h->growc, BK_KEYS << OSW_BITS, 1u << 30, s, grew,
+                     [h](GrowPlan &plan, uint32_t cap) { ffat_plan_state(h, plan, cap); return 0; },
+                     [h](uint32_t cap, const GrowPlan &plan) { ffat_derive(h, cap); h->state_bytes += plan.grown_bytes(); return 0; });
+}
+
+// growth of a time-based front end: its rings of pending panes and per-key pane bookkeeping, and its count-based back end. At most
+// 65536 keys: the back end takes the popped panes in place, which needs the bucket path (as tb_create requires)
+static int tb_grow(wfb_ffat *h, cudaStream_t s, bool *grew)
+{
+    return grow_keys(h->ff, h->ops->key_bytes, h->growc, BK_KEYS << OSW_BITS, BK_KEYS << OSW_BITS, s, grew,
+        [h](GrowPlan &plan, uint32_t cap) {
+            TbDev &tb = h->tb;
+            const size_t old = h->ff.max_keys, RB = h->ops->result_bytes;
+            if (static_cast<uint64_t>(tb.capq) * cap * RB > (32ull << 30)) return WFB_E_CAPACITY; // (the guard of tb_create)
+            plan.add(tb.first, sizeof(uint64_t) * old, sizeof(uint64_t) * cap, true, 0);
+            plan.add(tb.num, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, true, 0);
+            plan.add(tb.num_new, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, false, -1);
+            plan.add(tb.trig, sizeof(uint64_t) * old, sizeof(uint64_t) * cap, true, -1); // (tail: Bp - 1, below)
+            plan.add(tb.done, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, true, 0);
+            plan.add(tb.ring, RB * tb.capq * old, RB * tb.capq * cap, true, -1);
+            plan.add(tb.present, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, false, -1);
+            plan.add(tb.cnt, sizeof(uint32_t) * (old + 1), sizeof(uint32_t) * (cap + 1ull), false, -1);
+            ffat_plan_state(h->cb, plan, cap);
+            return 0;
+        },
+        [h, s](uint32_t cap, const GrowPlan &plan) {
+            const uint32_t old = h->cb->ff.max_keys; // (the back end still has the old capacity)
+            std::vector<uint64_t> t0(cap - old, h->tb.Bp - 1); // :463
+            CK(cudaMemcpyAsync(h->tb.trig + old, t0.data(), sizeof(uint64_t) * t0.size(), cudaMemcpyHostToDevice, s));
+            CK(cudaStreamSynchronize(s)); // (t0 lives until here)
+            ffat_derive(h->cb, cap);
+            h->cb->ff.slot_key = h->ff.slot_key;
+            h->state_bytes += plan.grown_bytes();
+            return 0;
+        });
+}
+
 static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uint32_t nb, uint32_t max_keys, uint64_t lateness, uint32_t flags)
 {
     const ProgramOps *o = program(prog);
@@ -1179,6 +1370,7 @@ static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, ui
     tb.n_present = h->tb_misc + 2; tb.ignored = h->tb_misc + 4; tb.need = h->tb_misc + 5; tb.err = ff.err_flags;
 #undef ALLOC
     rc = h->ts.init(); if (rc) { wfb_ffat_destroy(h); return rc; }
+    if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_ffat_destroy(h); return rc; } } // (the back end grows with it)
     rc = wfb_ffat_create(&h->cb, lp, win_p, slide_p, nb, max_keys, 0, 0, flags & WFB_FFAT_DENSE_KEYS);
     if (rc) { wfb_ffat_destroy(h); return rc; }
     // the front end hands the popped panes to the back end in place, with the slot of every record: that needs the bucket path with the
@@ -1226,7 +1418,16 @@ int wfb_ffat_process_tb(wfb_ffat_t *h, const wfb_functors_t *pre, const wfb_batc
         CK(cudaMemsetAsync(misc, 0, sizeof(uint32_t) * 4, s));
         CK(cudaMemsetAsync(misc + 5, 0, sizeof(uint32_t), s));
         // 1. lift + composite (slot, pane) keys; 2. stable sort; 3. (key, pane) segments; 4. partials; 5. merge into the rings
+        if (h->ff.grow) CK(cudaMemcpyAsync(misc + 6, misc + 4, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s)); // (ignored tuples before this batch)
         rc = h->ops->tb_lift(static_cast<const unsigned char *>(b.tuples), b.ts, b.n, h->ff, h->tb, F, h->tb_lifted, h->tb_kA, s, prm); if (rc) return rc;
+        for (bool grew = h->ff.grow != 0; grew; ) { // more keys than the capacity: grow, then lift the batch again
+            rc = tb_grow(h, s, &grew); if (rc) return rc;
+            if (!grew) break;
+            CK(cudaMemsetAsync(misc + 5, 0, sizeof(uint32_t), s));
+            CK(cudaMemcpyAsync(misc + 4, misc + 6, sizeof(uint32_t), cudaMemcpyDeviceToDevice, s)); // (the rerun counts this batch's late tuples again)
+            rc = h->ops->tb_lift(static_cast<const unsigned char *>(b.tuples), b.ts, b.n, h->ff, h->tb, F, h->tb_lifted, h->tb_kA, s, prm); if (rc) return rc;
+            h->launches += 2;
+        }
         uint32_t tb_need_bits = 2;
         { // the rings must hold every pane from a key's first pending one to its newest (PendingPanes_Queue::push_panes :367-372)
             uint32_t need = 0;
@@ -1301,6 +1502,7 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
                     uint32_t max_keys, int win_type, uint64_t lateness, uint32_t flags)
 {
     if (!hh || win == 0 || slide == 0 || wins_per_batch == 0 || max_keys == 0) return WFB_E_BADARG;
+    if ((flags & WFB_KEYS_GROW) && (flags & (WFB_FFAT_DENSE_KEYS | WFB_FFAT_PIPELINED))) return WFB_E_BADARG; // (dense: slot = key, nothing to grow)
     if (win_type == 1) return tb_create(hh, prog, win, slide, wins_per_batch, max_keys, lateness, flags);
     if (win_type != 0) return WFB_E_UNSUPPORTED;
     const ProgramOps *o = program(prog);
@@ -1374,9 +1576,7 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
         h->ingest_ctas_per_sm = e ? static_cast<uint32_t>(std::atoi(e)) : 2u;
     }
 #undef ALLOC
-    uint32_t bits = 0; while ((1ull << bits) < max_keys) bits++;
-    h->sort_passes = std::max(1u, (bits + 7) / 8);
-    h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
+    if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_ffat_destroy(h); return rc; } }
     { const char *e = std::getenv("WFB_BUCKET_MOVE"); h->bucket_move = e && std::atoi(e) != 0; }
     { const char *e = std::getenv("WFB_L2_HINTS"); h->l2_hints = !(e && std::atoi(e) == 0); }
     { const char *e = std::getenv("WFB_SPARSE"); h->sparse_ingest = !(e && std::atoi(e) == 0); }
@@ -1394,20 +1594,15 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
             if (std::getenv("WFB_VERBOSE")) std::fprintf(stderr, "[wfb] persisting L2: max %d MB, set %zu MB\n", maxp >> 20, want >> 20);
         }
     }
-    { // bucket path: every bucket holds at most BK_KEYS keys and the pane length fits 32 bits
-        const char *e = std::getenv("WFB_UPDATE");
-        h->buckets = !(e && std::strcmp(e, "lanes") == 0) && (1u << h->bucket_shift) <= BK_KEYS && ff.pane < (1ull << 32);
-        // streaming update: one path update per completed pane inside the item loop, so panes of a few items at least
-        // lazy FlatFAT levels (FfatDev::lazy): bucket path, the on-chip tree of one group must fit 32 KB, and building the n - 1 internal
-        // nodes once per fired group must be cheaper than a root path (log n nodes) per completed pane: a group fires every sp * Nb panes.
-        // (Nb = 1 with slide = pane fires on every pane: eager levels there. WFB_LAZY_TREE=0 / 1 forces either.)
-        { const char *lz = std::getenv("WFB_LAZY_TREE");
-          const bool fits = h->buckets && static_cast<size_t>(2) * ff.n_leaves * RB <= (32u << 10);
-          const bool pays = static_cast<uint64_t>(ff.n_leaves) <= 2ull * std::max(1u, ff.log_leaves) * ff.sp * ff.nb;
-          ff.lazy = (fits && (lz ? std::atoi(lz) != 0 : pays)) ? 1u : 0u; }
-        h->stream_update = h->buckets && !h->bucket_move && e && std::strcmp(e, "stream") == 0; // (measured: 173 us against 153 us for the bucket kernel at the bench configuration)
-        const char *t = std::getenv("WFB_TILE_H16");
-        h->tile_h16 = h->buckets && !(t && std::atoi(t) == 0);
+    ffat_derive_paths(h);
+    { // lazy FlatFAT levels (FfatDev::lazy): bucket path, the on-chip tree of one group must fit 32 KB, and building the n - 1 internal
+      // nodes once per fired group must be cheaper than a root path (log n nodes) per completed pane: a group fires every sp * Nb panes.
+      // (Nb = 1 with slide = pane fires on every pane: eager levels there. WFB_LAZY_TREE=0 / 1 forces either.) A growing handle keeps
+      // the layout it was created with when it leaves the bucket path: the update kernels of both paths read and write either one.
+        const char *lz = std::getenv("WFB_LAZY_TREE");
+        const bool fits = h->buckets && static_cast<size_t>(2) * ff.n_leaves * RB <= (32u << 10);
+        const bool pays = static_cast<uint64_t>(ff.n_leaves) <= 2ull * std::max(1u, ff.log_leaves) * ff.sp * ff.nb;
+        ff.lazy = (fits && (lz ? std::atoi(lz) != 0 : pays)) ? 1u : 0u;
         const char *rs = std::getenv("WFB_RANK_SCATTER");
         h->rank_scatter = !(rs && std::atoi(rs) == 0);
     }
@@ -1432,7 +1627,7 @@ int wfb_ffat_destroy(wfb_ffat_t *h)
     cudaFree(h->tb_popped); cudaFree(h->tb_popped_slots); cudaFree(h->tb_head); cudaFree(h->tb_seg);
     if (h->s2) cudaStreamDestroy(h->s2);
     for (auto &e : h->tev) cudaEventDestroy(e);
-    h->ts.destroy();
+    h->ts.destroy(); h->growc.destroy();
     delete h;
     cudaGetLastError();
     return 0;
@@ -1448,6 +1643,7 @@ int wfb_ffat_set_params(wfb_ffat_t *h, const void *params, size_t bytes)
     return 0;
 }
 uint64_t wfb_ffat_state_bytes(const wfb_ffat_t *h) { return h ? h->state_bytes : 0; }
+uint32_t wfb_ffat_key_capacity(const wfb_ffat_t *h) { return h ? h->ff.max_keys : 0; }
 int wfb_ffat_set_key_shard(wfb_ffat_t *h, uint32_t num_shards, uint32_t shard)
 {
     if (!h || num_shards == 0 || shard >= num_shards || !h->ff.dense || h->call_no != 0) return WFB_E_BADARG;
@@ -1475,8 +1671,7 @@ static int ffat_ensure_segment(wfb_ffat *h, SegScratch &g, uint32_t total, uint3
         if (h->move_payload || h->bucket_move) CK(cudaMalloc(&g.lifted_sorted, static_cast<size_t>(g.cap) * RB));
         CK(cudaMalloc(&g.slotsA, sizeof(uint32_t) * g.cap)); CK(cudaMalloc(&g.slotsB, sizeof(uint32_t) * g.cap));
         CK(cudaMalloc(&g.posA, sizeof(uint32_t) * g.cap)); CK(cudaMalloc(&g.posB, sizeof(uint32_t) * g.cap));
-        const uint64_t per_group = std::max<uint64_t>(1, h->ff.slide * h->ff.nb);
-        g.trig_cap = static_cast<uint32_t>(std::min<uint64_t>(g.cap / per_group + h->ff.max_keys + 1, 0x7fffffffull));
+        g.trig_cap = ffat_trig_cap(h, g.cap, h->ff.max_keys);
         CK(cudaMalloc(&g.trig, sizeof(Trigger) * g.trig_cap));
         if (h->pipelined) { // every group that can fire in one segment: trig_cap groups of Nb results
             g.res_cap = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(g.trig_cap) * h->ff.nb, 0x7fffffffull));
@@ -1623,98 +1818,108 @@ static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch
     }
     nbatches = static_cast<uint32_t>(hb.size());
     SEC(0);
-    // bucket path: no global compaction in the streaming pass -- tile t owns positions [t*TILE, +TILE) of the segment
-    const bool sparse = h->buckets && h->sparse_ingest;
-    const uint64_t seg_cap = sparse ? static_cast<uint64_t>(tiles) * TILE : total;
-    if (seg_cap > 0x7fffffffull) return WFB_E_BADARG;
-    rc = ffat_ensure_segment(h, g, static_cast<uint32_t>(seg_cap), nbatches, s); if (rc) return rc;
-    rc = h->ts.ensure_tiles(tiles); if (rc) return rc;
-    { int rc_ = h->ts.stage.h2d(g.d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
-    g.nbatches = nbatches; g.total = static_cast<uint32_t>(seg_cap); g.sparse = sparse;
-    if (sparse) { // first position of every batch (the compacting pass writes the compact offsets itself)
-        std::vector<uint32_t> boff(nbatches + 1);
-        for (uint32_t i = 0; i < nbatches; i++) boff[i] = hb[i].tile_begin * TILE;
-        boff[nbatches] = tiles * TILE;
-        { int rc_ = h->ts.stage.h2d(g.batch_off, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
-    }
-
-    SEC(1);
-    FfatDev ff = h->ff; // this call's view of the state: per-segment buffers of parity `par`
-    ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = g.trig_cap; ff.n_heavy = g.n_heavy;
-
-    const uint32_t npasses = h->buckets ? 1u : h->sort_passes;
-    const uint32_t pshift = h->buckets ? h->bucket_shift : 0u;
-    const bool fuse_hist = npasses <= 4; // the streaming pass also counts the digits of the slot sort that follows
-    if (fuse_hist) { rc = h->buckets ? RadixSorter::prepare_wide(g.sort_ctl, s) : RadixSorter::prepare(g.sort_ctl, npasses, s); if (rc) return rc; }
-    h->mark(0, s);
-    // 1. streaming pass: [map -> filter ->] lift, key -> slot, stable compaction over the whole segment
-    TileArgs a; std::memset(&a, 0, sizeof(a));
-    if (fuse_hist) { a.sort_ctl = g.sort_ctl; a.sort_passes = npasses; a.sort_shift = pshift; a.sort_dbits = h->buckets ? OSW_BITS : 8u; }
-    g.hist_ready = fuse_hist;
-    a.batches = g.d_batches; a.nbatches = nbatches; a.num_tiles = tiles;
-    a.lifted = g.lifted; a.slots = g.slotsA; a.batch_off = g.batch_off; a.n_total = g.n_total; a.ff = ff;
-    g.lifted_src = g.lifted;
-    if (sparse && !h->pipelined && !h->bucket_move && (h->ops->reserved & 1u) && h->inplace_ok) {
-        // pass-through program and every batch at its tile position inside one buffer: read the records where they are
-        const unsigned char *base = hb[0].tuples;
-        bool ok = (reinterpret_cast<uintptr_t>(base) & 15u) == 0;
-        for (uint32_t i = 0; ok && i < nbatches; i++) ok = hb[i].tuples == base + static_cast<size_t>(hb[i].tile_begin) * TILE * h->ops->tuple_bytes;
-        if (ok) { a.inplace = 1; g.lifted_src = base; a.ext_slots = ext_slots; }
-    }
-    if (ext_slots != nullptr && !a.inplace) return WFB_E_UNSUPPORTED; // (the front end always meets the in-place conditions)
-    h->ts.next_launch(a);
-    a.max_ctas_per_sm = h->ingest_ctas_per_sm;
-    a.l2_hints = h->l2_hints ? 1u : 0u;
-    a.sparse = sparse ? 1u : 0u;
-    a.count_keys = h->buckets ? 0u : 1u;
-    g.h32_ready = false;
-    if (sparse && fuse_hist && h->fuse_tile_hist && !h->pipelined) { // (pipelined: the rows would be shared by two segments in flight)
-        // the tile pass also files its digit counts per tile of the wide partition
-        rc = h->sorter.prepare_h32(g.total, s, &a.wide_h32); if (rc) return rc;
-        g.h32_ready = true;
-    }
-    g.h16_ready = false; g.ranked = false;
-    if (a.inplace && a.sort_passes <= 1 && h->ops->slots_inplace && h->inplace_kernel) {
-        // records read in place: only the slots (and the digit counts) are produced -- no tiles to stage, a plain kernel does it
-        if (sparse && fuse_hist && h->tile_h16 && !h->pipelined && !g.h32_ready) { // whole wide tiles per CTA: rows + ranks for the partition, as the tile pass does
-            rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc;
-            a.sort_ctl = nullptr;
-            g.h16_ready = true;
-            a.pack_rank = (h->rank_scatter && ff.max_keys <= 65536u) ? 1u : 0u;
-            g.ranked = a.pack_rank != 0;
+    FfatDev ff; // this call's view of the state: per-segment buffers of parity `par`
+    // the pass that inserts the call's keys into the key table; a growing handle runs it again after the table grew
+    const auto ingest = [&]() -> int {
+        // bucket path: no global compaction in the streaming pass -- tile t owns positions [t*TILE, +TILE) of the segment
+        const bool sparse = h->buckets && h->sparse_ingest;
+        const uint64_t seg_cap = sparse ? static_cast<uint64_t>(tiles) * TILE : total;
+        if (seg_cap > 0x7fffffffull) return WFB_E_BADARG;
+        rc = ffat_ensure_segment(h, g, static_cast<uint32_t>(seg_cap), nbatches, s); if (rc) return rc;
+        rc = h->ts.ensure_tiles(tiles); if (rc) return rc;
+        { int rc_ = h->ts.stage.h2d(g.d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
+        g.nbatches = nbatches; g.total = static_cast<uint32_t>(seg_cap); g.sparse = sparse;
+        if (sparse) { // first position of every batch (the compacting pass writes the compact offsets itself)
+            std::vector<uint32_t> boff(nbatches + 1);
+            for (uint32_t i = 0; i < nbatches; i++) boff[i] = hb[i].tile_begin * TILE;
+            boff[nbatches] = tiles * TILE;
+            { int rc_ = h->ts.stage.h2d(g.batch_off, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
         }
-        rc = h->ops->slots_inplace(a, pre ? static_cast<const void *>(pre) : h->pp(), s); if (rc) return rc;
-    } else {
-        uint32_t claims = tiles;
-        if (sparse && fuse_hist && h->tile_h16 && !g.h32_ready) {
-            // a CTA claims the 16 tiles of a wide tile at once, counts its digits in shared memory and files the row itself:
-            // the partition that follows needs neither a counting pass nor the per-CTA global digit counts
-            if (h->pipelined && (g.total + OSW_TILE - 1) / OSW_TILE > h->sorter.wide_tiles) CK(cudaStreamSynchronize(h->s2)); // (the rows are about to be re-allocated)
-            rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc; // (also sizes the chunk rows the partition needs)
-            if (h->pipelined) {
-                const uint32_t wt = (g.total + OSW_TILE - 1) / OSW_TILE;
-                if (wt > g.h16_tiles) {
-                    CK(cudaStreamSynchronize(s)); CK(cudaStreamSynchronize(h->s2));
-                    cudaFree(g.h16);
-                    g.h16_tiles = std::max(wt, 2 * g.h16_tiles);
-                    CK(cudaMalloc(&g.h16, sizeof(uint16_t) * OSW_DIGITS * g.h16_tiles));
-                }
-                a.wide_h16 = g.h16;
+
+        SEC(1);
+        ff = h->ff;
+        ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = g.trig_cap; ff.n_heavy = g.n_heavy;
+
+        const uint32_t npasses = h->buckets ? 1u : h->sort_passes;
+        const uint32_t pshift = h->buckets ? h->bucket_shift : 0u;
+        const bool fuse_hist = npasses <= 4; // the streaming pass also counts the digits of the slot sort that follows
+        if (fuse_hist) { rc = h->buckets ? RadixSorter::prepare_wide(g.sort_ctl, s) : RadixSorter::prepare(g.sort_ctl, npasses, s); if (rc) return rc; }
+        h->mark(0, s);
+        // 1. streaming pass: [map -> filter ->] lift, key -> slot, stable compaction over the whole segment
+        TileArgs a; std::memset(&a, 0, sizeof(a));
+        if (fuse_hist) { a.sort_ctl = g.sort_ctl; a.sort_passes = npasses; a.sort_shift = pshift; a.sort_dbits = h->buckets ? OSW_BITS : 8u; }
+        g.hist_ready = fuse_hist;
+        a.batches = g.d_batches; a.nbatches = nbatches; a.num_tiles = tiles;
+        a.lifted = g.lifted; a.slots = g.slotsA; a.batch_off = g.batch_off; a.n_total = g.n_total; a.ff = ff;
+        g.lifted_src = g.lifted;
+        if (sparse && !h->pipelined && !h->bucket_move && (h->ops->reserved & 1u) && h->inplace_ok) {
+            // pass-through program and every batch at its tile position inside one buffer: read the records where they are
+            const unsigned char *base = hb[0].tuples;
+            bool ok = (reinterpret_cast<uintptr_t>(base) & 15u) == 0;
+            for (uint32_t i = 0; ok && i < nbatches; i++) ok = hb[i].tuples == base + static_cast<size_t>(hb[i].tile_begin) * TILE * h->ops->tuple_bytes;
+            if (ok) { a.inplace = 1; g.lifted_src = base; a.ext_slots = ext_slots; }
+        }
+        if (ext_slots != nullptr && !a.inplace) return WFB_E_UNSUPPORTED; // (the front end always meets the in-place conditions)
+        h->ts.next_launch(a);
+        a.max_ctas_per_sm = h->ingest_ctas_per_sm;
+        a.l2_hints = h->l2_hints ? 1u : 0u;
+        a.sparse = sparse ? 1u : 0u;
+        a.count_keys = h->buckets ? 0u : 1u;
+        g.h32_ready = false;
+        if (sparse && fuse_hist && h->fuse_tile_hist && !h->pipelined) { // (pipelined: the rows would be shared by two segments in flight)
+            // the tile pass also files its digit counts per tile of the wide partition
+            rc = h->sorter.prepare_h32(g.total, s, &a.wide_h32); if (rc) return rc;
+            g.h32_ready = true;
+        }
+        g.h16_ready = false; g.ranked = false;
+        if (a.inplace && a.sort_passes <= 1 && h->ops->slots_inplace && h->inplace_kernel) {
+            // records read in place: only the slots (and the digit counts) are produced -- no tiles to stage, a plain kernel does it
+            if (sparse && fuse_hist && h->tile_h16 && !h->pipelined && !g.h32_ready) { // whole wide tiles per CTA: rows + ranks for the partition, as the tile pass does
+                rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc;
+                a.sort_ctl = nullptr;
+                g.h16_ready = true;
+                a.pack_rank = (h->rank_scatter && ff.max_keys <= 65536u) ? 1u : 0u;
+                g.ranked = a.pack_rank != 0;
             }
-            a.tiles_per_ticket = OSW_TILE_POS / TILE;
-            a.sort_ctl = nullptr; // (the chunk-sum kernel accumulates the global counts into g.sort_ctl, cleared above)
-            claims = (tiles + a.tiles_per_ticket - 1) / a.tiles_per_ticket;
-            g.h16_ready = true;
-            a.pack_rank = (h->rank_scatter && ff.max_keys <= 65536u) ? 1u : 0u;
-            g.ranked = a.pack_rank != 0;
+            rc = h->ops->slots_inplace(a, pre ? static_cast<const void *>(pre) : h->pp(), s); if (rc) return rc;
+        } else {
+            uint32_t claims = tiles;
+            if (sparse && fuse_hist && h->tile_h16 && !g.h32_ready) {
+                // a CTA claims the 16 tiles of a wide tile at once, counts its digits in shared memory and files the row itself:
+                // the partition that follows needs neither a counting pass nor the per-CTA global digit counts
+                if (h->pipelined && (g.total + OSW_TILE - 1) / OSW_TILE > h->sorter.wide_tiles) CK(cudaStreamSynchronize(h->s2)); // (the rows are about to be re-allocated)
+                rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc; // (also sizes the chunk rows the partition needs)
+                if (h->pipelined) {
+                    const uint32_t wt = (g.total + OSW_TILE - 1) / OSW_TILE;
+                    if (wt > g.h16_tiles) {
+                        CK(cudaStreamSynchronize(s)); CK(cudaStreamSynchronize(h->s2));
+                        cudaFree(g.h16);
+                        g.h16_tiles = std::max(wt, 2 * g.h16_tiles);
+                        CK(cudaMalloc(&g.h16, sizeof(uint16_t) * OSW_DIGITS * g.h16_tiles));
+                    }
+                    a.wide_h16 = g.h16;
+                }
+                a.tiles_per_ticket = OSW_TILE_POS / TILE;
+                a.sort_ctl = nullptr; // (the chunk-sum kernel accumulates the global counts into g.sort_ctl, cleared above)
+                claims = (tiles + a.tiles_per_ticket - 1) / a.tiles_per_ticket;
+                g.h16_ready = true;
+                a.pack_rank = (h->rank_scatter && ff.max_keys <= 65536u) ? 1u : 0u;
+                g.ranked = a.pack_rank != 0;
+            }
+            uint32_t grid = 0;
+            rc = h->ops->tile_pass(MODE_INGEST, a, pre ? static_cast<const void *>(pre) : h->pp(), claims, s, &grid, span_begin, span_end); if (rc) return rc;
+            h->ts.launched(claims, grid);
         }
-        uint32_t grid = 0;
-        rc = h->ops->tile_pass(MODE_INGEST, a, pre ? static_cast<const void *>(pre) : h->pp(), claims, s, &grid, span_begin, span_end); if (rc) return rc;
-        h->ts.launched(claims, grid);
+        h->launches++;
+        h->mark(1, s);
+        SEC(2);
+        return 0;
+    };
+    rc = ingest(); if (rc) return rc;
+    for (bool grew = h->ff.grow != 0; grew; ) { // more keys than the capacity: grow, then run the pass again
+        rc = ffat_grow(h, s, &grew); if (rc) return rc;
+        if (grew) { rc = ingest(); if (rc) return rc; h->launches++; }
     }
-    h->launches++;
-    h->mark(1, s);
-    SEC(2);
 
     if (!h->pipelined) {
         if (!h->append_results) CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t), s));

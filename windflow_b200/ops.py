@@ -34,6 +34,7 @@ RESULT_DTYPE = {PROG_TUPLE64: RESULT32, PROG_WFTEST16: WFWIN24, PROG_WFWIN24: WF
                 PROG_TUPLE64_FKEY: RESULT32D, PROG_TUPLE64_K16: RESULT48K}
 
 KEY_RR, KEY_UNIFORM, KEY_ZIPF = 0, 1, 2
+KEYS_GROW = 4  # WFB_KEYS_GROW
 SEED = 0x5EED5EED
 
 
@@ -196,12 +197,19 @@ class Engine:
 class KeyedState:
     """Per-operator keyed state of a stateful Map_GPU / Filter_GPU (wf/map_gpu.hpp:212-299, wf/filter_gpu.hpp:247-355)."""
 
-    def __init__(self, prog, max_keys, dense_keys=False):
+    def __init__(self, prog, max_keys, dense_keys=False, grow_keys=False):
+        """grow_keys: max_keys is the initial capacity, the table grows with the keys (WFB_KEYS_GROW)."""
         self.L = _lib.lib()
         if self.L.wfb_device_count() <= 0:
             raise RuntimeError("windflow_b200: no CUDA device (there is no CPU fallback)")
         self.h = C.c_void_p()
-        check(self.L.wfb_kstate_create(C.byref(self.h), prog, max_keys, 1 if dense_keys else 0), "wfb_kstate_create")
+        check(self.L.wfb_kstate_create(C.byref(self.h), prog, max_keys, (1 if dense_keys else 0) | (KEYS_GROW if grow_keys else 0)),
+              "wfb_kstate_create")
+
+    @property
+    def key_capacity(self):
+        """Keys the table holds now (max_keys, or what a growing table has grown to)."""
+        return int(self.L.wfb_kstate_key_capacity(self.h))
 
     def close(self):
         if self.h:
@@ -252,16 +260,17 @@ class FfatWindowsGPU:
     """Ffat_Windows_GPU replica state (wf/ffat_windows_gpu.hpp, wf/ffat_replica_gpu.hpp): count-based windows
     `withCBWindows(win, slide)`, `withNumWinPerBatch(nb)`."""
 
-    def __init__(self, prog, win, slide, nb, max_keys, dense_keys=False, win_type=0, lateness=0, pipelined=False):
+    def __init__(self, prog, win, slide, nb, max_keys, dense_keys=False, win_type=0, lateness=0, pipelined=False, grow_keys=False):
+        """grow_keys: max_keys is the initial capacity, the key table grows with the keys (WFB_KEYS_GROW)."""
         self.L = _lib.lib()
         if self.L.wfb_device_count() <= 0:
             raise RuntimeError("windflow_b200: no CUDA device (there is no CPU fallback)")
         self.prog, self.win, self.slide, self.nb, self.max_keys = prog, win, slide, nb, max_keys
         self.win_type = win_type  # 0 count-based, 1 time-based (win / slide / lateness in timestamp units)
         self.h = C.c_void_p()
-        self.pipelined = pipelined
+        self.pipelined, self.grow_keys = pipelined, grow_keys
         check(self.L.wfb_ffat_create(C.byref(self.h), prog, win, slide, nb, max_keys, win_type, lateness,
-                                     (1 if dense_keys else 0) | (2 if pipelined else 0)), "wfb_ffat_create")
+                                     (1 if dense_keys else 0) | (2 if pipelined else 0) | (KEYS_GROW if grow_keys else 0)), "wfb_ffat_create")
         self.res_dtype = RESULT_DTYPE[prog]
         self._keep = None
         self._max_items = 0  # largest segment seen: a pipelined handle delivers the previous call's results into this call's buffer
@@ -289,11 +298,20 @@ class FfatWindowsGPU:
         """Dense-key handle of one keyby shard: keys with key % num_shards == shard, slot = key // num_shards."""
         check(self.L.wfb_ffat_set_key_shard(self.h, num_shards, shard), "wfb_ffat_set_key_shard")
 
+    @property
+    def key_capacity(self):
+        """Keys the table holds now (max_keys, or what a growing table has grown to)."""
+        return int(self.L.wfb_ffat_key_capacity(self.h))
+
     def max_results(self, n_items):
         """Upper bound on the results one call over n_items input items can produce (count-based windows; time-based
         callers size the output for the groups a watermark jump can complete)."""
-        keys = self.max_keys if self.win_type == 0 else max(self.max_keys * 8, 65536)  # (time-based: a watermark jump completes several groups per key)
-        return (n_items // max(1, self.slide * self.nb) + keys + 1) * self.nb  # every key may fire one more group than its items alone account for
+        cap = self.key_capacity
+        keys = cap if self.win_type == 0 else max(cap * 8, 65536)  # (time-based: a watermark jump completes several groups per key)
+        groups = n_items // max(1, self.slide * self.nb) + keys + 1  # every key may fire one more group than its items alone account for
+        if self.grow_keys:  # a key new in the call fires its first group after B = (Nb-1)*slide + win of its items (time-based: a key of
+            groups += n_items if self.win_type else n_items // ((self.nb - 1) * self.slide + self.win)  # the call may fire with one item)
+        return groups * self.nb
 
     def process(self, batches, pre=None, out=None, out_ts=None, n_out=None, stream=None):
         """One stream segment (list of DeviceBatch). Returns (out uint8 tensor, out_ts int64 tensor, n_out tensor)."""
