@@ -7,7 +7,6 @@ run() { tag=$1; shift
   python -c "
 import json; d=json.load(open('gpurun_out/exp_$tag.json')); p=d['roofline']['phase_ms_per_step']; print('$tag', round(d['value']/1e9,2),'GT/s ms/step', round(d['ms_per_step'],3), {k:round(v,3) for k,v in p.items()}, d['gpu_launches'])" || tail -5 gpurun_out/exp_$tag.err
 }
-run lanes WFB_UPDATE=lanes
-run buckets WFB_UPDATE=buckets
-run buckets_move WFB_UPDATE=buckets WFB_BUCKET_MOVE=1
-WFB_UPDATE=buckets WFB_LIB=$PWD/windflow_b200/variants/lib_trace.so timeout 300 python tools/bk_trace.py
+run buckets
+run buckets_move WFB_BUCKET_MOVE=1
+WFB_LIB=$PWD/windflow_b200/variants/lib_trace.so timeout 300 python tools/bk_trace.py

@@ -100,7 +100,7 @@ struct FfatDev {
     uint32_t trig_cap;
     uint32_t *heavy;           // slots with more than light_max items in the segment (handled warp-per-key)
     uint32_t *n_heavy;
-    uint32_t light_max;
+    uint32_t light_max;        // 256 (a run-time value: as a constant, ptxas spills k_ffat_update_lanes)
     // window geometry (in tuples and in panes)
     uint64_t win, slide, B;    // B = (Nb-1)*slide + win  (ffat_replica_gpu.hpp:657)
     uint32_t nb;               // windows per trigger
@@ -134,8 +134,6 @@ struct TileArgs {
     uint32_t sparse;           // MODE_INGEST, 1: no global compaction -- tile t owns lifted / slots [t*TILE, +TILE) (survivors first,
                                // INVALID_SLOT padding), so tiles are independent: no look-back chain, positions are tuple indices
     uint32_t count_keys;       // MODE_INGEST: 1 = per-key item counts of the segment (ff.seg_cnt) for the full-sort update kernels
-    uint32_t *wide_h32;        // MODE_INGEST + sparse: per-tile digit counts of the wide partition that follows ([position / 4096][1024], 32-bit),
-                               // accumulated here so that the partition needs no counting pass of its own (null: it counts itself)
     uint16_t *wide_h16;        // MODE_INGEST + sparse: per-tile digit counts of the wide partition ([position / 4096][1024], 16-bit rows), filed by
                                // the tile pass itself: with tiles_per_ticket = 16 a CTA owns whole wide tiles, counts their digits in shared
                                // memory and writes each row once -- the partition then needs no counting pass (k_wide_tile_hist) of its own
@@ -595,8 +593,6 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
                     } else if (a.sort_ctl != nullptr && !(a.sparse && slot == INVALID_SLOT)) { // digit counts for the radix passes over the slots (invalid slots sort last / are skipped)
                         for (uint32_t ps = 0; ps < a.sort_passes; ps++)
                             atomicAdd(&s_hist[(ps << a.sort_dbits) + ((slot >> (a.sort_shift + a.sort_dbits * ps)) & ((1u << a.sort_dbits) - 1u))], 1u);
-                        if (a.wide_h32 != nullptr) // (tile t owns positions [256 t, +256): wide tile t / 16)
-                            atomicAdd(&a.wide_h32[static_cast<size_t>(m.tile / (OSW_TILE_POS / TILE)) * 1024u + ((slot >> a.sort_shift) & 1023u)], 1u);
                     }
                 }
             }
@@ -838,8 +834,7 @@ static __global__ void __launch_bounds__(1024) k_scan_u32(const uint32_t *in, ui
 // ------------------------------------------------------------------------------------------------------
 constexpr int OS_THREADS = 256;
 constexpr int OS_MAX_PASSES = 8;
-// elements per thread (ITEMS): <= 16 for 32-bit keys, <= 8 for 64-bit keys (static smem <= 48 KB)
-template <class K> struct OsCfg { static constexpr int MAX_ITEMS = sizeof(K) == 4 ? 16 : 8; };
+constexpr int OS_ITEMS = 8; // elements per thread of a pass
 
 template <class K>
 __global__ void __launch_bounds__(256) k_radix_ghist(const K *__restrict__ keys, const uint32_t *__restrict__ n_ptr, uint32_t n_host,
@@ -857,14 +852,12 @@ __global__ void __launch_bounds__(256) k_radix_ghist(const K *__restrict__ keys,
     for (uint32_t i = threadIdx.x; i < passes * 256; i += blockDim.x) if (h[i]) atomicAdd(&ctl[i], h[i]);
 }
 
-template <class K, int OS_ITEMS>
+template <class K>
 __global__ void __launch_bounds__(OS_THREADS) k_onesweep_pass(const K *__restrict__ keys_in, const uint32_t *__restrict__ vals_in,
                                                               K *__restrict__ keys_out, uint32_t *__restrict__ vals_out,
                                                               const uint32_t *__restrict__ n_ptr, uint32_t n_host, uint32_t pass,
                                                               uint32_t passes, uint32_t *__restrict__ ctl,
                                                               uint64_t *__restrict__ tile_state, uint32_t epoch,
-                                                              const unsigned char *__restrict__ payload_in,
-                                                              unsigned char *__restrict__ payload_out, uint32_t payload_bytes,
                                                               uint32_t *__restrict__ seg_first, uint32_t seg_first_n,
                                                               uint32_t base_shift)
 {
@@ -970,35 +963,23 @@ __global__ void __launch_bounds__(OS_THREADS) k_onesweep_pass(const K *__restric
         const uint32_t d = static_cast<uint32_t>(kk >> shift) & 255u;
         const uint32_t dst = bin_base[d] + (i - dig_off[d]);
         keys_out[dst] = kk;
-        const uint32_t v = svals[i];
-        vals_out[dst] = v;
+        vals_out[dst] = svals[i];
         // last pass of the window operator's sort: first sorted position of every key (entries start at 0xffffffff)
         if (seg_first != nullptr && static_cast<uint64_t>(kk) < seg_first_n) atomicMin(&seg_first[static_cast<uint32_t>(kk)], dst);
-        if (payload_out != nullptr) { // the last pass also moves the records: out[dst] = in[value]
-            if ((payload_bytes & 15u) == 0) {
-                const uint4 *src = reinterpret_cast<const uint4 *>(payload_in + static_cast<size_t>(v) * payload_bytes);
-                uint4 *dstp = reinterpret_cast<uint4 *>(payload_out + static_cast<size_t>(dst) * payload_bytes);
-                for (uint32_t q = 0; q < payload_bytes / 16; q++) dstp[q] = src[q];
-            } else {
-                const uint64_t *src = reinterpret_cast<const uint64_t *>(payload_in + static_cast<size_t>(v) * payload_bytes);
-                uint64_t *dstp = reinterpret_cast<uint64_t *>(payload_out + static_cast<size_t>(dst) * payload_bytes);
-                for (uint32_t q = 0; q < payload_bytes / 8; q++) dstp[q] = src[q];
-            }
-        }
     }
 }
 
 // ------------------------------------------------------------------------------------------------------
 // k_slots_inplace: the streaming pass of a pass-through program whose records already sit at their tile positions
 // (TileArgs::inplace): nothing is staged or copied, so a plain grid-stride kernel replaces k_tile_pass -- key -> slot (or the
-// caller's slot), INVALID_SLOT padding, the digit counts of the wide partition (shared-memory counts, one flush per CTA).
+// caller's slot), INVALID_SLOT padding, the 16-bit rows of the wide partition (TileArgs::wide_h16).
 // 32-byte records make 8-KB tiles, too small to amortise the tile pass's per-tile machinery (measured 1.2 TB/s there).
 // ------------------------------------------------------------------------------------------------------
 template <class P>
 __global__ void __launch_bounds__(256) k_slots_inplace(const TileArgs a, const typename P::params_t prm)
 {
     using T = typename P::tuple_t;
-    __shared__ uint32_t s_h[1024];
+    __shared__ uint32_t s_h[512];
     const uint32_t tid = threadIdx.x;
     const uint32_t npos = a.num_tiles * TILE;
     if (blockIdx.x == 0 && tid == 0 && a.ff.n_trig != nullptr) { *a.ff.n_trig = 0; *a.ff.n_heavy = 0; } // per-segment lists of the update kernels
@@ -1019,43 +1000,24 @@ __global__ void __launch_bounds__(256) k_slots_inplace(const TileArgs a, const t
         }
         return slot;
     };
-    if (a.wide_h16 != nullptr) {
-        // a CTA owns whole wide tiles (4096 positions): digit counts in shared memory (two 16-bit counters per word), one row per wide tile,
-        // and -- TileArgs::pack_rank -- every slot leaves with the count its digit had when it was counted (k_wide_scatter_ranked)
-        const uint32_t nwide = (npos + OSW_TILE_POS - 1) / OSW_TILE_POS;
-        for (uint32_t wt = blockIdx.x; wt < nwide; wt += gridDim.x) {
-            for (uint32_t i = tid; i < 512; i += blockDim.x) s_h[i] = 0;
-            __syncthreads();
-            for (uint32_t p = wt * OSW_TILE_POS + tid; p < min(npos, (wt + 1) * OSW_TILE_POS); p += blockDim.x) {
-                uint32_t slot = slot_at(p);
-                if (slot != INVALID_SLOT) {
-                    const uint32_t d = (slot >> a.sort_shift) & 1023u;
-                    const uint32_t before = atomicAdd(&s_h[d >> 1], 1u << ((d & 1u) * 16u));
-                    if (a.pack_rank) slot |= ((before >> ((d & 1u) * 16u)) & 0xffffu) << 16;
-                }
-                a.slots[p] = slot;
-            }
-            __syncthreads();
-            for (uint32_t i = tid; i < 512; i += blockDim.x) reinterpret_cast<uint32_t *>(a.wide_h16 + static_cast<size_t>(wt) * 1024u)[i] = s_h[i];
-            __syncthreads();
-        }
-        return;
-    }
-    const bool hist = a.sort_ctl != nullptr;
-    if (hist) for (uint32_t i = tid; i < 1024; i += blockDim.x) s_h[i] = 0;
-    __syncthreads();
-    const uint32_t dmask = (1u << a.sort_dbits) - 1u;
-    for (uint32_t p = blockIdx.x * blockDim.x + tid; p < npos; p += gridDim.x * blockDim.x) {
-        const uint32_t slot = slot_at(p);
-        if (slot != INVALID_SLOT) {
-            if (hist) atomicAdd(&s_h[(slot >> a.sort_shift) & dmask], 1u);
-            if (a.wide_h32 != nullptr) atomicAdd(&a.wide_h32[static_cast<size_t>(p / OSW_TILE_POS) * 1024u + ((slot >> a.sort_shift) & 1023u)], 1u);
-        }
-        a.slots[p] = slot;
-    }
-    if (hist) {
+    // a CTA owns whole wide tiles (4096 positions): digit counts in shared memory (two 16-bit counters per word), one row per wide tile,
+    // and -- TileArgs::pack_rank -- every slot leaves with the count its digit had when it was counted (k_wide_scatter_ranked)
+    const uint32_t nwide = (npos + OSW_TILE_POS - 1) / OSW_TILE_POS;
+    for (uint32_t wt = blockIdx.x; wt < nwide; wt += gridDim.x) {
+        for (uint32_t i = tid; i < 512; i += blockDim.x) s_h[i] = 0;
         __syncthreads();
-        for (uint32_t i = tid; i < (1u << a.sort_dbits) && i < 1024; i += blockDim.x) { const uint32_t c = s_h[i]; if (c) atomicAdd(&a.sort_ctl[i], c); }
+        for (uint32_t p = wt * OSW_TILE_POS + tid; p < min(npos, (wt + 1) * OSW_TILE_POS); p += blockDim.x) {
+            uint32_t slot = slot_at(p);
+            if (slot != INVALID_SLOT) {
+                const uint32_t d = (slot >> a.sort_shift) & 1023u;
+                const uint32_t before = atomicAdd(&s_h[d >> 1], 1u << ((d & 1u) * 16u));
+                if (a.pack_rank) slot |= ((before >> ((d & 1u) * 16u)) & 0xffffu) << 16;
+            }
+            a.slots[p] = slot;
+        }
+        __syncthreads();
+        for (uint32_t i = tid; i < 512; i += blockDim.x) reinterpret_cast<uint32_t *>(a.wide_h16 + static_cast<size_t>(wt) * 1024u)[i] = s_h[i];
+        __syncthreads();
     }
 }
 
@@ -1112,19 +1074,7 @@ __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_hist(const K *__restr
     }
 }
 
-// C[chunk][digit] = sum of the 32-bit per-tile rows of the chunk (when the tile pass filled them: no counting pass)
-static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums(const uint32_t *__restrict__ H32, uint32_t tiles, uint32_t chunk_shift, uint32_t *__restrict__ C)
-{
-    const uint32_t chunk = blockIdx.x, tid = threadIdx.x;
-    const uint32_t t0 = chunk << chunk_shift, t1 = min(tiles, t0 + (1u << chunk_shift));
-    uint4 acc = make_uint4(0, 0, 0, 0);
-    const uint4 *row = reinterpret_cast<const uint4 *>(H32) + tid;
-#pragma unroll 8
-    for (uint32_t t = t0; t < t1; t++) { const uint4 v = row[static_cast<size_t>(t) * (OSW_DIGITS / 4)]; acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w; }
-    reinterpret_cast<uint4 *>(C + static_cast<size_t>(chunk) * OSW_DIGITS)[tid] = acc;
-}
-
-// the same for the 16-bit rows the tile pass files (TileArgs::wide_h16)
+// C[chunk][digit] = sum of the 16-bit per-tile rows of the chunk that the tile pass files (TileArgs::wide_h16)
 static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums16(const uint16_t *__restrict__ H, uint32_t tiles, uint32_t chunk_shift, uint32_t *__restrict__ C,
                                                                           uint32_t *__restrict__ ctl_counts = nullptr)
 {
@@ -1149,8 +1099,7 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums16(const 
 // finish turns the chunk sums C[chunk][digit] into the first output position of every (chunk, digit) -- exclusive scan over the digits
 // of the totals + exclusive scan over the chunks, in place -- and sets ctl_counts[digit] = total of the digit. A tile's first output
 // position of digit d is then C[chunk][d] + T[tile][d]: two rows per scatter CTA, whatever the tile's place in its chunk.
-// `done` (one word, zero between launches: the last CTA clears it) counts the finished chunks. T = nullptr: only the chunk rows
-// (k_wide_scatter, which adds the earlier rows of its chunk itself).
+// `done` (one word, zero between launches: the last CTA clears it) counts the finished chunks.
 static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const uint16_t *__restrict__ H, uint32_t tiles, uint32_t chunk_shift, uint32_t chunks,
                                                                         uint32_t *__restrict__ C, uint32_t *__restrict__ T, uint32_t *__restrict__ ctl_counts,
                                                                         uint32_t *__restrict__ done)
@@ -1167,7 +1116,7 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const ui
 #pragma unroll 8
     for (uint32_t t = t0; t < t1; t++) {
         const ushort4 v = row[static_cast<size_t>(t) * (OSW_DIGITS / 4)];
-        if (T != nullptr) trow[static_cast<size_t>(t) * (OSW_DIGITS / 4)] = acc;
+        trow[static_cast<size_t>(t) * (OSW_DIGITS / 4)] = acc;
         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
     }
     uint4 *C4 = reinterpret_cast<uint4 *>(C);
@@ -1427,11 +1376,8 @@ __global__ void __launch_bounds__(OSW_THREADS, WFB_OSW_MINBLOCKS) k_wide_scatter
                                                               uint32_t chunk_shift, const uint16_t *__restrict__ H, const uint32_t *__restrict__ C,
                                                               const uint32_t *__restrict__ ctl_counts,
                                                               const unsigned char *__restrict__ payload_in, unsigned char *__restrict__ payload_out,
-                                                              uint32_t payload_bytes, uint32_t skip_invalid, uint32_t region_stride,
-                                                              const uint32_t *__restrict__ H32, uint32_t cx)
+                                                              uint32_t payload_bytes, uint32_t skip_invalid, uint32_t region_stride)
 {
-    // cx != 0: C holds the first output position of every (chunk, digit) already (k_wide_tile_bases); ctl_counts is not read
-    // H32 != nullptr: the per-tile counts are 32-bit rows filled by the producer of the keys (the tile pass) instead of H
     // region_stride != 0: bin d starts at d * region_stride (fixed-capacity regions; elements beyond the capacity are dropped)
     constexpr uint32_t NW = OSW_THREADS / 32;
     __shared__ __align__(16) uint16_t cntw[NW][OSW_DIGITS]; // per-warp digit counts -> exclusive offsets over the warps
@@ -1450,22 +1396,13 @@ __global__ void __launch_bounds__(OSW_THREADS, WFB_OSW_MINBLOCKS) k_wide_scatter
     {
         const uint32_t chunk = tile >> chunk_shift;
         const uint4 *crow = reinterpret_cast<const uint4 *>(C) + tid;
-        if (cx) { const uint4 v = crow[static_cast<size_t>(chunk) * (OSW_DIGITS / 4)]; acc[0] = v.x; acc[1] = v.y; acc[2] = v.z; acc[3] = v.w; }
-        else {
 #pragma unroll 8
-            for (uint32_t c = 0; c < chunk; c++) { const uint4 v = crow[static_cast<size_t>(c) * (OSW_DIGITS / 4)]; acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w; }
-        }
-        if (H32 != nullptr) {
-            const uint4 *hrow = reinterpret_cast<const uint4 *>(H32) + tid;
-#pragma unroll 8
-            for (uint32_t t = chunk << chunk_shift; t < tile; t++) { const uint4 v = hrow[static_cast<size_t>(t) * (OSW_DIGITS / 4)]; acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w; }
-        } else {
-            const ushort4 *hrow = reinterpret_cast<const ushort4 *>(H) + tid;
+        for (uint32_t c = 0; c < chunk; c++) { const uint4 v = crow[static_cast<size_t>(c) * (OSW_DIGITS / 4)]; acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w; }
+        const ushort4 *hrow = reinterpret_cast<const ushort4 *>(H) + tid;
 #pragma unroll 16
-            for (uint32_t t = chunk << chunk_shift; t < tile; t++) { const ushort4 v = hrow[static_cast<size_t>(t) * (OSW_DIGITS / 4)]; acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w; }
-        }
+        for (uint32_t t = chunk << chunk_shift; t < tile; t++) { const ushort4 v = hrow[static_cast<size_t>(t) * (OSW_DIGITS / 4)]; acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w; }
     }
-    const uint4 g4 = cx ? make_uint4(0, 0, 0, 0) : reinterpret_cast<const uint4 *>(ctl_counts)[tid];
+    const uint4 g4 = reinterpret_cast<const uint4 *>(ctl_counts)[tid];
     const uint32_t gsum = g4.x + g4.y + g4.z + g4.w;
     uint32_t incl = gsum;
 #pragma unroll
@@ -1695,7 +1632,7 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
                                                            const uint32_t *__restrict__ batch_off, const DevBatch *__restrict__ batches,
                                                            uint32_t nbatches, unsigned char *__restrict__ out_res,
                                                            uint64_t *__restrict__ out_ts, uint32_t out_cap, uint32_t *__restrict__ n_out,
-                                                           uint32_t gather, const typename P::params_t prm)
+                                                           const typename P::params_t prm)
 {
     using R = typename P::result_t;
     constexpr uint32_t RB = sizeof(R);
@@ -1735,7 +1672,7 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
                 alignas(16) R it[U];
                 const uint32_t k = min(U, m - j);
 #pragma unroll
-                for (uint32_t q = 0; q < U; q++) if (q < k) p[q] = gather ? sorted_pos[off + j + q] : (off + j + q);
+                for (uint32_t q = 0; q < U; q++) if (q < k) p[q] = sorted_pos[off + j + q];
 #pragma unroll
                 for (uint32_t q = 0; q < U; q++) if (q < k) ld_rec<R>(lifted + static_cast<size_t>(p[q]) * RB, it[q]);
 #pragma unroll
@@ -2280,286 +2217,8 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
 }
 
 // ------------------------------------------------------------------------------------------------------
-// k_ffat_update_stream: the window update as 32 independent STREAMS per warp -- no in-bucket sort, no per-key runs, no block
-// barriers in the loop. One CTA (2 warps) per bucket of the wide partition; warp w owns the bucket's keys [32 w, 32 w + 32) and
-// LANE k OF THE WARP IS KEY 32 w + k: the key's count, open pane (accumulator in registers), next leaf and next trigger live in
-// that lane's registers for the whole kernel, and the lane folds the key's items itself, in arrival order:
-//   producer  every warp reads the bucket's (slot, position) pairs in arrival order (128 per step, coalesced, prefetched one step
-//             ahead; the two warps share the lines through L1). The positions of the warp's own items go to PER-KEY FIFO queues in
-//             shared memory (match_any gives an item its rank among the group's items of the same key, the key lane's tail comes
-//             by shuffle): arrival order per key is queue order.
-//   consumer  in a round every lane pops the next position of ITS key, starts the copy of that record global -> shared (cp.async
-//             into a private 3-deep ring: no registers, no other lane involved) and folds the record it asked for three rounds ago
-//             into the open pane. All 32 lanes work on 32 different keys: a round costs ~40 warp instructions for up to 32
-//             items, and three gathers per lane are in flight. Rounds run whenever the queues hold two items per key on average.
-//   a lane that completes a pane writes the FlatFAT leaf and recomputes the root path -- with the siblings of the first leaf each
-//   key completes staged in shared memory at kernel start (cp.async by the key's own lane), so the usual completion issues no
-//   dependent global load; a fired group is deferred to k_ffat_windows; should the same key complete ANOTHER pane later in this
-//   call (it would overwrite ring leaves the deferred windows still read), the pending group is evaluated first by the whole warp
-//   and its list entry voided. No per-key item counts of the segment are needed for that decision (the bucket kernel counts first).
-// Built for panes of at least a few items (a pane per item would make every round a path update): the host selects
-// k_ffat_update_buckets otherwise.
-// ------------------------------------------------------------------------------------------------------
-#ifndef WFB_ST_MINBLOCKS
-#define WFB_ST_MINBLOCKS 7
-#endif
-constexpr uint32_t ST_THREADS = 64, ST_WARPS = ST_THREADS / 32;
-constexpr uint32_t ST_QCAP = 32;   // positions a key's queue holds (a whole group of 32 items of one key fits an empty queue)
-constexpr uint32_t ST_FLY = 3;     // gathers in flight per lane
-constexpr uint32_t ST_BACKLOG = 64; // consumer rounds run while the warp's queues hold at least this many items (two per key: few idle lanes)
-constexpr uint32_t ST_NONE = 0xffffffffu;
-static_assert(ST_WARPS * 32 == BK_KEYS, "one key per lane");
-
-template <class P>
-__global__ void __launch_bounds__(ST_THREADS, WFB_ST_MINBLOCKS) k_ffat_update_stream(const FfatDev ff, const unsigned char *__restrict__ lifted,
-                                                                     const uint32_t *__restrict__ bk_slots, const uint32_t *__restrict__ bk_pos,
-                                                                     const uint32_t *__restrict__ digit_counts, uint32_t shift,
-                                                                     const uint32_t *__restrict__ batch_off, const DevBatch *__restrict__ batches,
-                                                                     uint32_t nbatches, unsigned char *__restrict__ out_res,
-                                                                     uint64_t *__restrict__ out_ts, uint32_t out_cap, uint32_t *__restrict__ n_out,
-                                                                     const typename P::params_t prm)
-{
-    using R = typename P::result_t;
-    constexpr uint32_t RB = sizeof(R);
-    constexpr uint32_t DPT = OSW_DIGITS / ST_THREADS;
-    constexpr uint32_t CPB = (RB % 16 == 0) ? 16 : 8;
-    constexpr uint32_t SIBL = RB <= 32 ? 8 : (RB <= 64 ? 4 : (RB <= 128 ? 2 : 1)); // FlatFAT levels whose siblings are staged
-    static_assert(DPT % 4 == 0 && RB % 8 == 0, "layout");
-    __shared__ __align__(16) unsigned char s_sib[BK_KEYS * SIBL * RB];          // siblings of the leaf key k completes first (private to the key's lane)
-    __shared__ __align__(16) unsigned char s_stage[ST_THREADS * ST_FLY * RB];   // records in flight: ST_FLY per lane (private to the lane)
-    __shared__ uint32_t q_pos[ST_THREADS][ST_QCAP + 1];                         // per-key FIFO of arrival positions (+1: bank-conflict padding)
-    __shared__ uint32_t misc[ST_WARPS], s_boff[2];
-
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t bucket = blockIdx.x;
-    const uint32_t kpc = min(BK_KEYS, 1u << shift);
-    const uint32_t key_lo = bucket << shift;
-    const uint32_t n = ff.n_leaves, logn = ff.log_leaves;
-    const uint32_t P32 = static_cast<uint32_t>(ff.pane);
-    const uint64_t group_items = ff.slide * ff.nb;
-    const size_t tree_stride = static_cast<size_t>(2 * n - 1) * RB;
-
-    // ---- my key's state (loads first: they overlap the scan below) ------------------------------------------------------------------
-    const uint32_t my_k = tid; // local key of this lane
-    const bool has_key = my_k < kpc && key_lo + my_k < ff.max_keys;
-    const uint32_t my_slot = key_lo + my_k;
-    unsigned char *const my_tree = ff.tree + static_cast<size_t>(has_key ? my_slot : 0u) * tree_stride;
-    uint64_t st_c = 0;
-    alignas(16) R acc;
-    if (has_key) {
-        st_c = ff.cnt[my_slot];
-        ld_rec<R>(ff.acc + static_cast<size_t>(my_slot) * RB, acc);
-    }
-    // ---- bucket range = exclusive scan of the pass histogram ------------------------------------------------------------------------
-    {
-        uint32_t cc[DPT];
-#pragma unroll
-        for (uint32_t q = 0; q < DPT / 4; q++) {
-            const uint4 v = reinterpret_cast<const uint4 *>(digit_counts)[tid * (DPT / 4) + q];
-            cc[4 * q] = v.x; cc[4 * q + 1] = v.y; cc[4 * q + 2] = v.z; cc[4 * q + 3] = v.w;
-        }
-        uint32_t sum = 0;
-#pragma unroll
-        for (uint32_t q = 0; q < DPT; q++) sum += cc[q];
-        uint32_t incl = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if (lane >= static_cast<uint32_t>(o)) incl += v; }
-        if (lane == 31) misc[warp] = incl;
-        __syncthreads();
-        if (tid == bucket / DPT) {
-            uint32_t base = incl - sum;
-            for (uint32_t w = 0; w < warp; w++) base += misc[w];
-            uint32_t own = 0;
-#pragma unroll
-            for (uint32_t q = 0; q < DPT; q++) { if (q < bucket % DPT) base += cc[q]; if (q == bucket % DPT) own = cc[q]; }
-            s_boff[0] = base; s_boff[1] = base + own;
-        }
-    }
-    uint64_t g = 0, tt = 0;          // groups fired | ordinal (1-based, among the key's items of this call) of the item that fires the next group
-    uint32_t cp = 0, leaf = 0, cons = 0, pend = ST_NONE; // items in the open pane | leaf it becomes | items consumed in this call | deferred group of this call
-    bool staged = false;
-    if (has_key) {
-        const uint64_t c = st_c;
-        cp = static_cast<uint32_t>(c % P32); leaf = static_cast<uint32_t>((c / P32) & (n - 1));
-        if (c < ff.B) { g = 0; tt = ff.B - c; }
-        else { g = 1 + (c - ff.B) / group_items; tt = ff.B + g * group_items - c; }
-        for (uint32_t l = 0; l < (ff.lazy ? 0u : min(logn, SIBL)); l++) {
-            const unsigned char *src = my_tree + static_cast<size_t>(level_off(n, l) + ((leaf >> l) ^ 1u)) * RB;
-            unsigned char *dst = s_sib + (my_k * SIBL + l) * RB;
-#pragma unroll
-            for (uint32_t q = 0; q < RB / CPB; q++) cp_async<CPB>(dst + q * CPB, src + q * CPB);
-        }
-        staged = true;
-    }
-    __syncthreads();
-    const uint32_t b0 = s_boff[0], b1 = s_boff[1];
-    cp_async_wait_all(); // (the siblings are read by the lane that copied them)
-    if (b0 == b1) return;
-
-    // the whole warp evaluates the Nb windows of one fired group
-    auto eval_group = [&](uint32_t e_slot, key_words_t<P> e_key, uint64_t e_g, uint32_t e_pos, uint32_t e_obase) {
-        const unsigned char *e_tree = ff.tree + static_cast<size_t>(e_slot) * tree_stride;
-        const uint64_t wm = batch_watermark(batch_off, batches, nbatches, e_pos);
-        for (uint32_t i = lane; i < ff.nb; i += 32)
-            ffat_eval_window<P>(ff, e_tree, e_key, e_g * ff.nb + i, wm, e_obase + i, out_res, out_ts, out_cap, prm);
-    };
-
-    // ---- consumer: one round. Every lane: fold the record it asked for ST_FLY rounds ago, pop the next position of its key, ask for it --
-    uint32_t q_head = 0, q_tail = 0;     // my key's queue (indices grow; entry i lives at i % ST_QCAP)
-    uint32_t total = 0;                  // items queued in the whole warp (warp-uniform)
-    uint32_t fly_pos0 = 0, fly_pos1 = 0, fly_pos2 = 0; // positions of my gathers in flight, oldest first
-    uint32_t fly_valid = 0;              // bit i: fly_pos<i> is a real gather
-    uint32_t round_no = 0;               // warp-uniform: the stage slot of this round is round_no % ST_FLY
-    static_assert(ST_FLY == 3, "three gathers in flight per lane");
-    unsigned char *const my_stage = s_stage + static_cast<size_t>(tid) * ST_FLY * RB;
-    uint32_t *const my_q = &q_pos[tid][0];
-    auto consume_round = [&]() {
-        cp_async_wait_group<ST_FLY - 1>(); // the copy committed ST_FLY rounds ago has landed (one group per round, empty or not)
-        unsigned char *slot = my_stage + (round_no % ST_FLY) * RB;
-        const bool folded = (fly_valid & 1u) != 0;
-        const uint32_t it_pos = fly_pos0;
-        if (folded) {
-            alignas(16) R it;
-            ld_rec<R>(slot, it);
-            if (cp == 0) acc = it; else P::comb(acc, it, acc, prm);
-            cp++; cons++;
-        }
-        fly_pos0 = fly_pos1; fly_pos1 = fly_pos2; fly_valid >>= 1;
-        const bool popped = q_head != q_tail;
-        if (popped) {
-            const uint32_t pos = my_q[q_head % ST_QCAP];
-            q_head++;
-            const unsigned char *src = lifted + static_cast<size_t>(pos) * RB;
-#pragma unroll
-            for (uint32_t q = 0; q < RB / CPB; q++) cp_async<CPB>(slot + q * CPB, src + q * CPB);
-            fly_pos2 = pos; fly_valid |= 1u << (ST_FLY - 1);
-        }
-        cp_async_commit();
-        round_no++;
-        total -= __popc(__ballot_sync(FULL, popped));
-        if (!__any_sync(FULL, folded && cp == P32)) return;
-        // ---- some key completed a pane (about once per round): leaf, root path, fired group --------------------------------------------------
-        const bool completes = folded && cp == P32;
-        // a key about to overwrite ring leaves while a group of it is still deferred: evaluate that group first
-        uint32_t ev = __ballot_sync(FULL, completes && pend != ST_NONE);
-        while (ev) {
-            const int src = __ffs(ev) - 1;
-            ev &= ev - 1;
-            const uint32_t ti = __shfl_sync(FULL, pend, src);
-            const Trigger tr = ff.trig[ti];
-            eval_group(tr.slot, trig_key<P>(ff, tr), tr.g, tr.last_pos, tr.obase);
-            if (lane == static_cast<uint32_t>(src)) { ff.trig[ti].slot = INVALID_SLOT; pend = ST_NONE; } // k_ffat_windows skips voided entries
-            __syncwarp();
-        }
-        bool eval_now = false;
-        uint32_t ev_obase = 0; uint64_t ev_g = 0;
-        if (completes) {
-            cp = 0;
-            const uint32_t lf = leaf;
-            leaf = (leaf + 1) & (n - 1);
-            st_rec<R>(my_tree + static_cast<size_t>(lf) * RB, acc);
-            alignas(16) R cur = acc;
-            for (uint32_t l = 0; l < (ff.lazy ? 0u : logn); l++) { // (lazy: only the leaf is written)
-                alignas(16) R sb;
-                if (staged && l < SIBL) ld_rec<R>(s_sib + (my_k * SIBL + l) * RB, sb);
-                else ld_rec<R>(my_tree + static_cast<size_t>(level_off(n, l) + ((lf >> l) ^ 1u)) * RB, sb);
-                alignas(16) R parent = cur;
-                if ((lf >> l) & 1u) P::comb(sb, cur, parent, prm); else P::comb(cur, sb, parent, prm);
-                cur = parent;
-                st_rec<R>(my_tree + static_cast<size_t>(level_off(n, l + 1) + (lf >> (l + 1))) * RB, cur);
-            }
-            staged = false; // the next pane of the key reads the tree this one has just written
-            if (cons == tt) { // the group fires: Nb windows, evaluated after the update (k_ffat_windows)
-                const uint32_t obase = atomicAdd(n_out, ff.nb);
-                const uint32_t ti = atomicAdd(ff.n_trig, 1u);
-                if (ti < ff.trig_cap) {
-                    Trigger tr; tr.key = trig_word(key_of_slot<P>(ff, my_slot)); tr.g = g; tr.slot = my_slot; tr.last_pos = it_pos; tr.obase = obase; tr.pad = 0;
-                    ff.trig[ti] = tr;
-                    pend = ti;
-                } else { eval_now = true; ev_obase = obase; ev_g = g; } // list full: evaluate here
-                g++; tt += group_items;
-            }
-        }
-        uint32_t pd = __ballot_sync(FULL, eval_now);
-        while (pd) {
-            const int src = __ffs(pd) - 1;
-            pd &= pd - 1;
-            const uint32_t e_obase = __shfl_sync(FULL, ev_obase, src), e_pos = __shfl_sync(FULL, it_pos, src);
-            const uint64_t e_g = __shfl_sync(FULL, ev_g, src);
-            const uint32_t e_slot = key_lo + warp * 32u + static_cast<uint32_t>(src);
-            __syncwarp(); // the path nodes the source lane has just written
-            eval_group(e_slot, key_of_slot<P>(ff, e_slot), e_g, e_pos, e_obase);
-            __syncwarp();
-        }
-    };
-
-    // ---- the stream as ONE loop with one producer site and one consumer site (the consumer body is long: instantiating it at several call
-    // sites costs more in instruction-cache misses than it saves in branches) ---------------------------------------------------------
-    // producer: the bucket's pairs, 32 per step (loaded 128 at a time, one step ahead), into the per-key queues
-    uint32_t sl0, sl1, sl2, sl3, ps0, ps1, ps2, ps3;     // the 128 pairs being queued
-    uint32_t nsl0, nsl1, nsl2, nsl3, nps0, nps1, nps2, nps3; // the next 128, in flight
-    auto load4 = [&](uint32_t base, uint32_t &a0, uint32_t &a1, uint32_t &a2, uint32_t &a3, uint32_t &p0, uint32_t &p1, uint32_t &p2, uint32_t &p3) {
-        const uint32_t i0 = base + lane, i1 = i0 + 32, i2 = i0 + 64, i3 = i0 + 96;
-        a0 = i0 < b1 ? bk_slots[i0] : INVALID_SLOT; a1 = i1 < b1 ? bk_slots[i1] : INVALID_SLOT;
-        a2 = i2 < b1 ? bk_slots[i2] : INVALID_SLOT; a3 = i3 < b1 ? bk_slots[i3] : INVALID_SLOT;
-        p0 = i0 < b1 ? bk_pos[i0] : 0u; p1 = i1 < b1 ? bk_pos[i1] : 0u; p2 = i2 < b1 ? bk_pos[i2] : 0u; p3 = i3 < b1 ? bk_pos[i3] : 0u;
-    };
-    load4(b0, nsl0, nsl1, nsl2, nsl3, nps0, nps1, nps2, nps3);
-    sl0 = sl1 = sl2 = sl3 = INVALID_SLOT; ps0 = ps1 = ps2 = ps3 = 0;
-    uint32_t next_base = b0;  // first pair of the 128 in nsl/nps
-    uint32_t u = 4;           // group of the current 128 to queue next (4: fetch the next 128)
-    bool stream_done = false; // every pair of the bucket has been queued
-#pragma unroll 1
-    for (;;) {
-        bool want_round = total >= ST_BACKLOG || (stream_done && (total != 0 || __any_sync(FULL, fly_valid != 0)));
-        if (!want_round) {
-            if (stream_done) break;
-            if (u == 4) { // the 128 pairs loaded a step ago become current; the following 128 start to fly
-                if (next_base >= b1) { stream_done = true; continue; }
-                sl0 = nsl0; sl1 = nsl1; sl2 = nsl2; sl3 = nsl3; ps0 = nps0; ps1 = nps1; ps2 = nps2; ps3 = nps3;
-                next_base += 128;
-                load4(next_base, nsl0, nsl1, nsl2, nsl3, nps0, nps1, nps2, nps3);
-                u = 0;
-            }
-            const uint32_t slu = u == 0 ? sl0 : (u == 1 ? sl1 : (u == 2 ? sl2 : sl3));
-            const uint32_t psu = u == 0 ? ps0 : (u == 1 ? ps1 : (u == 2 ? ps2 : ps3));
-            const uint32_t lkf = slu - key_lo; // (slots outside the bucket's keys, the padding included, wrap to large values)
-            const bool mine = lkf < kpc && (lkf >> 5) == warp;
-            const uint32_t lk = lkf & 31u;
-            const uint32_t mmask = __ballot_sync(FULL, mine);
-            if (mmask == 0) { u++; continue; }
-            // key-lane view: the group's items of MY key (five ballots transpose the item keys into one mask per key lane)
-            uint32_t m = mmask;
-#pragma unroll
-            for (uint32_t b = 0; b < 5; b++) { const uint32_t B = __ballot_sync(FULL, mine && ((lk >> b) & 1u)); m &= ((lane >> b) & 1u) ? B : ~B; }
-            const uint32_t incoming = __popc(m);
-            want_round = __any_sync(FULL, q_tail - q_head + incoming > ST_QCAP); // (a key that floods its queue: drain a round, then retry this group)
-            if (!want_round) {
-                // item-lane view: my rank among the group's items of my key, my key's tail
-                const uint32_t peers = __match_any_sync(FULL, mine ? lk : 32u + lane);
-                const uint32_t tail = __shfl_sync(FULL, q_tail, lk);
-                if (mine) q_pos[warp * 32u + lk][(tail + __popc(peers & lanemask_lt())) % ST_QCAP] = psu;
-                q_tail += incoming;
-                total += __popc(mmask);
-                u++;
-                __syncwarp(); // the queue entries are visible to the key lanes
-                continue;
-            }
-        }
-        consume_round();
-    }
-    cp_async_wait_all();
-    // ---- my key's state back -----------------------------------------------------------------------------------------------------------
-    if (has_key && cons != 0) {
-        ff.cnt[my_slot] = st_c + cons;
-        if (cp) st_rec<R>(ff.acc + static_cast<size_t>(my_slot) * RB, acc);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------
-// k_ffat_update: one warp per key that received items in this stream segment.
-//   items of the key, in arrival order: lifted[sorted_pos[seg_off[slot] .. +seg_cnt[slot])] (gather = 1), or, when the last
-//   sort pass also moved the records (gather = 0), lifted[seg_off[slot] .. +seg_cnt[slot])
+// k_ffat_update: one warp per key that k_ffat_update_lanes put on the heavy list.
+//   items of the key, in arrival order: lifted[sorted_pos[seg_off[slot] .. +seg_cnt[slot])]
 //   -> ordered warp fold into the open pane (pane = gcd(win, slide) items)
 //   -> completed pane = new FlatFAT leaf (ring of n_leaves panes) + recompute of its root path
 //   -> when the key's count reaches the trigger: Nb window queries (greedy aligned-node fold, the same walk as
@@ -2637,7 +2296,6 @@ __global__ void __launch_bounds__(256) k_ffat_windows(const FfatDev ff, const ui
     for (uint64_t w = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; w < total; w += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
         const uint32_t ti = static_cast<uint32_t>(w / ff.nb), i = static_cast<uint32_t>(w % ff.nb);
         const Trigger tr = ff.trig[ti];
-        if (tr.slot == INVALID_SLOT) continue; // evaluated inside the update kernel (k_ffat_update_stream)
         const uint64_t wm = batch_watermark(batch_off, batches, nbatches, tr.last_pos);
         ffat_eval_window<P>(ff, ff.tree + static_cast<size_t>(tr.slot) * tree_stride, trig_key<P>(ff, tr), tr.g * ff.nb + i, wm, tr.obase + i,
                             out_res, out_ts, out_cap, prm);
@@ -2669,7 +2327,6 @@ __global__ void __launch_bounds__(128) k_ffat_windows_lazy(const FfatDev ff, con
     FfatDev fs = ff; fs.lazy = 0; // the on-chip tree has every level: the ordinary walk
     for (uint32_t ti = blockIdx.x * wpb + warp; ti < nt; ti += gridDim.x * wpb) {
         const Trigger tr = ff.trig[ti];
-        if (tr.slot == INVALID_SLOT) continue; // evaluated inside the update kernel
         const unsigned char *leaves = ff.tree + static_cast<size_t>(tr.slot) * tree_stride;
         for (uint32_t i = lane; i < n * (RB / 8); i += 32) reinterpret_cast<uint64_t *>(t)[i] = reinterpret_cast<const uint64_t *>(leaves)[i];
         __syncwarp();
@@ -2698,23 +2355,21 @@ __global__ void __launch_bounds__(256) k_ffat_update(const FfatDev ff, const uns
                                                      const uint32_t *__restrict__ batch_off, const DevBatch *__restrict__ batches,
                                                      uint32_t nbatches, unsigned char *__restrict__ out_res,
                                                      uint64_t *__restrict__ out_ts, uint32_t out_cap, uint32_t *__restrict__ n_out,
-                                                     uint32_t gather, const typename P::params_t prm, uint32_t use_heavy_list)
+                                                     const typename P::params_t prm)
 {
     using R = typename P::result_t;
     constexpr uint32_t RB = sizeof(R);
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t nslots = ff.dense ? ff.max_keys : min(*ff.n_slots, ff.max_keys);
     const uint32_t n = ff.n_leaves, logn = ff.log_leaves;
     const uint64_t P_ = ff.pane;
     const uint64_t group_items = ff.slide * ff.nb;
     const size_t tree_stride = static_cast<size_t>(2 * n - 1) * RB;
 
-    // use_heavy_list = 1: only the keys k_ffat_update_lanes put on the heavy list; 0: every key of the segment
-    const uint32_t nwork = use_heavy_list ? min(*ff.n_heavy, ff.max_keys) : nslots;
+    const uint32_t nwork = min(*ff.n_heavy, ff.max_keys);
     for (uint32_t wi = gwarp; wi < nwork; wi += nwarps) {
-        const uint32_t slot = use_heavy_list ? ff.heavy[wi] : wi;
+        const uint32_t slot = ff.heavy[wi];
         const uint32_t m = ff.seg_cnt[slot];
         if (m == 0) continue;
         const uint32_t off = ff.seg_off[slot];
@@ -2725,11 +2380,6 @@ __global__ void __launch_bounds__(256) k_ffat_update(const FfatDev ff, const uns
         if (c % P_ != 0) ld_rec<R>(ff.acc + static_cast<size_t>(slot) * RB, acc); // every lane keeps a copy
         uint64_t g = (c < ff.B) ? 0 : 1 + (c - ff.B) / group_items;
         uint64_t trig = ff.B + g * group_items;
-        if (!gather) { // pull the key's (contiguous) records towards L2 before the chunk loop needs them
-            const unsigned char *seg = lifted + static_cast<size_t>(off) * RB;
-            const uint32_t lines = (m * RB + 127u) / 128u;
-            for (uint32_t l = lane; l < lines && l < 128u; l += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(seg + static_cast<size_t>(l) * 128u));
-        }
 
         uint32_t j = 0;
         while (j < m) {
@@ -2737,8 +2387,7 @@ __global__ void __launch_bounds__(256) k_ffat_update(const FfatDev ff, const uns
             const uint32_t take = min(min(32u, m - j), room);
             alignas(16) R r;
             if (lane < take) {
-                const uint32_t p = gather ? sorted_pos[off + j + lane] : (off + j + lane);
-                ld_rec<R>(lifted + static_cast<size_t>(p) * RB, r);
+                ld_rec<R>(lifted + static_cast<size_t>(sorted_pos[off + j + lane]) * RB, r);
             }
             // ordered fold: after the step with stride o, lane l holds items [l, l+2o) (clipped to take)
 #pragma unroll

@@ -65,7 +65,7 @@ struct ProgramOps {
                      uint64_t span_begin, uint64_t span_end);
     int (*ffat_update)(const FfatDev &ff, const unsigned char *lifted, const uint32_t *sorted_pos, const uint32_t *batch_off,
                        const DevBatch *batches, uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts,
-                       uint32_t out_cap, uint32_t *n_out, uint32_t grid, cudaStream_t s, uint32_t gather, const void *params, uint32_t lanes_grid);
+                       uint32_t out_cap, uint32_t *n_out, uint32_t grid, cudaStream_t s, const void *params, uint32_t lanes_grid);
     int (*ffat_buckets)(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_slots, const uint32_t *bk_pos,
                         const uint32_t *digit_counts, uint32_t shift, uint32_t moved, const uint32_t *batch_off, const DevBatch *batches,
                         uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts, uint32_t out_cap, uint32_t *n_out, cudaStream_t s,
@@ -108,11 +108,6 @@ struct ProgramOps {
     int (*reduce_segments_batches)(const DevBatch *batches, const uint32_t *boff, const uint64_t *skeys, const uint32_t *sidx,
                                    const uint32_t *seg_begin, const uint32_t *first_seg, const uint32_t *n_segs, uint32_t key_bits,
                                    uint32_t total, uint32_t *long_list, uint32_t *n_long, cudaStream_t s, const void *params);
-    // window update after the wide partition, streaming variant (k_ffat_update_stream): same contract as ffat_buckets, records gathered
-    int (*ffat_stream)(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_slots, const uint32_t *bk_pos,
-                       const uint32_t *digit_counts, uint32_t shift, const uint32_t *batch_off, const DevBatch *batches,
-                       uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts, uint32_t out_cap, uint32_t *n_out, cudaStream_t s,
-                       const void *params);
     // key_t (wfb_keys.cuh): bytes of its canonical words (8 or 16), KEY_KIND_* and sizeof(key_t) (the order words of a key that is not
     // an integer have no bits above 8 * key_size: a float's fit in 32)
     uint32_t key_bytes, key_kind, key_size;
@@ -174,18 +169,13 @@ int tile_pass_dispatch(int mode, TileArgs &a, const void *params, uint32_t want_
 template <class P>
 int ffat_update_dispatch(const FfatDev &ff, const unsigned char *lifted, const uint32_t *sorted_pos, const uint32_t *batch_off,
                          const DevBatch *batches, uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts,
-                         uint32_t out_cap, uint32_t *n_out, uint32_t grid, cudaStream_t s, uint32_t gather, const void *params,
-                         uint32_t lanes_grid)
+                         uint32_t out_cap, uint32_t *n_out, uint32_t grid, cudaStream_t s, const void *params, uint32_t lanes_grid)
 {
+    // thread-per-key pass for the light keys, then warp-per-key only for the heavy list it produced
     const typename P::params_t prm = load_params<P>(params);
-    if (lanes_grid) { // thread-per-key pass for the light keys, then warp-per-key only for the heavy list it produced
-        k_ffat_update_lanes<P><<<lanes_grid, 128, 0, s>>>(ff, lifted, sorted_pos, batch_off, batches, nbatches, out_res, out_ts, out_cap, n_out,
-                                                           gather, prm);
-        k_ffat_update<P><<<std::max(1u, std::min(grid, static_cast<uint32_t>(wfb::num_sms()) * 2u)), 256, 0, s>>>(
-            ff, lifted, sorted_pos, batch_off, batches, nbatches, out_res, out_ts, out_cap, n_out, gather, prm, 1u);
-    } else {
-        k_ffat_update<P><<<grid, 256, 0, s>>>(ff, lifted, sorted_pos, batch_off, batches, nbatches, out_res, out_ts, out_cap, n_out, gather, prm, 0u);
-    }
+    k_ffat_update_lanes<P><<<lanes_grid, 128, 0, s>>>(ff, lifted, sorted_pos, batch_off, batches, nbatches, out_res, out_ts, out_cap, n_out, prm);
+    k_ffat_update<P><<<std::max(1u, std::min(grid, static_cast<uint32_t>(wfb::num_sms()) * 2u)), 256, 0, s>>>(
+        ff, lifted, sorted_pos, batch_off, batches, nbatches, out_res, out_ts, out_cap, n_out, prm);
     WFB_CK(cudaGetLastError());
     return 0;
 }
@@ -200,18 +190,6 @@ int ffat_buckets_dispatch(const FfatDev &ff, const unsigned char *lifted, const 
                                                                                  nbatches, out_res, out_ts, out_cap, n_out, load_params<P>(params));
     else k_ffat_update_buckets<P, false><<<OSW_DIGITS, BK_THREADS, 0, s>>>(ff, lifted, bk_slots, bk_pos, digit_counts, shift, moved, batch_off, batches,
                                                                           nbatches, out_res, out_ts, out_cap, n_out, load_params<P>(params));
-    WFB_CK(cudaGetLastError());
-    return 0;
-}
-
-template <class P>
-int ffat_stream_dispatch(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_slots, const uint32_t *bk_pos,
-                         const uint32_t *digit_counts, uint32_t shift, const uint32_t *batch_off, const DevBatch *batches,
-                         uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts, uint32_t out_cap, uint32_t *n_out, cudaStream_t s,
-                         const void *params)
-{
-    k_ffat_update_stream<P><<<OSW_DIGITS, ST_THREADS, 0, s>>>(ff, lifted, bk_slots, bk_pos, digit_counts, shift, batch_off, batches,
-                                                              nbatches, out_res, out_ts, out_cap, n_out, load_params<P>(params));
     WFB_CK(cudaGetLastError());
     return 0;
 }
@@ -412,7 +390,6 @@ const void *lifted_ops_of()
         t.params_bytes = sizeof(typename L::params_t); t.reserved = 1u; // pass-through
         t.tile_pass = &tile_pass_ingest_dispatch<L>; t.slots_inplace = &slots_inplace_dispatch<L>;
         t.ffat_update = &ffat_update_dispatch<L>; t.ffat_buckets = &ffat_buckets_dispatch<L>; t.ffat_windows = &ffat_windows_dispatch<L>;
-        t.ffat_stream = &ffat_stream_dispatch<L>;
         t.key_bytes = 8u * key_codec<L>::words; t.key_kind = key_codec<L>::kind; t.key_size = sizeof(typename L::key_t);
         t.reserved2 = program_has_result_key<P>::value ? 1u : 0u; // bit 0: the lifted records carry their key (usable behind an exchange)
         return t;
@@ -430,7 +407,6 @@ ProgramOps make_ops()
     o.tile_pass = &tile_pass_dispatch<P>;
     o.ffat_update = &ffat_update_dispatch<P>;
     o.ffat_buckets = &ffat_buckets_dispatch<P>;
-    o.ffat_stream = &ffat_stream_dispatch<P>;
     o.ffat_windows = &ffat_windows_dispatch<P>;
     o.extract_keys = &extract_keys_dispatch<P>;
     o.reduce_segments = &reduce_segments_dispatch<P>;

@@ -148,18 +148,9 @@ struct RadixSorter {
         }
         return 0;
     }
-    void destroy() { cudaFree(ctl); cudaFree(state); cudaFree(wideH); cudaFree(wideC); cudaFree(wideT); cudaFree(wideDone); cudaFree(wideH32); }
+    void destroy() { cudaFree(ctl); cudaFree(state); cudaFree(wideH); cudaFree(wideC); cudaFree(wideT); cudaFree(wideDone); }
 
     // stable sort of (kA[i], i) by the low 8*passes bits; n on the device (n_ptr) or the host (n_host), cap = upper bound
-    template <class K, int ITEMS>
-    void launch_pass(uint32_t tiles, const K *kin, const uint32_t *vin, K *kout, uint32_t *vout, const uint32_t *n_ptr, uint32_t n_host,
-                     uint32_t p, uint32_t passes, cudaStream_t s, const unsigned char *pin, unsigned char *pout, uint32_t pbytes,
-                     uint32_t *seg_first, uint32_t seg_first_n, uint32_t base_shift)
-    {
-        k_onesweep_pass<K, ITEMS><<<tiles, OS_THREADS, 0, s>>>(kin, vin, kout, vout, n_ptr, n_host, p, passes, ctl, state, epoch,
-                                                               pin, pout, pbytes, seg_first, seg_first_n, base_shift);
-    }
-
     // clears the histograms / tickets of the next sort; call it BEFORE a producer that fills the histograms itself
     static constexpr size_t CTL_WORDS = OS_MAX_PASSES * 256 + OS_MAX_PASSES > OSW_DIGITS + 1 ? OS_MAX_PASSES * 256 + OS_MAX_PASSES : OSW_DIGITS + 1;
     static int prepare(uint32_t *ctl_buf, uint32_t passes, cudaStream_t s)
@@ -180,21 +171,6 @@ struct RadixSorter {
     uint16_t *wideH = nullptr; uint32_t *wideC = nullptr; uint32_t wide_tiles = 0, wide_chunks = 0;
     uint32_t *wideT = nullptr;    // [tiles][1024]: sum of the earlier rows of the tile's chunk (k_wide_tile_bases)
     uint32_t *wideDone = nullptr; // finished chunks of k_wide_tile_bases (zero between launches)
-    uint32_t *wideH32 = nullptr; uint32_t wide32_tiles = 0; // per-tile counts filled by the producer of the keys (32-bit rows)
-    // rows for `cap` positions, zeroed on stream s: the producer adds its digit counts, sort_wide(..., h32_ready) consumes them
-    int prepare_h32(uint32_t cap, cudaStream_t s, uint32_t **rows)
-    {
-        const uint32_t tiles = std::max(1u, (cap + OSW_TILE - 1) / OSW_TILE);
-        if (tiles > wide32_tiles) {
-            CK(cudaStreamSynchronize(s));
-            cudaFree(wideH32);
-            wide32_tiles = std::max(tiles, 2 * wide32_tiles);
-            CK(cudaMalloc(&wideH32, sizeof(uint32_t) * OSW_DIGITS * wide32_tiles));
-        }
-        CK(cudaMemsetAsync(wideH32, 0, sizeof(uint32_t) * OSW_DIGITS * tiles, s));
-        *rows = wideH32;
-        return 0;
-    }
     // tiles of the wide pass over `cap` positions and their chunks. prefix = false: about sqrt(tiles) chunks of >= 16 tiles, every
     // scatter CTA sums the rows of the earlier chunks itself; true (rows filed by the tile pass): chunks of 32 tiles; one kernel
     // (k_wide_tile_bases) computes the first output positions of every chunk and the in-chunk offsets of every tile, so a scatter
@@ -235,45 +211,40 @@ struct RadixSorter {
         *rows = wideH;
         return 0;
     }
-    const uint16_t *rows_override = nullptr; // set by sort_wide for the duration of one call
-    template <class K> static bool keys_out_ok(K *kout, uint32_t *vout) { return kout != nullptr && vout != nullptr; }
     template <class K, int RBYTES>
     void launch_wide_scatter(uint32_t tiles, const K *kin, K *kout, uint32_t *vout, const uint32_t *n_ptr, uint32_t n_host, uint32_t shift,
                              uint32_t chunk_shift, const uint32_t *c, cudaStream_t s, const unsigned char *pin, unsigned char *pout, uint32_t pbytes,
-                             uint32_t skip_invalid, uint32_t region_stride, const uint32_t *h32, uint32_t cx)
+                             uint32_t skip_invalid, uint32_t region_stride)
     {
-        k_wide_scatter<K, RBYTES><<<tiles, OSW_THREADS, 0, s>>>(kin, kout, vout, n_ptr, n_host, shift, chunk_shift, rows_override ? rows_override : wideH, wideC, c, pin, pout, pbytes, skip_invalid, region_stride, h32, cx);
+        k_wide_scatter<K, RBYTES><<<tiles, OSW_THREADS, 0, s>>>(kin, kout, vout, n_ptr, n_host, shift, chunk_shift, wideH, wideC, c, pin, pout, pbytes, skip_invalid, region_stride);
     }
     // payload_in / payload_out (optional): payload_bytes-sized records that travel with the elements (multiple of 8 bytes)
+    // ready_ctl: the producer of the keys (the tile pass) cleared it and filed the 16-bit rows of the wide tiles (TileArgs::wide_h16) --
+    // in h16_rows when they do not live in this sorter (a pipelined handle keeps one set per segment in flight) -- and, without few_bins,
+    // packed a rank with every key (TileArgs::pack_rank), by which k_wide_scatter_ranked places them. Null: k_wide_tile_hist counts.
     template <class K>
     int sort_wide(const K *kin, K *kout, uint32_t *vout, const uint32_t *n_ptr, uint32_t n_host, uint32_t cap, uint32_t shift,
                   cudaStream_t s, uint32_t *ready_ctl, const uint32_t **counts, const unsigned char *payload_in = nullptr,
                   unsigned char *payload_out = nullptr, uint32_t payload_bytes = 0, bool skip_invalid = false, uint32_t region_stride = 0, uint32_t few_bins = 0,
-                  bool h32_ready = false, bool h16_ready = false, uint16_t *h16_rows = nullptr, bool ranked = false)
+                  const uint16_t *h16_rows = nullptr)
     {
-        // ranked: the keys carry a rank in their upper half (TileArgs::pack_rank): k_wide_scatter_ranked
-        // h16_rows: the 16-bit rows the tile pass filed when they do not live in this sorter (a pipelined handle keeps one set per segment in flight)
         if (payload_in && (payload_bytes == 0 || (payload_bytes & 7u))) return WFB_E_BADARG;
         if (!ctl) CK(cudaMalloc(&ctl, sizeof(uint32_t) * CTL_WORDS));
-        const bool prefix = h16_ready && ready_ctl && !few_bins;
-        rows_override = prefix ? h16_rows : nullptr;
+        const bool ranked = ready_ctl && !few_bins;
+        const uint16_t *rows = h16_rows ? h16_rows : wideH;
         uint32_t tiles, chunk_shift, chunks;
-        wide_geometry(cap, prefix, &tiles, &chunk_shift, &chunks);
+        wide_geometry(cap, ranked, &tiles, &chunk_shift, &chunks);
         { int rc = ensure_wide_buffers(tiles, chunks, s); if (rc) return rc; }
         uint32_t *c = ready_ctl ? ready_ctl : ctl;
         if (!ready_ctl) { int rc = prepare_wide(c, s); if (rc) return rc; }
-        const uint32_t *h32 = nullptr;
-        if (h16_ready && ready_ctl && few_bins) { // a few bins (destinations), rows filed by the tile pass: chunk sums + the global counts (c was cleared by the caller)
-            k_wide_chunk_sums16<<<chunks, OSW_THREADS, 0, s>>>(h16_rows ? h16_rows : wideH, tiles, chunk_shift, wideC, c);
-        } else if (prefix) { // the tile pass filed the 16-bit rows (wideH): first output position of every (chunk, digit) and (tile, digit) + digit counts
+        if (ranked) { // first output position of every (chunk, digit) and (tile, digit) + digit counts
             if (!wideDone) { CK(cudaMalloc(&wideDone, sizeof(uint32_t))); CK(cudaMemsetAsync(wideDone, 0, sizeof(uint32_t), s)); }
-            k_wide_tile_bases<<<chunks, OSW_THREADS, 0, s>>>(h16_rows ? h16_rows : wideH, tiles, chunk_shift, chunks, wideC, ranked ? wideT : nullptr, c, wideDone);
-        } else if (h32_ready && ready_ctl && !few_bins) { // the producer of the keys counted the digits per tile: only the chunk sums are missing
-            k_wide_chunk_sums<<<chunks, OSW_THREADS, 0, s>>>(wideH32, tiles, chunk_shift, wideC);
-            h32 = wideH32;
+            k_wide_tile_bases<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, chunks, wideC, wideT, c, wideDone);
+        } else if (ready_ctl) { // a few bins (destinations): chunk sums + the global counts
+            k_wide_chunk_sums16<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, wideC, c);
         } else {
             CK(cudaMemsetAsync(wideC, 0, sizeof(uint32_t) * OSW_DIGITS * chunks, s));
-            k_wide_tile_hist<K><<<tiles, OSW_THREADS, 0, s>>>(kin, n_ptr, n_host, shift, chunk_shift, wideH, wideC, ready_ctl ? nullptr : c, skip_invalid ? 1u : 0u);
+            k_wide_tile_hist<K><<<tiles, OSW_THREADS, 0, s>>>(kin, n_ptr, n_host, shift, chunk_shift, wideH, wideC, c, skip_invalid ? 1u : 0u);
         }
         if (region_stride && few_bins && payload_in && few_bins <= 32 && (payload_bytes == 16 || payload_bytes == 24 || payload_bytes == 32 || payload_bytes == 64)) {
             // a few fixed-capacity regions (destination GPUs): ranks from ballots, records leave in runs
@@ -292,18 +263,12 @@ struct RadixSorter {
                 return 0;
             }
         }
-        if (prefix && ranked && sizeof(K) == 4 && !payload_in && keys_out_ok(kout, vout)) {
-            k_wide_scatter_ranked<0><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, chunk_shift,
-                                                                   h16_rows ? h16_rows : wideH, wideC, wideT, nullptr, nullptr);
-            CK(cudaGetLastError());
-            launches += 2;
-            *counts = c;
-            return 0;
-        }
-        if (prefix && ranked && sizeof(K) == 4 && payload_in && payload_out && kout && !region_stride) { // the records travel with their slots (bucketed exchange)
+        if (ranked) {
+            if (sizeof(K) != 4 || !kout || (payload_in ? !payload_out || region_stride : !vout)) return WFB_E_UNSUPPORTED;
 #define WFB_WSR(RB_) k_wide_scatter_ranked<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, \
-                                                                             chunk_shift, h16_rows ? h16_rows : wideH, wideC, wideT, payload_in, payload_out)
-            switch (payload_bytes) {
+                                                                             chunk_shift, rows, wideC, wideT, payload_in, payload_out)
+            if (!payload_in) WFB_WSR(0);
+            else switch (payload_bytes) { // the records travel with their slots (bucketed exchange)
                 case 16: WFB_WSR(16); break; case 24: WFB_WSR(24); break; case 32: WFB_WSR(32); break; case 48: WFB_WSR(48); break; case 64: WFB_WSR(64); break;
                 default: return WFB_E_UNSUPPORTED;
             }
@@ -313,7 +278,7 @@ struct RadixSorter {
             *counts = c;
             return 0;
         }
-#define WFB_WS(RB_) launch_wide_scatter<K, RB_>(tiles, kin, kout, vout, n_ptr, n_host, shift, chunk_shift, c, s, payload_in, payload_out, payload_bytes, skip_invalid ? 1u : 0u, region_stride, h32, prefix ? 1u : 0u)
+#define WFB_WS(RB_) launch_wide_scatter<K, RB_>(tiles, kin, kout, vout, n_ptr, n_host, shift, chunk_shift, c, s, payload_in, payload_out, payload_bytes, skip_invalid ? 1u : 0u, region_stride)
         if (!payload_in) WFB_WS(0);
         else switch (payload_bytes) {
             case 8: WFB_WS(8); break;   case 16: WFB_WS(16); break; case 24: WFB_WS(24); break; case 32: WFB_WS(32); break;
@@ -328,23 +293,14 @@ struct RadixSorter {
 
     template <class K>
     int sort(K *kA, K *kB, uint32_t *vA, uint32_t *vB, const uint32_t *n_ptr, uint32_t n_host, uint32_t cap, uint32_t passes,
-             cudaStream_t s, const K **skeys, const uint32_t **svals,
-             const unsigned char *payload_in = nullptr, unsigned char *payload_out = nullptr, uint32_t payload_bytes = 0,
-             uint32_t *ready_ctl = nullptr, uint32_t *seg_first = nullptr, uint32_t seg_first_n = 0, uint32_t base_shift = 0)
+             cudaStream_t s, const K **skeys, const uint32_t **svals, uint32_t *ready_ctl = nullptr, uint32_t *seg_first = nullptr, uint32_t seg_first_n = 0, uint32_t base_shift = 0)
     {
         // ready_ctl != nullptr: histograms already accumulated there by the producer of the keys (after prepare())
         uint32_t *const own_ctl = ctl;
         const bool hist_ready = ready_ctl != nullptr;
         if (hist_ready) ctl = ready_ctl;
         struct Restore { uint32_t *&c; uint32_t *v; ~Restore() { c = v; } } restore{ctl, own_ctl};
-        static int items = 0; // elements per thread of a pass (tuning knob: WFB_OS_ITEMS = 4, 8 or 16)
-        if (items == 0) {
-            const char *e = std::getenv("WFB_OS_ITEMS");
-            items = e ? std::atoi(e) : 8;
-            if (items != 4 && items != 8 && items != 16) items = 8;
-            if (items > OsCfg<K>::MAX_ITEMS) items = OsCfg<K>::MAX_ITEMS;
-        }
-        const uint32_t TE = OS_THREADS * static_cast<uint32_t>(items);
+        const uint32_t TE = OS_THREADS * OS_ITEMS;
         int rc = ensure(cap, OS_THREADS * 4, s, 256); if (rc) return rc;
         passes = std::min<uint32_t>(std::max(1u, passes), OS_MAX_PASSES);
         const uint32_t tiles = std::max(1u, (cap + TE - 1) / TE);
@@ -357,13 +313,8 @@ struct RadixSorter {
         K *kout = kB; uint32_t *vout = vB;
         for (uint32_t p = 0; p < passes; p++) {
             epoch = (epoch + 1) & 0x3fffffffu; if (epoch == 0) epoch = 1;
-            const bool last = (p + 1 == passes);
-            const unsigned char *pin = last ? payload_in : nullptr;
-            unsigned char *pout = last ? payload_out : nullptr;
-            uint32_t *sf = last ? seg_first : nullptr;
-            if (items == 4) launch_pass<K, 4>(tiles, kin, vin, kout, vout, n_ptr, n_host, p, passes, s, pin, pout, payload_bytes, sf, seg_first_n, base_shift);
-            else if (items == 8 || OsCfg<K>::MAX_ITEMS < 16) launch_pass<K, 8>(tiles, kin, vin, kout, vout, n_ptr, n_host, p, passes, s, pin, pout, payload_bytes, sf, seg_first_n, base_shift);
-            else launch_pass<K, (OsCfg<K>::MAX_ITEMS >= 16 ? 16 : 8)>(tiles, kin, vin, kout, vout, n_ptr, n_host, p, passes, s, pin, pout, payload_bytes, sf, seg_first_n, base_shift);
+            uint32_t *sf = (p + 1 == passes) ? seg_first : nullptr;
+            k_onesweep_pass<K><<<tiles, OS_THREADS, 0, s>>>(kin, vin, kout, vout, n_ptr, n_host, p, passes, ctl, state, epoch, sf, seg_first_n, base_shift);
             kin = kout; vin = vout;
             if (kout == kB) { kout = kA; vout = vA; } else { kout = kB; vout = vB; }
         }
@@ -562,10 +513,6 @@ struct SegScratch {
     uint32_t *batch_off = nullptr; uint32_t batch_off_cap = 0;
     DevBatch *d_batches = nullptr; uint32_t batch_cap = 0;
     uint32_t *n_total = nullptr;
-    bool sparse = false;          // this segment was ingested without global compaction (positions = tuple indices)
-    bool h32_ready = false;       // the streaming pass filed the per-tile digit counts of the wide partition (sorter.wideH32)
-    bool h16_ready = false;       // the tile pass filed them per wide tile as 16-bit rows (sorter.wideH), claiming 16 tiles per ticket
-    bool ranked = false;          // ... and packed a rank with every slot (TileArgs::pack_rank)
     uint16_t *h16 = nullptr; uint32_t h16_tiles = 0; // pipelined handles: this segment's own rows (the next segment's tile pass files its rows while
                                                      // this segment's partition still reads these)
     const unsigned char *lifted_src = nullptr; // records of this segment: `lifted`, or the caller's buffer (in-place ingest)
@@ -576,7 +523,7 @@ struct SegScratch {
     // pipelined mode: results of the segment wait here until the next call / flush delivers them
     unsigned char *res = nullptr; uint64_t *res_ts = nullptr; uint32_t *res_n = nullptr; uint32_t res_cap = 0;
     cudaEvent_t ev_ingest = nullptr, ev_done = nullptr;
-    bool pending = false, hist_ready = false;
+    bool pending = false;
     uint32_t nbatches = 0, total = 0;
 
     void destroy()
@@ -620,21 +567,9 @@ struct wfb_ffat {
     GrowCheck growc;                // WFB_KEYS_GROW (ff.grow): the growth check after the key-inserting pass
     uint32_t *mg_scratch = nullptr; // (internal, ffat_process_prebucketed) per-(bucket, sub-bucket, source) counts, their scan, run starts
     bool append_results = false;  // (internal, wfb_mg_flush) the next call's results follow the ones already in the output buffer
-    bool buckets = true;          // one wide radix pass + per-bucket CTAs (<= 65536 keys); WFB_UPDATE=lanes selects the
-                                  // full sort + thread-per-key update instead
+    bool buckets = true;          // one wide radix pass + per-bucket CTAs (<= 65536 keys); else the full sort + thread-per-key update
     uint32_t bucket_shift = 0;    // the wide pass partitions on (slot >> bucket_shift) & 1023
     bool bucket_move = false;     // WFB_BUCKET_MOVE=1: the wide pass also moves the lifted records into their buckets
-    bool l2_hints = true;         // WFB_L2_HINTS=0: no eviction-priority hints on the ingest pass
-    bool fuse_tile_hist = false;  // WFB_FUSE_TILE_HIST=1: the tile pass also files the per-tile digit counts of the wide partition (one more
-                                  // global RED per survivor: measured +17 us on the tile pass against -8 us on the partition, so off)
-    bool stream_update = false;   // WFB_UPDATE=stream: k_ffat_update_stream (lane = key, per-key queues) instead of k_ffat_update_buckets
-    bool rank_scatter = true;     // with tile_h16: the tile pass also packs a rank with every slot and the partition places the pairs by it (k_wide_scatter_ranked); WFB_RANK_SCATTER=0: off
-    bool tile_h16 = true;         // the tile pass claims whole wide tiles and files their digit counts itself (no k_wide_tile_hist); WFB_TILE_H16=0: off
-    bool inplace_kernel = true;   // WFB_INPLACE_KERNEL=0: the in-place case also goes through the tile pass
-    bool inplace_ok = true;       // WFB_INPLACE=0: always copy the records of a pass-through program
-    bool sparse_ingest = true;    // WFB_SPARSE=0: the bucket path also compacts the survivors over the whole segment
-    uint32_t ingest_ctas_per_sm = 0; // 0: as many as fit; pipelined handles leave room for the concurrent sort/update kernels
-    bool move_payload = false;    // tuning knob WFB_SORT_PAYLOAD=1: the last sort pass also moves the lifted records
     // optional per-phase timing (wfb_ffat_timing)
     bool timing = false;
     std::vector<cudaEvent_t> tev; // 4 events per recorded call
@@ -1023,14 +958,9 @@ static int shard_lift_impl(wfb_engine_t *e, const wfb_functors_t *pre, const wfb
     a.sort_ctl = ctl; a.sort_passes = 1; a.sort_shift = 0; a.sort_dbits = OSW_BITS;
     if (bucketed) { a.shard_slots = shard_slots; a.shard_keys = shard_keys; a.shard_err = counts_dev + MAX_SHARDS; a.sort_shift = shift; a.pack_rank = 1; }
     // the tile pass claims whole wide tiles and files the per-tile destination counts itself (no counting pass in the partition)
-    static const bool h16_env = !(std::getenv("WFB_TILE_H16") && std::atoi(std::getenv("WFB_TILE_H16")) == 0);
-    const bool h16 = h16_env || bucketed;
-    uint32_t claims = tiles;
-    if (h16) {
-        rc = e->sorter.ensure_wide(static_cast<uint32_t>(positions), s, &a.wide_h16); if (rc) return rc;
-        a.tiles_per_ticket = OSW_TILE_POS / TILE; a.sort_ctl = nullptr;
-        claims = (tiles + a.tiles_per_ticket - 1) / a.tiles_per_ticket;
-    }
+    rc = e->sorter.ensure_wide(static_cast<uint32_t>(positions), s, &a.wide_h16); if (rc) return rc;
+    a.tiles_per_ticket = OSW_TILE_POS / TILE; a.sort_ctl = nullptr;
+    const uint32_t claims = (tiles + a.tiles_per_ticket - 1) / a.tiles_per_ticket;
     e->ts.next_launch(a);
     uint32_t grid = 0;
     rc = e->ops->tile_pass(MODE_INGEST, a, pre ? static_cast<const void *>(pre) : e->pp(), claims, s, &grid, span_begin, span_end); if (rc) return rc;
@@ -1040,14 +970,13 @@ static int shard_lift_impl(wfb_engine_t *e, const wfb_functors_t *pre, const wfb
     const uint64_t before = e->sorter.launches;
     if (bucketed) {
         rc = e->sorter.sort_wide<uint32_t>(e->sh_dest, out_slots, nullptr, nullptr, static_cast<uint32_t>(positions), static_cast<uint32_t>(positions), shift, s,
-                                           ctl, &counts, e->sh_lifted, static_cast<unsigned char *>(out_regions), static_cast<uint32_t>(RB), true,
-                                           0, 0, false, true, nullptr, true);
+                                           ctl, &counts, e->sh_lifted, static_cast<unsigned char *>(out_regions), static_cast<uint32_t>(RB), true);
         if (rc) return rc;
         k_shard_bin_counts<<<1, 32 * MAX_SHARDS, 0, s>>>(counts, num_shards, shard_slots >> shift, counts_dev, send_meta, watermark);
     } else {
         rc = e->sorter.sort_wide<uint32_t>(e->sh_dest, nullptr, nullptr, nullptr, static_cast<uint32_t>(positions), static_cast<uint32_t>(positions), 0, s,
                                            e->sh_ctl, &counts, e->sh_lifted, static_cast<unsigned char *>(out_regions), static_cast<uint32_t>(RB), true,
-                                           region_capacity, num_shards, false, h16);
+                                           region_capacity, num_shards);
         if (rc) return rc;
         k_shard_counts<<<1, 32, 0, s>>>(counts, num_shards, region_capacity, counts_dev);
     }
@@ -1238,19 +1167,14 @@ static int lifted_program_of(int prog)
     return id;
 }
 
-// what create derives from the key capacity and the tuning knobs: the sort passes over the slots and the bucket / onesweep path
+// what create derives from the key capacity: the sort passes over the slots and the bucket / onesweep path
 static void ffat_derive_paths(wfb_ffat *h)
 {
     uint32_t bits = 0; while ((1ull << bits) < h->ff.max_keys) bits++;
     h->sort_passes = std::max(1u, (bits + 7) / 8);
     h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
     // bucket path: every bucket holds at most BK_KEYS keys and the pane length fits 32 bits
-    const char *e = std::getenv("WFB_UPDATE");
-    h->buckets = !(e && std::strcmp(e, "lanes") == 0) && (1u << h->bucket_shift) <= BK_KEYS && h->ff.pane < (1ull << 32);
-    // streaming update: one path update per completed pane inside the item loop, so panes of a few items at least
-    h->stream_update = h->buckets && !h->bucket_move && e && std::strcmp(e, "stream") == 0; // (measured: 173 us against 153 us for the bucket kernel at the bench configuration)
-    const char *t = std::getenv("WFB_TILE_H16");
-    h->tile_h16 = h->buckets && !(t && std::atoi(t) == 0);
+    h->buckets = (1u << h->bucket_shift) <= BK_KEYS && h->ff.pane < (1ull << 32);
 }
 
 // deferred window groups a segment of seg_cap records can fire: one per slide * Nb records, and one more per key
@@ -1374,9 +1298,9 @@ static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, ui
     rc = wfb_ffat_create(&h->cb, lp, win_p, slide_p, nb, max_keys, 0, 0, flags & WFB_FFAT_DENSE_KEYS);
     if (rc) { wfb_ffat_destroy(h); return rc; }
     // the front end hands the popped panes to the back end in place, with the slot of every record: that needs the bucket path with the
-    // in-place ingest (at most 65536 keys; not with the WFB_SPARSE=0 / WFB_INPLACE=0 / WFB_UPDATE=lanes / WFB_BUCKET_MOVE=1 knobs). Refuse here,
-    // before any pane has been consumed, rather than at the first firing batch
-    if (!h->cb->buckets || !h->cb->sparse_ingest || !h->cb->inplace_ok || h->cb->bucket_move) { wfb_ffat_destroy(h); return WFB_E_UNSUPPORTED; }
+    // in-place ingest (at most 65536 keys; not with WFB_BUCKET_MOVE=1). Refuse here, before any pane has been consumed, rather than at the
+    // first firing batch
+    if (!h->cb->buckets || h->cb->bucket_move) { wfb_ffat_destroy(h); return WFB_E_UNSUPPORTED; }
     // the back end never looks keys up (the front end hands it the slot of every record): it only needs slot -> key for the results
     if (!ff.dense) { cudaFree(h->cb->ff.slot_key); h->cb->ff.slot_key = ff.slot_key; h->cb->ff.n_slots = ff.n_slots; h->cb->shares_slot_key = true; }
     h->state_bytes = total + h->cb->state_bytes;
@@ -1512,7 +1436,6 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
     wfb_ffat *h = new (std::nothrow) wfb_ffat();
     if (!h) return WFB_E_BADARG;
     h->prog = prog; h->ops = o; h->win_type = win_type;
-    { const char *e = std::getenv("WFB_SORT_PAYLOAD"); h->move_payload = e && std::atoi(e) != 0; }
     rc = h->ts.init(); if (rc) { delete h; return rc; }
     FfatDev &ff = h->ff;
     ff.win = win; ff.slide = slide; ff.nb = wins_per_batch;
@@ -1523,9 +1446,8 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
     ff.pane = static_cast<uint32_t>(pane); ff.wp = static_cast<uint32_t>(win / pane); ff.sp = static_cast<uint32_t>(slide / pane);
     // ring of n leaves (a power of two) for the bp panes a group reads + spare leaves: a key that completes up to `spare` further panes in
     // the call that fires a group leaves the group's leaves alone, so the group can wait for the deferred pass (one warp per group, levels
-    // built on chip) instead of being evaluated inside the update kernel. WFB_RING_SPARE: minimum spare leaves (default min(bp, 32)).
-    static const int spare_env = std::getenv("WFB_RING_SPARE") ? std::atoi(std::getenv("WFB_RING_SPARE")) : -1;
-    const uint64_t spare_min = spare_env >= 0 ? static_cast<uint64_t>(spare_env) : std::min<uint64_t>(bp, 32);
+    // built on chip) instead of being evaluated inside the update kernel. At least min(bp, 32) spare leaves.
+    const uint64_t spare_min = std::min<uint64_t>(bp, 32);
     uint32_t n = 1, lg = 0; while (n < bp + spare_min) { n <<= 1; lg++; }
     ff.n_leaves = n; ff.log_leaves = lg;
     ff.defer_items = (static_cast<uint64_t>(n) - bp + 1) * pane;
@@ -1557,7 +1479,7 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
     ALLOC(ff.seg_off, sizeof(uint32_t) * (static_cast<size_t>(max_keys) + 1));
     CK(cudaMemset(ff.seg_off, 0xff, sizeof(uint32_t) * (static_cast<size_t>(max_keys) + 1)));
     ALLOC(ff.heavy, sizeof(uint32_t) * max_keys);
-    { const char *e = std::getenv("WFB_LIGHT_MAX"); ff.light_max = e ? static_cast<uint32_t>(std::atoi(e)) : 256u; }
+    ff.light_max = 256;
     h->pipelined = (flags & WFB_FFAT_PIPELINED) != 0;
     for (int p = 0; p < (h->pipelined ? 2 : 1); p++) {
         SegScratch &g = h->seg[p];
@@ -1570,41 +1492,18 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
         CK(cudaEventCreateWithFlags(&g.ev_ingest, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&g.ev_done, cudaEventDisableTiming));
     }
-    if (h->pipelined) {
-        CK(cudaStreamCreateWithFlags(&h->s2, cudaStreamNonBlocking));
-        const char *e = std::getenv("WFB_INGEST_CTAS_PER_SM");
-        h->ingest_ctas_per_sm = e ? static_cast<uint32_t>(std::atoi(e)) : 2u;
-    }
+    if (h->pipelined) CK(cudaStreamCreateWithFlags(&h->s2, cudaStreamNonBlocking));
 #undef ALLOC
     if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_ffat_destroy(h); return rc; } }
     { const char *e = std::getenv("WFB_BUCKET_MOVE"); h->bucket_move = e && std::atoi(e) != 0; }
-    { const char *e = std::getenv("WFB_L2_HINTS"); h->l2_hints = !(e && std::atoi(e) == 0); }
-    { const char *e = std::getenv("WFB_SPARSE"); h->sparse_ingest = !(e && std::atoi(e) == 0); }
-    { const char *e = std::getenv("WFB_INPLACE"); h->inplace_ok = !(e && std::atoi(e) == 0); }
-    { const char *e = std::getenv("WFB_INPLACE_KERNEL"); h->inplace_kernel = !(e && std::atoi(e) == 0); }
-    { const char *e = std::getenv("WFB_FUSE_TILE_HIST"); h->fuse_tile_hist = e && std::atoi(e) != 0; }
-    { // WFB_L2_PERSIST=<MB>: L2 set-aside for evict-last lines (the lifted records between the ingest pass and the update)
-        const char *e = std::getenv("WFB_L2_PERSIST");
-        if (e && std::atoi(e) > 0) {
-            int dev = 0, maxp = 0;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, dev);
-            const size_t want = std::min<size_t>(static_cast<size_t>(std::atoi(e)) << 20, static_cast<size_t>(maxp));
-            cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want);
-            if (std::getenv("WFB_VERBOSE")) std::fprintf(stderr, "[wfb] persisting L2: max %d MB, set %zu MB\n", maxp >> 20, want >> 20);
-        }
-    }
     ffat_derive_paths(h);
     { // lazy FlatFAT levels (FfatDev::lazy): bucket path, the on-chip tree of one group must fit 32 KB, and building the n - 1 internal
       // nodes once per fired group must be cheaper than a root path (log n nodes) per completed pane: a group fires every sp * Nb panes.
-      // (Nb = 1 with slide = pane fires on every pane: eager levels there. WFB_LAZY_TREE=0 / 1 forces either.) A growing handle keeps
-      // the layout it was created with when it leaves the bucket path: the update kernels of both paths read and write either one.
-        const char *lz = std::getenv("WFB_LAZY_TREE");
+      // (Nb = 1 with slide = pane fires on every pane: eager levels there.) A growing handle keeps the layout it was created with when
+      // it leaves the bucket path: the update kernels of both paths read and write either one.
         const bool fits = h->buckets && static_cast<size_t>(2) * ff.n_leaves * RB <= (32u << 10);
         const bool pays = static_cast<uint64_t>(ff.n_leaves) <= 2ull * std::max(1u, ff.log_leaves) * ff.sp * ff.nb;
-        ff.lazy = (fits && (lz ? std::atoi(lz) != 0 : pays)) ? 1u : 0u;
-        const char *rs = std::getenv("WFB_RANK_SCATTER");
-        h->rank_scatter = !(rs && std::atoi(rs) == 0);
+        ff.lazy = (fits && pays) ? 1u : 0u;
     }
     h->state_bytes = total;
     *hh = h;
@@ -1656,8 +1555,6 @@ int wfb_ffat_set_key_shard(wfb_ffat_t *h, uint32_t num_shards, uint32_t shard)
 }
 
 static double host_now_us() { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e6 + t.tv_nsec * 1e-3; }
-static double g_sec[8]; static double g_sec_t = 0; static bool g_sec_on = false;
-#define SEC(i) do { if (g_sec_on) { const double n_ = host_now_us(); g_sec[i] += n_ - g_sec_t; g_sec_t = n_; } } while (0)
 static int ffat_ensure_segment(wfb_ffat *h, SegScratch &g, uint32_t total, uint32_t nbatches, cudaStream_t s)
 {
     if (total > g.cap) {
@@ -1668,7 +1565,7 @@ static int ffat_ensure_segment(wfb_ffat *h, SegScratch &g, uint32_t total, uint3
         g.cap = std::max(total, 2 * g.cap);
         const size_t RB = h->ops->result_bytes;
         CK(cudaMalloc(&g.lifted, static_cast<size_t>(g.cap) * RB));
-        if (h->move_payload || h->bucket_move) CK(cudaMalloc(&g.lifted_sorted, static_cast<size_t>(g.cap) * RB));
+        if (h->bucket_move) CK(cudaMalloc(&g.lifted_sorted, static_cast<size_t>(g.cap) * RB));
         CK(cudaMalloc(&g.slotsA, sizeof(uint32_t) * g.cap)); CK(cudaMalloc(&g.slotsB, sizeof(uint32_t) * g.cap));
         CK(cudaMalloc(&g.posA, sizeof(uint32_t) * g.cap)); CK(cudaMalloc(&g.posB, sizeof(uint32_t) * g.cap));
         g.trig_cap = ffat_trig_cap(h, g.cap, h->ff.max_keys);
@@ -1701,38 +1598,31 @@ static int ffat_window_phase(wfb_ffat *h, SegScratch &g, const FfatDev &ff, unsi
     if (h->buckets) {
         // ONE wide radix pass on the top 10 slot bits: 1024 buckets of consecutive keys, arrival order inside a bucket ...
         const uint32_t *counts = nullptr;
-        rc = h->sorter.sort_wide<uint32_t>(g.slotsA, g.slotsB, g.posB, g.sparse ? nullptr : g.n_total, g.total, g.total, h->bucket_shift, s,
-                                           g.hist_ready ? g.sort_ctl : nullptr, &counts, h->bucket_move ? g.lifted : nullptr,
-                                           h->bucket_move ? g.lifted_sorted : nullptr, static_cast<uint32_t>(h->ops->result_bytes), g.sparse, 0, 0, g.h32_ready, g.h16_ready, h->pipelined ? g.h16 : nullptr, g.ranked);
+        rc = h->sorter.sort_wide<uint32_t>(g.slotsA, g.slotsB, g.posB, nullptr, g.total, g.total, h->bucket_shift, s, g.sort_ctl, &counts,
+                                           h->bucket_move ? g.lifted : nullptr, h->bucket_move ? g.lifted_sorted : nullptr,
+                                           static_cast<uint32_t>(h->ops->result_bytes), true, 0, 0, h->pipelined ? g.h16 : nullptr);
         if (rc) return rc;
         h->launches += h->sorter.launches - before;
         h->mark(2, s);
-        SEC(3);
         // ... then one CTA per bucket finishes the job (local split by key, per-key ordered fold, FlatFAT update)
-        if (h->stream_update && h->ops->ffat_stream)
-            rc = h->ops->ffat_stream(ff, g.lifted_src, g.slotsB, g.posB, counts, h->bucket_shift, g.batch_off, g.d_batches, g.nbatches, out, out_ts, out_cap, n_out, s, h->pp());
-        else
-            rc = h->ops->ffat_buckets(ff, h->bucket_move ? g.lifted_sorted : g.lifted_src, g.slotsB, g.posB, counts, h->bucket_shift, h->bucket_move ? 1u : 0u, g.batch_off, g.d_batches, g.nbatches, out, out_ts,
-                                      out_cap, n_out, s, h->pp());
+        rc = h->ops->ffat_buckets(ff, h->bucket_move ? g.lifted_sorted : g.lifted_src, g.slotsB, g.posB, counts, h->bucket_shift, h->bucket_move ? 1u : 0u, g.batch_off, g.d_batches, g.nbatches, out, out_ts,
+                                  out_cap, n_out, s, h->pp());
         if (rc) return rc;
         h->launches += 1;
     } else {
         // stable sort of (slot, arrival position) by slot: onesweep radix, 8 bits per pass
         rc = h->sorter.sort<uint32_t>(g.slotsA, g.slotsB, g.posA, g.posB, g.n_total, 0, g.total, h->sort_passes, s, &sorted_slots,
-                                      &sorted_pos, h->move_payload ? g.lifted : nullptr, h->move_payload ? g.lifted_sorted : nullptr,
-                                      h->ops->result_bytes, g.hist_ready ? g.sort_ctl : nullptr, ff.seg_off, ff.max_keys);
+                                      &sorted_pos, g.sort_ctl, ff.seg_off, ff.max_keys);
         if (rc) return rc;
         h->launches += h->sorter.launches - before;
         h->mark(2, s);
         // one thread per key (one warp per heavy key): pane fold, FlatFAT update
         uint32_t ugrid = std::max(1u, std::min((ff.max_keys + 7) / 8, static_cast<uint32_t>(g_num_sms) * 8u));
-        rc = h->ops->ffat_update(ff, h->move_payload ? g.lifted_sorted : g.lifted, sorted_pos, g.batch_off, g.d_batches, g.nbatches,
-                                 out, out_ts, out_cap, n_out, ugrid, s, h->move_payload ? 0u : 1u, h->pp(),
-                                 h->ff.light_max ? std::max(1u, std::min((ff.max_keys + 127u) / 128u, static_cast<uint32_t>(g_num_sms) * 16u)) : 0u);
+        rc = h->ops->ffat_update(ff, g.lifted, sorted_pos, g.batch_off, g.d_batches, g.nbatches, out, out_ts, out_cap, n_out, ugrid, s, h->pp(),
+                                 std::max(1u, std::min((ff.max_keys + 127u) / 128u, static_cast<uint32_t>(g_num_sms) * 16u)));
         if (rc) return rc;
-        h->launches += h->ff.light_max ? 2 : 1;
+        h->launches += 2;
     }
-    SEC(4);
     // deferred window groups: one thread per window
     rc = h->ops->ffat_windows(ff, g.batch_off, g.d_batches, g.nbatches, out, out_ts, out_cap, static_cast<uint32_t>(g_num_sms) * 4u, s, h->pp(), n_out);
     if (rc) return rc;
@@ -1761,30 +1651,9 @@ int wfb_ffat_process_cb(wfb_ffat_t *h, const wfb_functors_t *pre, const wfb_batc
 
 // ext_slots != nullptr: the key slot of the record at every position is given (one batch, read in place; used by the
 // time-based front end, whose programs' lifted variants have no key extractor)
-static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch_t *batches_h, uint32_t nbatches,
-                                 void *out_results, uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, void *stream,
-                                 const uint32_t *ext_slots);
 static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_t *batches_h, uint32_t nbatches,
                                 void *out_results, uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, void *stream,
                                 const uint32_t *ext_slots)
-{
-    static const bool prof = std::getenv("WFB_HOST_PROFILE") != nullptr; // host time spent issuing a call (tuning aid)
-    if (!prof) return ffat_process_cb_impl2(h, pre, batches_h, nbatches, out_results, out_ts, out_capacity, n_out_dev, stream, ext_slots);
-    static double acc = 0; static uint64_t calls = 0;
-    const double t0 = host_now_us();
-    g_sec_on = true; g_sec_t = t0;
-    const int rc = ffat_process_cb_impl2(h, pre, batches_h, nbatches, out_results, out_ts, out_capacity, n_out_dev, stream, ext_slots);
-    acc += host_now_us() - t0;
-    if (++calls % 64 == 0) {
-        std::fprintf(stderr, "[wfb] process_cb host issue: %.1f us/call over the last 64 calls; sections:", acc / 64); acc = 0;
-        for (int i = 0; i < 8; i++) { std::fprintf(stderr, " %.1f", g_sec[i] / 64); g_sec[i] = 0; }
-        std::fprintf(stderr, "\n");
-    }
-    return rc;
-}
-static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch_t *batches_h, uint32_t nbatches,
-                                 void *out_results, uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, void *stream,
-                                 const uint32_t *ext_slots)
 {
     if (!h || !n_out_dev || (nbatches && !batches_h) || (out_capacity && !out_results)) return WFB_E_BADARG;
     if (h->win_type != 0) return WFB_E_BADARG; // time-based handles: wfb_ffat_process_tb
@@ -1817,18 +1686,17 @@ static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch
         return 0;
     }
     nbatches = static_cast<uint32_t>(hb.size());
-    SEC(0);
     FfatDev ff; // this call's view of the state: per-segment buffers of parity `par`
     // the pass that inserts the call's keys into the key table; a growing handle runs it again after the table grew
     const auto ingest = [&]() -> int {
         // bucket path: no global compaction in the streaming pass -- tile t owns positions [t*TILE, +TILE) of the segment
-        const bool sparse = h->buckets && h->sparse_ingest;
+        const bool sparse = h->buckets;
         const uint64_t seg_cap = sparse ? static_cast<uint64_t>(tiles) * TILE : total;
         if (seg_cap > 0x7fffffffull) return WFB_E_BADARG;
         rc = ffat_ensure_segment(h, g, static_cast<uint32_t>(seg_cap), nbatches, s); if (rc) return rc;
         rc = h->ts.ensure_tiles(tiles); if (rc) return rc;
         { int rc_ = h->ts.stage.h2d(g.d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
-        g.nbatches = nbatches; g.total = static_cast<uint32_t>(seg_cap); g.sparse = sparse;
+        g.nbatches = nbatches; g.total = static_cast<uint32_t>(seg_cap);
         if (sparse) { // first position of every batch (the compacting pass writes the compact offsets itself)
             std::vector<uint32_t> boff(nbatches + 1);
             for (uint32_t i = 0; i < nbatches; i++) boff[i] = hb[i].tile_begin * TILE;
@@ -1836,23 +1704,20 @@ static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch
             { int rc_ = h->ts.stage.h2d(g.batch_off, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
         }
 
-        SEC(1);
         ff = h->ff;
         ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = g.trig_cap; ff.n_heavy = g.n_heavy;
 
+        // the streaming pass also counts the digits of the slot sort that follows
         const uint32_t npasses = h->buckets ? 1u : h->sort_passes;
-        const uint32_t pshift = h->buckets ? h->bucket_shift : 0u;
-        const bool fuse_hist = npasses <= 4; // the streaming pass also counts the digits of the slot sort that follows
-        if (fuse_hist) { rc = h->buckets ? RadixSorter::prepare_wide(g.sort_ctl, s) : RadixSorter::prepare(g.sort_ctl, npasses, s); if (rc) return rc; }
+        rc = h->buckets ? RadixSorter::prepare_wide(g.sort_ctl, s) : RadixSorter::prepare(g.sort_ctl, npasses, s); if (rc) return rc;
         h->mark(0, s);
         // 1. streaming pass: [map -> filter ->] lift, key -> slot, stable compaction over the whole segment
         TileArgs a; std::memset(&a, 0, sizeof(a));
-        if (fuse_hist) { a.sort_ctl = g.sort_ctl; a.sort_passes = npasses; a.sort_shift = pshift; a.sort_dbits = h->buckets ? OSW_BITS : 8u; }
-        g.hist_ready = fuse_hist;
+        a.sort_ctl = g.sort_ctl; a.sort_passes = npasses; a.sort_shift = h->buckets ? h->bucket_shift : 0u; a.sort_dbits = h->buckets ? OSW_BITS : 8u;
         a.batches = g.d_batches; a.nbatches = nbatches; a.num_tiles = tiles;
         a.lifted = g.lifted; a.slots = g.slotsA; a.batch_off = g.batch_off; a.n_total = g.n_total; a.ff = ff;
         g.lifted_src = g.lifted;
-        if (sparse && !h->pipelined && !h->bucket_move && (h->ops->reserved & 1u) && h->inplace_ok) {
+        if (sparse && !h->pipelined && !h->bucket_move && (h->ops->reserved & 1u)) {
             // pass-through program and every batch at its tile position inside one buffer: read the records where they are
             const unsigned char *base = hb[0].tuples;
             bool ok = (reinterpret_cast<uintptr_t>(base) & 15u) == 0;
@@ -1861,58 +1726,42 @@ static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch
         }
         if (ext_slots != nullptr && !a.inplace) return WFB_E_UNSUPPORTED; // (the front end always meets the in-place conditions)
         h->ts.next_launch(a);
-        a.max_ctas_per_sm = h->ingest_ctas_per_sm;
-        a.l2_hints = h->l2_hints ? 1u : 0u;
+        a.max_ctas_per_sm = h->pipelined ? 2u : 0u; // (pipelined: leave room for the concurrent sort / update kernels)
+        a.l2_hints = 1;
         a.sparse = sparse ? 1u : 0u;
         a.count_keys = h->buckets ? 0u : 1u;
-        g.h32_ready = false;
-        if (sparse && fuse_hist && h->fuse_tile_hist && !h->pipelined) { // (pipelined: the rows would be shared by two segments in flight)
-            // the tile pass also files its digit counts per tile of the wide partition
-            rc = h->sorter.prepare_h32(g.total, s, &a.wide_h32); if (rc) return rc;
-            g.h32_ready = true;
-        }
-        g.h16_ready = false; g.ranked = false;
-        if (a.inplace && a.sort_passes <= 1 && h->ops->slots_inplace && h->inplace_kernel) {
-            // records read in place: only the slots (and the digit counts) are produced -- no tiles to stage, a plain kernel does it
-            if (sparse && fuse_hist && h->tile_h16 && !h->pipelined && !g.h32_ready) { // whole wide tiles per CTA: rows + ranks for the partition, as the tile pass does
-                rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc;
-                a.sort_ctl = nullptr;
-                g.h16_ready = true;
-                a.pack_rank = (h->rank_scatter && ff.max_keys <= 65536u) ? 1u : 0u;
-                g.ranked = a.pack_rank != 0;
+        uint32_t claims = tiles;
+        if (sparse) {
+            // a CTA claims the 16 tiles of a wide tile at once, counts its digits in shared memory and files the row itself, and packs a
+            // rank with every slot (bucket-path slots fit 16 bits): the partition that follows needs neither a counting pass nor the
+            // per-CTA global digit counts
+            if (h->pipelined && (g.total + OSW_TILE - 1) / OSW_TILE > h->sorter.wide_tiles) CK(cudaStreamSynchronize(h->s2)); // (the rows are about to be re-allocated)
+            rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc; // (also sizes the chunk rows the partition needs)
+            if (h->pipelined) {
+                const uint32_t wt = (g.total + OSW_TILE - 1) / OSW_TILE;
+                if (wt > g.h16_tiles) {
+                    CK(cudaStreamSynchronize(s)); CK(cudaStreamSynchronize(h->s2));
+                    cudaFree(g.h16);
+                    g.h16_tiles = std::max(wt, 2 * g.h16_tiles);
+                    CK(cudaMalloc(&g.h16, sizeof(uint16_t) * OSW_DIGITS * g.h16_tiles));
+                }
+                a.wide_h16 = g.h16;
             }
+            a.tiles_per_ticket = OSW_TILE_POS / TILE;
+            a.sort_ctl = nullptr; // (the partition accumulates the global counts into g.sort_ctl, cleared above)
+            a.pack_rank = 1;
+            claims = (tiles + a.tiles_per_ticket - 1) / a.tiles_per_ticket;
+        }
+        if (a.inplace && h->ops->slots_inplace) {
+            // records read in place: only the slots and the rows are produced -- no tiles to stage, a plain kernel does it
             rc = h->ops->slots_inplace(a, pre ? static_cast<const void *>(pre) : h->pp(), s); if (rc) return rc;
         } else {
-            uint32_t claims = tiles;
-            if (sparse && fuse_hist && h->tile_h16 && !g.h32_ready) {
-                // a CTA claims the 16 tiles of a wide tile at once, counts its digits in shared memory and files the row itself:
-                // the partition that follows needs neither a counting pass nor the per-CTA global digit counts
-                if (h->pipelined && (g.total + OSW_TILE - 1) / OSW_TILE > h->sorter.wide_tiles) CK(cudaStreamSynchronize(h->s2)); // (the rows are about to be re-allocated)
-                rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc; // (also sizes the chunk rows the partition needs)
-                if (h->pipelined) {
-                    const uint32_t wt = (g.total + OSW_TILE - 1) / OSW_TILE;
-                    if (wt > g.h16_tiles) {
-                        CK(cudaStreamSynchronize(s)); CK(cudaStreamSynchronize(h->s2));
-                        cudaFree(g.h16);
-                        g.h16_tiles = std::max(wt, 2 * g.h16_tiles);
-                        CK(cudaMalloc(&g.h16, sizeof(uint16_t) * OSW_DIGITS * g.h16_tiles));
-                    }
-                    a.wide_h16 = g.h16;
-                }
-                a.tiles_per_ticket = OSW_TILE_POS / TILE;
-                a.sort_ctl = nullptr; // (the chunk-sum kernel accumulates the global counts into g.sort_ctl, cleared above)
-                claims = (tiles + a.tiles_per_ticket - 1) / a.tiles_per_ticket;
-                g.h16_ready = true;
-                a.pack_rank = (h->rank_scatter && ff.max_keys <= 65536u) ? 1u : 0u;
-                g.ranked = a.pack_rank != 0;
-            }
             uint32_t grid = 0;
             rc = h->ops->tile_pass(MODE_INGEST, a, pre ? static_cast<const void *>(pre) : h->pp(), claims, s, &grid, span_begin, span_end); if (rc) return rc;
             h->ts.launched(claims, grid);
         }
         h->launches++;
         h->mark(1, s);
-        SEC(2);
         return 0;
     };
     rc = ingest(); if (rc) return rc;
@@ -1925,7 +1774,6 @@ static int ffat_process_cb_impl2(wfb_ffat_t *h, const void *pre, const wfb_batch
         if (!h->append_results) CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t), s));
         rc = ffat_window_phase(h, g, ff, out, out_ts, out_capacity, n_out_dev, s); if (rc) return rc;
         h->mark(3, s);
-        SEC(5);
     } else {
         // the ingest pass of this segment is queued: now hand over the previous segment's results, then start this
         // segment's sort + update on the internal stream, where it overlaps the NEXT call's ingest pass
@@ -1966,7 +1814,7 @@ static int ffat_process_prebucketed(wfb_ffat *h, const unsigned char *records, c
     }
     { int rc_ = h->ts.stage.h2d(g.d_batches, hb.data(), sizeof(DevBatch) * nsrc, s); if (rc_) return rc_; }
     { int rc_ = h->ts.stage.h2d(g.batch_off, offs_h, sizeof(uint32_t) * (nsrc + 1), s); if (rc_) return rc_; }
-    g.nbatches = nsrc; g.total = total; g.sparse = true; g.lifted_src = records;
+    g.nbatches = nsrc; g.total = total; g.lifted_src = records;
     FfatDev ff = h->ff;
     ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = g.trig_cap; ff.n_heavy = g.n_heavy;
     rc = RadixSorter::prepare_wide(g.sort_ctl, s); if (rc) return rc; // (buckets at or above bps stay empty)
