@@ -136,8 +136,10 @@ int wfb_map_filter_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_b
 /* ---- Map_GPU / Filter_GPU, keyed-stateful ------------------------------------------------------------------------
  * func(tuple, state_of_key) applied in per-key arrival order; a key's state (the program's state_t, zero-initialised) lives
  * in the handle, which the replicas of one operator share (they see disjoint keys). K queued batches per call; arrival
- * order = batch order, then index order. replaces Stateful_MAPGPU_Kernel / Stateful_FILTERGPU_Kernel + the TBB key map,
- * spinlock and per-key state allocation, wf/map_gpu.hpp:80-102, :212-299, wf/filter_gpu.hpp:91-117, :247-355. */
+ * order = batch order, then index order. max_keys up to 2^30 (WFB_E_UNSUPPORTED above): up to 65536 keys the items are
+ * split into buckets of at most 64 keys, above that they are sorted by key slot; the results are the same. replaces
+ * Stateful_MAPGPU_Kernel / Stateful_FILTERGPU_Kernel + the TBB key map, spinlock and per-key state allocation,
+ * wf/map_gpu.hpp:80-102, :212-299, wf/filter_gpu.hpp:91-117, :247-355. */
 typedef struct wfb_kstate wfb_kstate_t;
 int wfb_kstate_create(wfb_kstate_t **h, int prog, uint32_t max_keys, uint32_t flags /* WFB_FFAT_DENSE_KEYS or WFB_KEYS_GROW */);
 int wfb_kstate_destroy(wfb_kstate_t *h);
@@ -208,8 +210,8 @@ int wfb_shard_lift(wfb_engine_t *e, const wfb_functors_t *pre, const wfb_batch_t
  *                          are kept, so every key's state survives. The only cost on calls that do not grow is one 8-byte device-to-host
  *                          copy the host waits for. A growth that cannot allocate returns WFB_E_CAPACITY and leaves the handle as it was.
  *                          Also accepted by wfb_kstate_create. Not with WFB_FFAT_DENSE_KEYS, WFB_FFAT_PIPELINED or a key shard
- *                          (WFB_E_BADARG). The doubling stops at 65536 keys while the keys fit: time-based and keyed-stateful handles
- *                          grow up to 65536 keys, count-based ones then double again up to 2^30. On a growing handle the integer key
+ *                          (WFB_E_BADARG). The doubling stops once at 65536 keys while the keys fit (the last capacity of the
+ *                          bucket path), then doubles again up to 2^30, for every kind of handle. On a growing handle the integer key
  *                          2^64-1 (the free-entry marker) is refused with error bit 0, as the all-ones 16-byte key is. */
 #define WFB_KEYS_GROW 4u
 int wfb_ffat_create(wfb_ffat_t **h, int prog, uint64_t win, uint64_t slide, uint32_t wins_per_batch,

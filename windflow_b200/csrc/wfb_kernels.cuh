@@ -3014,7 +3014,8 @@ __global__ void k_tb_pop_write(const FfatDev ff, const TbDev tb, uint64_t first_
 // Keyed-stateful Map_GPU / Filter_GPU (wf/map_gpu.hpp:80-102, :212-299; wf/filter_gpu.hpp:91-117, :247-355): the same
 // shape as the window update -- slots of the segment's tuples, ONE wide partition pass into 1024 buckets of consecutive
 // slots, one CTA per bucket splits its items by key (stable) and ONE THREAD per key walks its run in arrival order with
-// the key's state in registers. Stateful filter: keep flags, then a stable per-batch compaction.
+// the key's state in registers (above 65536 keys: a full sort by slot and k_ks_apply_runs). Stateful filter: keep flags,
+// then a stable per-batch compaction.
 // ------------------------------------------------------------------------------------------------------
 template <class P>
 __global__ void k_ks_slots(const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff, uint32_t nb, uint32_t total, const FfatDev ff,
@@ -3152,6 +3153,37 @@ __global__ void __launch_bounds__(KS_THREADS) k_ks_apply(const FfatDev ff, const
         __syncthreads();
     }
     if (has_key && touched) *reinterpret_cast<S *>(states + static_cast<size_t>(key_lo + tid) * sizeof(S)) = st;
+}
+
+// More than 65536 keys: the (slot, arrival position) pairs come fully sorted by slot (stable onesweep passes with 8·passes > log2
+// capacity, so INVALID_SLOT sorts behind every real slot). The thread whose item starts a run -- its slot differs from its
+// predecessor's -- walks that run in arrival order with the key's state in registers: work follows the call's items, not the capacity.
+template <class P, bool FILTER>
+__global__ void __launch_bounds__(256) k_ks_apply_runs(const FfatDev ff, const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff,
+                                                       uint32_t nb, uint32_t n, const uint32_t *__restrict__ sorted_slots,
+                                                       const uint32_t *__restrict__ sorted_pos, unsigned char *__restrict__ states,
+                                                       unsigned char *__restrict__ keep, const typename P::params_t prm)
+{
+    using T = typename P::tuple_t;
+    using S = typename P::state_t;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t slot = sorted_slots[i];
+        if (slot >= ff.max_keys || (i > 0 && sorted_slots[i - 1] == slot)) continue; // (no slot: the item is not applied)
+        S *sp = reinterpret_cast<S *>(states + static_cast<size_t>(slot) * sizeof(S));
+        alignas(8) S st = *sp;
+        uint32_t j = i;
+        do {
+            const uint32_t gi = sorted_pos[j];
+            const uint32_t b = batch_of(boff, nb, gi);
+            unsigned char *tp = const_cast<unsigned char *>(batches[b].tuples) + static_cast<size_t>(gi - boff[b]) * sizeof(T);
+            alignas(16) T t;
+            ld_rec<T>(tp, t);
+            if constexpr (FILTER) keep[gi] = P::filter_stateful(t, st, prm) ? 1 : 0;
+            else P::map_stateful(t, st, prm);
+            st_rec<T>(tp, t);
+        } while (++j < n && sorted_slots[j] == slot);
+        *sp = st;
+    }
 }
 
 // stable per-batch compaction by the keep flags of a stateful filter: tile counts, scan, scatter

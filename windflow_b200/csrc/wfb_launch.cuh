@@ -100,6 +100,10 @@ struct ProgramOps {
     int (*ks_apply)(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, const uint32_t *bk_slots,
                     const uint32_t *bk_pos, const uint32_t *digit_counts, uint32_t shift, unsigned char *states, unsigned char *keep, cudaStream_t s,
                     const void *params);
+    // (more than 65536 keys) the same over the n (slot, position) pairs sorted by slot
+    int (*ks_apply_runs)(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n,
+                         const uint32_t *sorted_slots, const uint32_t *sorted_pos, unsigned char *states, unsigned char *keep, cudaStream_t s,
+                         const void *params);
     int (*flag_scatter)(const unsigned char *keep, const uint32_t *tile_base, const uint32_t *boff, uint32_t nb, uint32_t n,
                         const uint32_t *rank_start, const DevBatch *batches, cudaStream_t s);
     // Reduce_GPU over K queued batches
@@ -260,6 +264,18 @@ int ks_apply_dispatch(int filter, const FfatDev &ff, const DevBatch *batches, co
     } else return WFB_E_UNSUPPORTED;
 }
 template <class P>
+int ks_apply_runs_dispatch(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n,
+                           const uint32_t *sorted_slots, const uint32_t *sorted_pos, unsigned char *states, unsigned char *keep, cudaStream_t s,
+                           const void *params)
+{
+    if constexpr (program_has_state<P>::value) {
+        if (filter) k_ks_apply_runs<P, true><<<grid_for(n, 256), 256, 0, s>>>(ff, batches, boff, nb, n, sorted_slots, sorted_pos, states, keep, load_params<P>(params));
+        else k_ks_apply_runs<P, false><<<grid_for(n, 256), 256, 0, s>>>(ff, batches, boff, nb, n, sorted_slots, sorted_pos, states, keep, load_params<P>(params));
+        WFB_CK(cudaGetLastError());
+        return 0;
+    } else return WFB_E_UNSUPPORTED;
+}
+template <class P>
 int flag_scatter_dispatch(const unsigned char *keep, const uint32_t *tile_base, const uint32_t *boff, uint32_t nb, uint32_t n,
                           const uint32_t *rank_start, const DevBatch *batches, cudaStream_t s)
 {
@@ -414,7 +430,7 @@ ProgramOps make_ops()
     o.gather = &gather_dispatch<P>;
     o.slots_inplace = &slots_inplace_dispatch<P>;
     o.state_bytes = program_state_bytes<P>(); o.reserved2 = 0;
-    o.ks_slots = &ks_slots_dispatch<P>; o.ks_apply = &ks_apply_dispatch<P>; o.flag_scatter = &flag_scatter_dispatch<P>;
+    o.ks_slots = &ks_slots_dispatch<P>; o.ks_apply = &ks_apply_dispatch<P>; o.ks_apply_runs = &ks_apply_runs_dispatch<P>; o.flag_scatter = &flag_scatter_dispatch<P>;
     o.tb_lift = &tb_lift_dispatch<P>; o.tb_reduce = &tb_reduce_dispatch<P>; o.tb_merge = &tb_merge_dispatch<P>; o.tb_pop_write = &tb_pop_write_dispatch<P>;
     o.extract_keys_batches = &extract_keys_batches_dispatch<P>;
     o.reduce_segments_batches = &reduce_segments_batches_dispatch<P>;

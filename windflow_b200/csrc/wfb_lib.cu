@@ -996,16 +996,27 @@ struct wfb_kstate {
     FfatDev ff{};                 // key table only (dense or open addressing)
     unsigned char *states = nullptr;
     RadixSorter sorter;
-    uint32_t bucket_shift = 0;
+    bool buckets = true;          // at most 65536 keys: buckets of at most 64 keys (k_ks_apply); else a full sort (k_ks_apply_runs)
+    uint32_t bucket_shift = 0, sort_passes = 0;
     DevBatch *d_batches = nullptr; uint32_t *d_boff = nullptr; uint32_t batch_cap = 0;
     uint32_t cap = 0;             // tuples per call
-    uint32_t *slotsA = nullptr, *slotsB = nullptr, *posB = nullptr, *tile_cnt = nullptr, *rank_start = nullptr;
+    uint32_t *slotsA = nullptr, *slotsB = nullptr, *posA = nullptr, *posB = nullptr, *tile_cnt = nullptr, *rank_start = nullptr;
     unsigned char *keep = nullptr;
     uint64_t launches = 0;
     PinnedStage stage;
     GrowCheck growc;              // WFB_KEYS_GROW (ff.grow)
 };
 extern "C" {
+
+// what the key capacity decides: up to 65536 keys, 1024 buckets of at most 64 keys; above, a full sort by slot over 8-bit passes with
+// 8·passes > log2(capacity), so that the low bits of INVALID_SLOT sort behind every real slot instead of aliasing one
+static void kstate_derive_paths(wfb_kstate *h, uint32_t cap)
+{
+    uint32_t bits = 0; while ((1ull << bits) < cap) bits++;
+    h->buckets = bits <= OSW_BITS + 6;
+    h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
+    h->sort_passes = bits / 8 + 1;
+}
 
 int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t flags)
 {
@@ -1015,12 +1026,12 @@ int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t f
     if (o->state_bytes == 0) return WFB_E_UNSUPPORTED; // the program has no state_t / stateful functors
     if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
     if ((flags & WFB_KEYS_GROW) && (flags & WFB_FFAT_DENSE_KEYS)) return WFB_E_BADARG;       // (slot = key: nothing to grow)
-    uint32_t bits = 0; while ((1ull << bits) < max_keys) bits++;
-    if (bits > OSW_BITS + 6) return WFB_E_UNSUPPORTED;  // 1024 buckets of at most 64 keys
+    if (max_keys > (1u << 30)) return WFB_E_UNSUPPORTED;  // (the count-based limit)
     int rc = device_ready(); if (rc) return rc;
     wfb_kstate *h = new (std::nothrow) wfb_kstate();
     if (!h) return WFB_E_BADARG;
-    h->prog = prog; h->ops = o; h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
+    h->prog = prog; h->ops = o;
+    kstate_derive_paths(h, max_keys);
     FfatDev &ff = h->ff;
     ff.max_keys = max_keys; ff.dense = (flags & WFB_FFAT_DENSE_KEYS) ? 1u : 0u;
     if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_kstate_destroy(h); return rc; } }
@@ -1046,7 +1057,7 @@ int wfb_kstate_destroy(wfb_kstate_t *h)
     if (!h) return 0;
     cudaDeviceSynchronize();
     cudaFree(h->ff.ht_keys); cudaFree(h->ff.ht_slots); cudaFree(h->ff.n_slots); cudaFree(h->ff.slot_key); cudaFree(h->states);
-    cudaFree(h->d_batches); cudaFree(h->d_boff); cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posB); cudaFree(h->tile_cnt);
+    cudaFree(h->d_batches); cudaFree(h->d_boff); cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posA); cudaFree(h->posB); cudaFree(h->tile_cnt);
     cudaFree(h->rank_start); cudaFree(h->keep);
     h->sorter.destroy(); h->stage.destroy(); h->growc.destroy();
     delete h;
@@ -1090,37 +1101,41 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
     }
     if (n > h->cap) {
         CK(cudaStreamSynchronize(s));
-        cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posB); cudaFree(h->tile_cnt); cudaFree(h->keep);
+        cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posA); cudaFree(h->posB); cudaFree(h->tile_cnt); cudaFree(h->keep);
         h->cap = std::max(n, 2 * h->cap);
         CK(cudaMalloc(&h->slotsA, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->slotsB, sizeof(uint32_t) * h->cap));
-        CK(cudaMalloc(&h->posB, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->keep, h->cap));
+        CK(cudaMalloc(&h->posA, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->posB, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->keep, h->cap));
         CK(cudaMalloc(&h->tile_cnt, sizeof(uint32_t) * ((h->cap + SEGT - 1) / SEGT + 1)));
     }
     { int rc_ = h->stage.h2d(h->d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
     { int rc_ = h->stage.h2d(h->d_boff, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
     // 1. slots; 2. one wide partition pass into 1024 buckets of consecutive slots; 3. per-bucket CTAs, one thread per key
+    // (more than 65536 keys: 2. a stable sort by slot; 3. one thread per run of a slot)
     int rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc;
-    for (bool grew = h->ff.grow != 0; grew; ) { // (a growing handle: the buckets hold 64 keys at most, as at create)
-        rc = grow_keys(h->ff, h->ops->key_bytes, h->growc, 1u << (OSW_BITS + 6), 1u << (OSW_BITS + 6), s, &grew,
+    for (bool grew = h->ff.grow != 0; grew; ) { // (a growing handle stops at 65536 keys, the last capacity of the bucket path, on its way up)
+        rc = grow_keys(h->ff, h->ops->key_bytes, h->growc, 1u << (OSW_BITS + 6), 1u << 30, s, &grew,
                        [h](GrowPlan &plan, uint32_t cap) {
                            const size_t sb = h->ops->state_bytes;
                            plan.add(h->states, sb * h->ff.max_keys, sb * cap, true, 0); // state_t(): zero-initialised
                            return 0;
                        },
-                       [h](uint32_t cap, const GrowPlan &) {
-                           uint32_t bits = 0; while ((1ull << bits) < cap) bits++;
-                           h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
-                           return 0;
-                       });
+                       [h](uint32_t cap, const GrowPlan &) { kstate_derive_paths(h, cap); return 0; });
         if (rc) return rc;
         if (grew) { rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc; h->launches += 2; }
     }
-    const uint32_t *counts = nullptr;
     const uint64_t before = h->sorter.launches;
-    rc = h->sorter.sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, &counts, nullptr, nullptr, 0, true);
-    if (rc) return rc;
-    rc = h->ops->ks_apply(filter ? 1 : 0, h->ff, h->d_batches, h->d_boff, nbatches, h->slotsB, h->posB, counts, h->bucket_shift, h->states,
-                          h->keep, s, f);
+    if (h->buckets) {
+        const uint32_t *counts = nullptr;
+        rc = h->sorter.sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, &counts, nullptr, nullptr, 0, true);
+        if (rc) return rc;
+        rc = h->ops->ks_apply(filter ? 1 : 0, h->ff, h->d_batches, h->d_boff, nbatches, h->slotsB, h->posB, counts, h->bucket_shift, h->states,
+                              h->keep, s, f);
+    } else {
+        const uint32_t *sorted_slots, *sorted_pos;
+        rc = h->sorter.sort<uint32_t>(h->slotsA, h->slotsB, h->posA, h->posB, nullptr, n, n, h->sort_passes, s, &sorted_slots, &sorted_pos);
+        if (rc) return rc;
+        rc = h->ops->ks_apply_runs(filter ? 1 : 0, h->ff, h->d_batches, h->d_boff, nbatches, n, sorted_slots, sorted_pos, h->states, h->keep, s, f);
+    }
     if (rc) return rc;
     h->launches += 2 + (h->sorter.launches - before);
     if (filter) { // stable per-batch compaction by the keep flags
@@ -1213,11 +1228,11 @@ static int ffat_grow(wfb_ffat *h, cudaStream_t s, bool *grew)
                      [h](uint32_t cap, const GrowPlan &plan) { ffat_derive(h, cap); h->state_bytes += plan.grown_bytes(); return 0; });
 }
 
-// growth of a time-based front end: its rings of pending panes and per-key pane bookkeeping, and its count-based back end. At most
-// 65536 keys: the back end takes the popped panes in place, which needs the bucket path (as tb_create requires)
+// growth of a time-based front end: its rings of pending panes and per-key pane bookkeeping, and its count-based back end (which
+// leaves the bucket path above 65536 keys, as a count-based handle does)
 static int tb_grow(wfb_ffat *h, cudaStream_t s, bool *grew)
 {
-    return grow_keys(h->ff, h->ops->key_bytes, h->growc, BK_KEYS << OSW_BITS, BK_KEYS << OSW_BITS, s, grew,
+    return grow_keys(h->ff, h->ops->key_bytes, h->growc, BK_KEYS << OSW_BITS, 1u << 30, s, grew,
         [h](GrowPlan &plan, uint32_t cap) {
             TbDev &tb = h->tb;
             const size_t old = h->ff.max_keys, RB = h->ops->result_bytes;
@@ -1297,10 +1312,10 @@ static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, ui
     if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_ffat_destroy(h); return rc; } } // (the back end grows with it)
     rc = wfb_ffat_create(&h->cb, lp, win_p, slide_p, nb, max_keys, 0, 0, flags & WFB_FFAT_DENSE_KEYS);
     if (rc) { wfb_ffat_destroy(h); return rc; }
-    // the front end hands the popped panes to the back end in place, with the slot of every record: that needs the bucket path with the
-    // in-place ingest (at most 65536 keys; not with WFB_BUCKET_MOVE=1). Refuse here, before any pane has been consumed, rather than at the
-    // first firing batch
-    if (!h->cb->buckets || h->cb->bucket_move) { wfb_ffat_destroy(h); return WFB_E_UNSUPPORTED; }
+    // the front end hands the popped panes to the back end with the slot of every record. On the bucket path (at most 65536 keys) the
+    // back end reads them in place, which WFB_BUCKET_MOVE=1 does not do: refuse that here, before any pane has been consumed, rather than
+    // at the first firing batch. Above 65536 keys the full-sort path's streaming pass takes the slots as they are.
+    if (h->cb->buckets && h->cb->bucket_move) { wfb_ffat_destroy(h); return WFB_E_UNSUPPORTED; }
     // the back end never looks keys up (the front end hands it the slot of every record): it only needs slot -> key for the results
     if (!ff.dense) { cudaFree(h->cb->ff.slot_key); h->cb->ff.slot_key = ff.slot_key; h->cb->ff.n_slots = ff.n_slots; h->cb->shares_slot_key = true; }
     h->state_bytes = total + h->cb->state_bytes;
@@ -1649,8 +1664,8 @@ int wfb_ffat_process_cb(wfb_ffat_t *h, const wfb_functors_t *pre, const wfb_batc
     return ffat_process_cb_impl(h, pre, batches_h, nbatches, out_results, out_ts, out_capacity, n_out_dev, stream, nullptr);
 }
 
-// ext_slots != nullptr: the key slot of the record at every position is given (one batch, read in place; used by the
-// time-based front end, whose programs' lifted variants have no key extractor)
+// ext_slots != nullptr: the key slot of the record at every position is given (one batch, read in place on the bucket path; used by
+// the time-based front end, whose programs' lifted variants have no key extractor)
 static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_t *batches_h, uint32_t nbatches,
                                 void *out_results, uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, void *stream,
                                 const uint32_t *ext_slots)
@@ -1724,7 +1739,13 @@ static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_
             for (uint32_t i = 0; ok && i < nbatches; i++) ok = hb[i].tuples == base + static_cast<size_t>(hb[i].tile_begin) * TILE * h->ops->tuple_bytes;
             if (ok) { a.inplace = 1; g.lifted_src = base; a.ext_slots = ext_slots; }
         }
-        if (ext_slots != nullptr && !a.inplace) return WFB_E_UNSUPPORTED; // (the front end always meets the in-place conditions)
+        if (ext_slots != nullptr && !a.inplace) {
+            // full-sort path: the compacting pass reads the slot of position tile·TILE + thread. The time-based front end hands over one
+            // batch from tile 0 whose records all pass (a lifted program filters nothing): compacted position = popped index = position
+            if (sparse) return WFB_E_UNSUPPORTED; // (the front end always meets the in-place conditions on the bucket path)
+            if (nbatches != 1 || !(h->ops->reserved & 1u)) return WFB_E_BADARG;
+            a.ext_slots = ext_slots;
+        }
         h->ts.next_launch(a);
         a.max_ctas_per_sm = h->pipelined ? 2u : 0u; // (pipelined: leave room for the concurrent sort / update kernels)
         a.l2_hints = 1;
