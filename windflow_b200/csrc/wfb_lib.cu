@@ -1182,11 +1182,13 @@ static int lifted_program_of(int prog)
     return id;
 }
 
-// what create derives from the key capacity: the sort passes over the slots and the bucket / onesweep path
+// what create derives from the key capacity: the sort passes over the slots and the bucket / onesweep path. The full sort takes
+// 8·passes > log2(capacity) bits, so that the low bits of INVALID_SLOT (an item whose key found no slot) sort behind every real slot
+// instead of aliasing the last one (at a capacity of exactly 2^24, three passes would see 0xffffff = slot 2^24 - 1)
 static void ffat_derive_paths(wfb_ffat *h)
 {
     uint32_t bits = 0; while ((1ull << bits) < h->ff.max_keys) bits++;
-    h->sort_passes = std::max(1u, (bits + 7) / 8);
+    h->sort_passes = bits / 8 + 1;
     h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
     // bucket path: every bucket holds at most BK_KEYS keys and the pane length fits 32 bits
     h->buckets = (1u << h->bucket_shift) <= BK_KEYS && h->ff.pane < (1ull << 32);
