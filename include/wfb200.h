@@ -11,6 +11,8 @@
  * Conventions
  *  - all functions return 0 on success, a cudaError_t value (>0) for CUDA failures, or a negative
  *    WFB_E_* code; they never throw and never synchronise the stream unless stated;
+ *  - a call that cannot allocate the scratch memory it grows on demand returns the CUDA error and leaves the handle usable: a later
+ *    call allocates again;
  *  - pointers are DEVICE pointers unless the name ends in _h; `stream` is a cudaStream_t passed as void*;
  *  - a batch is structure-of-arrays: `tuples` (n * tuple_bytes, 16-byte aligned) and `ts` (n * uint64_t);
  *    user functors only ever see `tuple_t &`, so this replaces wf/basic_gpu.hpp:132-140's 72-byte AoS item

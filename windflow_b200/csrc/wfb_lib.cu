@@ -15,6 +15,7 @@
 #include "wfb_kernels.cuh"
 #include "wfb_launch.cuh"
 #include "wfb_programs.cuh"
+#include "wfb_scratch.h"
 
 using namespace wfb;
 
@@ -57,40 +58,39 @@ const ProgramOps *program(int prog)
 // copy is a real asynchronous DMA (a cudaMemcpyAsync from pageable memory is staged by the driver and serialises with the stream) ----
 struct PinnedStage {
     static constexpr int SLOTS = 8;
-    unsigned char *buf[SLOTS] = {}; size_t cap[SLOTS] = {}; cudaEvent_t ev[SLOTS] = {}; bool used[SLOTS] = {}; int next = 0;
+    PinnedScratch<unsigned char> buf[SLOTS]; cudaEvent_t ev[SLOTS] = {}; bool used[SLOTS] = {}; int next = 0;
     int h2d(void *dst, const void *src, size_t bytes, cudaStream_t s)
     {
         if (bytes == 0) return 0;
         const int i = next; next = (next + 1) % SLOTS;
         if (used[i]) CK(cudaEventSynchronize(ev[i])); // the copy that used this slot SLOTS calls ago has long finished
-        if (cap[i] < bytes) { if (buf[i]) cudaFreeHost(buf[i]); cap[i] = std::max<size_t>(bytes, 4096) * 2; CK(cudaMallocHost(reinterpret_cast<void **>(&buf[i]), cap[i])); }
+        CK(buf[i].ensure(bytes, ScratchWaits(), std::max<size_t>(bytes, 4096) * 2));
         if (!ev[i]) CK(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
         std::memcpy(buf[i], src, bytes);
         CK(cudaMemcpyAsync(dst, buf[i], bytes, cudaMemcpyHostToDevice, s));
         CK(cudaEventRecord(ev[i], s)); used[i] = true;
         return 0;
     }
-    void destroy() { for (int i = 0; i < SLOTS; i++) { if (buf[i]) cudaFreeHost(buf[i]); if (ev[i]) cudaEventDestroy(ev[i]); buf[i] = nullptr; ev[i] = nullptr; } }
+    void destroy() { for (int i = 0; i < SLOTS; i++) { if (ev[i]) cudaEventDestroy(ev[i]); ev[i] = nullptr; } }
 };
 
 // ---- scratch shared by the tile passes: ticket counter, epoch-tagged tile states, batch descriptors -----------
 struct TileScratch {
     PinnedStage stage;
-    uint64_t *tile_state = nullptr; uint32_t tile_cap = 0;
-    uint32_t *ticket = nullptr; uint32_t ticket_base = 0; uint32_t epoch = 0;
-    DevBatch *d_batches = nullptr; uint32_t batch_cap = 0;
+    Scratch<uint64_t> tile_state;
+    Scratch<uint32_t> ticket; uint32_t ticket_base = 0; uint32_t epoch = 0;
+    Scratch<DevBatch> d_batches;
     cudaStream_t last_stream = nullptr; bool used = false; cudaEvent_t ev = nullptr;
 
     int init()
     {
-        CK(cudaMalloc(&ticket, sizeof(uint32_t)));
+        CK(ticket.ensure(1));
         CK(cudaMemset(ticket, 0, sizeof(uint32_t)));
         CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
         return 0;
     }
     void destroy()
     {
-        cudaFree(tile_state); cudaFree(ticket); cudaFree(d_batches);
         stage.destroy();
         if (ev) cudaEventDestroy(ev);
     }
@@ -102,25 +102,8 @@ struct TileScratch {
         last_stream = s; used = true;
         return 0;
     }
-    int ensure_tiles(uint32_t num_tiles)
-    {
-        if (num_tiles <= tile_cap) return 0;
-        CK(cudaStreamSynchronize(last_stream));
-        cudaFree(tile_state);
-        tile_cap = std::max(num_tiles, 2 * tile_cap);
-        CK(cudaMalloc(&tile_state, sizeof(uint64_t) * tile_cap));
-        CK(cudaMemset(tile_state, 0, sizeof(uint64_t) * tile_cap)); // epoch 0 is never used by a launch
-        return 0;
-    }
-    int ensure_batches(uint32_t nb)
-    {
-        if (nb <= batch_cap) return 0;
-        CK(cudaStreamSynchronize(last_stream));
-        cudaFree(d_batches);
-        batch_cap = std::max(nb, 2 * batch_cap);
-        CK(cudaMalloc(&d_batches, sizeof(DevBatch) * batch_cap));
-        return 0;
-    }
+    int ensure_tiles(uint32_t num_tiles) { return tile_state.ensure_zeroed(num_tiles, last_stream, last_stream); } // epoch 0 is never used by a launch
+    int ensure_batches(uint32_t nb) { return d_batches.ensure(nb, last_stream); }
     void next_launch(TileArgs &a) { epoch = (epoch + 1) & 0x3fffffffu; if (epoch == 0) epoch = 1; a.epoch = epoch; a.ticket = ticket; a.ticket_base = ticket_base; a.tile_state = tile_state; }
     void launched(uint32_t num_claims, uint32_t grid) { ticket_base += num_claims + grid; } // one failing claim per CTA
 };
@@ -129,26 +112,10 @@ inline uint32_t tiles_of(uint32_t n) { return (n + TILE - 1) / TILE; }
 
 // scratch + launcher of the onesweep radix sort (one per engine / window handle)
 struct RadixSorter {
-    uint32_t *ctl = nullptr;        // [passes][256] histograms + [passes] tickets
-    uint64_t *state = nullptr;      // [tiles][digits] look-back words
-    uint64_t state_words = 0;
+    Scratch<uint32_t> ctl;          // [passes][256] histograms + [passes] tickets
+    Scratch<uint64_t> state;        // [tiles][digits] look-back words
     uint32_t epoch = 0;
     uint64_t launches = 0;
-
-    int ensure(uint32_t cap_elems, uint32_t min_tile, cudaStream_t s, uint32_t digits = 256)
-    {
-        if (!ctl) CK(cudaMalloc(&ctl, sizeof(uint32_t) * CTL_WORDS));
-        const uint32_t tiles = (cap_elems + min_tile - 1) / min_tile;
-        if (static_cast<uint64_t>(tiles) * digits > state_words) {
-            CK(cudaStreamSynchronize(s));
-            cudaFree(state);
-            state_words = static_cast<uint64_t>(tiles) * digits;
-            CK(cudaMalloc(&state, sizeof(uint64_t) * state_words));
-            CK(cudaMemset(state, 0, sizeof(uint64_t) * state_words));
-        }
-        return 0;
-    }
-    void destroy() { cudaFree(ctl); cudaFree(state); cudaFree(wideH); cudaFree(wideC); cudaFree(wideT); cudaFree(wideDone); }
 
     // stable sort of (kA[i], i) by the low 8*passes bits; n on the device (n_ptr) or the host (n_host), cap = upper bound
     // clears the histograms / tickets of the next sort; call it BEFORE a producer that fills the histograms itself
@@ -168,9 +135,9 @@ struct RadixSorter {
     }
     // ONE stable partition pass of (kin[i], i) on the digit (key >> shift) & 1023 into (kout, vout): per-tile counts, then
     // the scatter (no chained scan). *counts = the 1024 digit counts (ready_ctl if the producer of the keys made them).
-    uint16_t *wideH = nullptr; uint32_t *wideC = nullptr; uint32_t wide_tiles = 0, wide_chunks = 0;
-    uint32_t *wideT = nullptr;    // [tiles][1024]: sum of the earlier rows of the tile's chunk (k_wide_tile_bases)
-    uint32_t *wideDone = nullptr; // finished chunks of k_wide_tile_bases (zero between launches)
+    Scratch<uint16_t> wideH; Scratch<uint32_t> wideC;
+    Scratch<uint32_t> wideT;    // [tiles][1024]: sum of the earlier rows of the tile's chunk (k_wide_tile_bases)
+    Scratch<uint32_t> wideDone; // finished chunks of k_wide_tile_bases (zero between launches)
     // tiles of the wide pass over `cap` positions and their chunks. prefix = false: about sqrt(tiles) chunks of >= 16 tiles, every
     // scatter CTA sums the rows of the earlier chunks itself; true (rows filed by the tile pass): chunks of 32 tiles; one kernel
     // (k_wide_tile_bases) computes the first output positions of every chunk and the in-chunk offsets of every tile, so a scatter
@@ -185,29 +152,21 @@ struct RadixSorter {
     }
     // grows the rows and chunk rows of the wide pass; the chunk rows alone when only they are short, so that rows a producer has
     // already filed (ensure_wide, whose chunks of 32 tiles may be fewer than sort_wide's without a prefix) survive
-    int ensure_wide_buffers(uint32_t tiles, uint32_t chunks, cudaStream_t s)
+    int ensure_wide_buffers(uint32_t tiles, uint32_t chunks, ScratchWaits waits)
     {
-        if (tiles <= wide_tiles && chunks <= wide_chunks) return 0;
-        CK(cudaStreamSynchronize(s));
-        if (tiles > wide_tiles) {
-            cudaFree(wideH); cudaFree(wideT);
-            wide_tiles = tiles;
-            CK(cudaMalloc(&wideH, sizeof(uint16_t) * OSW_DIGITS * wide_tiles));
-            CK(cudaMalloc(&wideT, sizeof(uint32_t) * OSW_DIGITS * wide_tiles));
-        }
-        if (chunks > wide_chunks) {
-            cudaFree(wideC);
-            wide_chunks = chunks;
-            CK(cudaMalloc(&wideC, sizeof(uint32_t) * OSW_DIGITS * wide_chunks));
-        }
+        const size_t rows = static_cast<size_t>(OSW_DIGITS) * tiles, chunk_rows = static_cast<size_t>(OSW_DIGITS) * chunks;
+        CK(wideH.ensure(rows, waits, rows));
+        CK(wideT.ensure(rows, waits, rows));
+        CK(wideC.ensure(chunk_rows, waits, chunk_rows));
         return 0;
     }
-    // rows of the wide partition for `cap` positions, allocated before the producer of the keys files them (TileArgs::wide_h16)
-    int ensure_wide(uint32_t cap, cudaStream_t s, uint16_t **rows)
+    // rows of the wide partition for `cap` positions, allocated before the producer of the keys files them (TileArgs::wide_h16);
+    // waits: the streams that may still read the rows (a pipelined handle's sort stream too)
+    int ensure_wide(uint32_t cap, ScratchWaits waits, uint16_t **rows)
     {
         uint32_t tiles, chunk_shift, chunks;
         wide_geometry(cap, true, &tiles, &chunk_shift, &chunks);
-        { int rc = ensure_wide_buffers(tiles, chunks, s); if (rc) return rc; }
+        { int rc = ensure_wide_buffers(tiles, chunks, waits); if (rc) return rc; }
         *rows = wideH;
         return 0;
     }
@@ -229,7 +188,7 @@ struct RadixSorter {
                   const uint16_t *h16_rows = nullptr)
     {
         if (payload_in && (payload_bytes == 0 || (payload_bytes & 7u))) return WFB_E_BADARG;
-        if (!ctl) CK(cudaMalloc(&ctl, sizeof(uint32_t) * CTL_WORDS));
+        CK(ctl.ensure(CTL_WORDS));
         const bool ranked = ready_ctl && !few_bins;
         const uint16_t *rows = h16_rows ? h16_rows : wideH;
         uint32_t tiles, chunk_shift, chunks;
@@ -238,7 +197,7 @@ struct RadixSorter {
         uint32_t *c = ready_ctl ? ready_ctl : ctl;
         if (!ready_ctl) { int rc = prepare_wide(c, s); if (rc) return rc; }
         if (ranked) { // first output position of every (chunk, digit) and (tile, digit) + digit counts
-            if (!wideDone) { CK(cudaMalloc(&wideDone, sizeof(uint32_t))); CK(cudaMemsetAsync(wideDone, 0, sizeof(uint32_t), s)); }
+            CK(wideDone.ensure_zeroed(1, s));
             k_wide_tile_bases<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, chunks, wideC, wideT, c, wideDone);
         } else if (ready_ctl) { // a few bins (destinations): chunk sums + the global counts
             k_wide_chunk_sums16<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, wideC, c);
@@ -296,17 +255,17 @@ struct RadixSorter {
              cudaStream_t s, const K **skeys, const uint32_t **svals, uint32_t *ready_ctl = nullptr, uint32_t *seg_first = nullptr, uint32_t seg_first_n = 0, uint32_t base_shift = 0)
     {
         // ready_ctl != nullptr: histograms already accumulated there by the producer of the keys (after prepare())
-        uint32_t *const own_ctl = ctl;
         const bool hist_ready = ready_ctl != nullptr;
-        if (hist_ready) ctl = ready_ctl;
-        struct Restore { uint32_t *&c; uint32_t *v; ~Restore() { c = v; } } restore{ctl, own_ctl};
+        if (!hist_ready) CK(ctl.ensure(CTL_WORDS));
+        uint32_t *const c = hist_ready ? ready_ctl : static_cast<uint32_t *>(ctl);
         const uint32_t TE = OS_THREADS * OS_ITEMS;
-        int rc = ensure(cap, OS_THREADS * 4, s, 256); if (rc) return rc;
+        const uint64_t state_words = static_cast<uint64_t>((cap + OS_THREADS * 4 - 1) / (OS_THREADS * 4)) * 256;
+        CK(state.ensure_zeroed(state_words, s, s, state_words));
         passes = std::min<uint32_t>(std::max(1u, passes), OS_MAX_PASSES);
         const uint32_t tiles = std::max(1u, (cap + TE - 1) / TE);
         if (!hist_ready) {
-            CK(cudaMemsetAsync(ctl, 0, sizeof(uint32_t) * (passes * 256 + passes), s));
-            k_radix_ghist<K><<<std::min(tiles, static_cast<uint32_t>(g_num_sms) * 4u), 256, 0, s>>>(kA, n_ptr, n_host, passes, ctl, base_shift);
+            CK(cudaMemsetAsync(c, 0, sizeof(uint32_t) * (passes * 256 + passes), s));
+            k_radix_ghist<K><<<std::min(tiles, static_cast<uint32_t>(g_num_sms) * 4u), 256, 0, s>>>(kA, n_ptr, n_host, passes, c, base_shift);
             launches++;
         }
         const K *kin = kA; const uint32_t *vin = nullptr;
@@ -314,7 +273,7 @@ struct RadixSorter {
         for (uint32_t p = 0; p < passes; p++) {
             epoch = (epoch + 1) & 0x3fffffffu; if (epoch == 0) epoch = 1;
             uint32_t *sf = (p + 1 == passes) ? seg_first : nullptr;
-            k_onesweep_pass<K><<<tiles, OS_THREADS, 0, s>>>(kin, vin, kout, vout, n_ptr, n_host, p, passes, ctl, state, epoch, sf, seg_first_n, base_shift);
+            k_onesweep_pass<K><<<tiles, OS_THREADS, 0, s>>>(kin, vin, kout, vout, n_ptr, n_host, p, passes, c, state, epoch, sf, seg_first_n, base_shift);
             kin = kout; vin = vout;
             if (kout == kB) { kout = kA; vout = vA; } else { kout = kB; vout = vB; }
         }
@@ -423,30 +382,26 @@ struct wfb_engine {
     uint64_t launches = 0;
     // scratch of the per-batch keyed operators (sort buffers), grown on demand
     uint32_t key_bits = 64;
-    uint32_t cap = 0;
-    uint64_t *keysA = nullptr, *keysB = nullptr;
-    uint32_t *idxA = nullptr, *idxB = nullptr, *destA = nullptr, *destB = nullptr;
-    uint32_t *head = nullptr, *seg_begin = nullptr;
+    Scratch<uint64_t> keysA, keysB;
+    Scratch<uint32_t> idxA, idxB, destA, destB;
+    Scratch<uint32_t> head, seg_begin;
     // wfb_shard_lift: lifted records / destinations of one segment, tile t owns positions [t*TILE, +TILE)
-    unsigned char *sh_lifted = nullptr; uint32_t *sh_dest = nullptr, *sh_ctl = nullptr; uint64_t sh_cap = 0;
+    Scratch<unsigned char> sh_lifted; Scratch<uint32_t> sh_dest, sh_ctl;
     // wfb_reduce_by_key_batches: element offset of every batch, first segment of every batch, segment total
-    uint32_t *rb_off = nullptr, *rb_first = nullptr, *rb_total = nullptr; uint32_t rb_cap = 0;
-    uint32_t *rb_long = nullptr; uint32_t rb_long_cap = 0; // segments folded by a warp; rb_total[1] = their number
+    Scratch<uint32_t> rb_off, rb_first, rb_total;
+    Scratch<uint32_t> rb_long; // segments folded by a warp; rb_total[1] = their number
     RadixSorter sorter;
     // Reduce_GPU over keys that are not integers: the order words of the keys (whi: two-word keys) and the permutation of the first sort
-    uint64_t *wlo = nullptr, *whi = nullptr; uint32_t *wperm = nullptr; uint32_t wcap = 0;
+    Scratch<uint64_t> wlo, whi; Scratch<uint32_t> wperm;
 
+    // the sort buffers, all of keysA's capacity (seg_begin: one more)
     int ensure_sort(uint32_t n, cudaStream_t s)
     {
-        if (n <= cap) return 0;
-        CK(cudaStreamSynchronize(s));
-        cudaFree(keysA); cudaFree(keysB); cudaFree(idxA); cudaFree(idxB); cudaFree(destA); cudaFree(destB);
-        cudaFree(head); cudaFree(seg_begin);
-        cap = std::max(n, 2 * cap);
-        CK(cudaMalloc(&keysA, sizeof(uint64_t) * cap)); CK(cudaMalloc(&keysB, sizeof(uint64_t) * cap));
-        CK(cudaMalloc(&idxA, sizeof(uint32_t) * cap)); CK(cudaMalloc(&idxB, sizeof(uint32_t) * cap));
-        CK(cudaMalloc(&destA, sizeof(uint32_t) * cap)); CK(cudaMalloc(&destB, sizeof(uint32_t) * cap));
-        CK(cudaMalloc(&head, sizeof(uint32_t) * cap)); CK(cudaMalloc(&seg_begin, sizeof(uint32_t) * (static_cast<size_t>(cap) + 1)));
+        CK(keysA.ensure(n, s));
+        const size_t cap = keysA.capacity();
+        CK(keysB.ensure(n, s, cap)); CK(idxA.ensure(n, s, cap)); CK(idxB.ensure(n, s, cap));
+        CK(destA.ensure(n, s, cap)); CK(destB.ensure(n, s, cap));
+        CK(head.ensure(n, s, cap)); CK(seg_begin.ensure(n + 1ull, s, cap + 1));
         return 0;
     }
     // stable LSD radix sort of (keysA[i], i) by key over `bits` bits; returns the buffers holding the result
@@ -465,13 +420,9 @@ struct wfb_engine {
     {
         const bool two = ops->key_bytes == 16;
         const uint32_t bits = 8u * ops->key_size, lo_bits = std::min(bits, 64u), hi_bits = two ? bits - 64u : 0u;
-        if (n > wcap) {
-            CK(cudaStreamSynchronize(s));
-            cudaFree(wlo); cudaFree(whi); cudaFree(wperm); wlo = whi = nullptr; wperm = nullptr;
-            wcap = std::max(n, cap);
-            CK(cudaMalloc(&wlo, sizeof(uint64_t) * wcap));
-            if (two) { CK(cudaMalloc(&whi, sizeof(uint64_t) * wcap)); CK(cudaMalloc(&wperm, sizeof(uint32_t) * wcap)); }
-        }
+        const size_t wcap = std::max<size_t>(n, keysA.capacity());
+        CK(wlo.ensure(n, s, wcap));
+        if (two) { CK(whi.ensure(n, s, wcap)); CK(wperm.ensure(n, s, wcap)); }
         int rc = ops->key_order_words(batches, boff, nb, static_cast<const unsigned char *>(tuples), n, wlo, whi, s, pp()); if (rc) return rc;
         CK(cudaMemcpyAsync(keysA, wlo, sizeof(uint64_t) * n, cudaMemcpyDeviceToDevice, s));
         const uint64_t *sk; const uint32_t *perm;
@@ -493,44 +444,30 @@ struct wfb_engine {
         launches += 4;
         return 0;
     }
-    void free_sort()
-    {
-        cudaFree(keysA); cudaFree(keysB); cudaFree(idxA); cudaFree(idxB); cudaFree(destA); cudaFree(destB);
-        cudaFree(head); cudaFree(seg_begin);
-        cudaFree(sh_lifted); cudaFree(sh_dest); cudaFree(sh_ctl);
-        cudaFree(rb_off); cudaFree(rb_first); cudaFree(rb_total); cudaFree(rb_long);
-        cudaFree(wlo); cudaFree(whi); cudaFree(wperm);
-        sorter.destroy();
-    }
 };
 
 // per-segment scratch of one Ffat_Windows_GPU; two sets when the handle is pipelined (the ingest pass of segment k+1
 // overlaps sort + update of segment k)
 struct SegScratch {
-    uint32_t cap = 0;                     // capacity in records
-    unsigned char *lifted = nullptr, *lifted_sorted = nullptr;
-    uint32_t *slotsA = nullptr, *slotsB = nullptr, *posA = nullptr, *posB = nullptr;
-    uint32_t *batch_off = nullptr; uint32_t batch_off_cap = 0;
-    DevBatch *d_batches = nullptr; uint32_t batch_cap = 0;
+    Scratch<uint32_t> slotsA, slotsB, posA, posB; // the segment's capacity in records: slotsA's
+    Scratch<unsigned char> lifted, lifted_sorted;
+    Scratch<uint32_t> batch_off; Scratch<DevBatch> d_batches;
     uint32_t *n_total = nullptr;
-    uint16_t *h16 = nullptr; uint32_t h16_tiles = 0; // pipelined handles: this segment's own rows (the next segment's tile pass files its rows while
-                                                     // this segment's partition still reads these)
+    Scratch<uint16_t> h16; // pipelined handles: this segment's own rows (the next segment's tile pass files its rows while this segment's
+                           // partition still reads these)
     const unsigned char *lifted_src = nullptr; // records of this segment: `lifted`, or the caller's buffer (in-place ingest)
     uint32_t *seg_cnt = nullptr;          // per-slot item counts of the segment (max_keys)
-    Trigger *trig = nullptr; uint32_t *n_trig = nullptr; uint32_t trig_cap = 0;
+    Scratch<Trigger> trig; uint32_t *n_trig = nullptr;
     uint32_t *n_heavy = nullptr;
     uint32_t *sort_ctl = nullptr;         // digit histograms + tickets of this segment's slot sort
     // pipelined mode: results of the segment wait here until the next call / flush delivers them
-    unsigned char *res = nullptr; uint64_t *res_ts = nullptr; uint32_t *res_n = nullptr; uint32_t res_cap = 0;
+    Scratch<unsigned char> res; Scratch<uint64_t> res_ts; uint32_t *res_n = nullptr;
     cudaEvent_t ev_ingest = nullptr, ev_done = nullptr;
     bool pending = false;
     uint32_t nbatches = 0, total = 0;
 
     void destroy()
     {
-        cudaFree(lifted); cudaFree(lifted_sorted); cudaFree(slotsA); cudaFree(slotsB); cudaFree(posA); cudaFree(posB);
-        cudaFree(batch_off); cudaFree(d_batches); cudaFree(n_total); cudaFree(seg_cnt); cudaFree(trig); cudaFree(sort_ctl);
-        cudaFree(res); cudaFree(res_ts); cudaFree(h16); // n_trig and res_n live inside the n_total allocation
         if (ev_ingest) cudaEventDestroy(ev_ingest);
         if (ev_done) cudaEventDestroy(ev_done);
     }
@@ -557,15 +494,15 @@ struct wfb_ffat {
     TbDev tb{};
     wfb_ffat *cb = nullptr;
     uint64_t tb_lateness = 0;
-    uint32_t tb_cap = 0, tb_pop_cap = 0;            // scratch capacities (tuples per batch, popped panes)
-    uint64_t *tb_kA = nullptr, *tb_kB = nullptr; uint32_t *tb_iA = nullptr, *tb_iB = nullptr;
-    unsigned char *tb_lifted = nullptr, *tb_part = nullptr, *tb_popped = nullptr;
-    uint32_t *tb_popped_slots = nullptr;
+    Scratch<uint64_t> tb_kA, tb_kB; Scratch<uint32_t> tb_iA, tb_iB; // scratch of a batch (capacity in tuples: tb_kA's)
+    Scratch<unsigned char> tb_lifted, tb_part;
+    Scratch<unsigned char> tb_popped; Scratch<uint32_t> tb_popped_slots; // the popped panes (capacity in records: tb_popped's / result bytes)
     bool shares_slot_key = false;                   // back end of a time-based handle: ff.slot_key / ff.n_slots belong to the front end
     uint32_t *own_n_slots = nullptr;                // the allocation behind ff.n_slots / ff.err_flags of this handle
-    uint32_t *tb_head = nullptr, *tb_seg = nullptr, *tb_misc = nullptr; // misc: [0] n_segs [1] first_seg dummy [2] n_present [3] popped total [4] ignored [5] ring capacity needed [6] ignored before the batch (growing handles)
+    Scratch<uint32_t> tb_head, tb_seg;
+    uint32_t *tb_misc = nullptr;    // [0] n_segs [1] first_seg dummy [2] n_present [3] popped total [4] ignored [5] ring capacity needed [6] ignored before the batch (growing handles)
     GrowCheck growc;                // WFB_KEYS_GROW (ff.grow): the growth check after the key-inserting pass
-    uint32_t *mg_scratch = nullptr; // (internal, ffat_process_prebucketed) per-(bucket, sub-bucket, source) counts, their scan, run starts
+    Scratch<uint32_t> mg_scratch;   // (internal, ffat_process_prebucketed) per-(bucket, sub-bucket, source) counts, their scan, run starts
     bool append_results = false;  // (internal, wfb_mg_flush) the next call's results follow the ones already in the output buffer
     bool buckets = true;          // one wide radix pass + per-bucket CTAs (<= 65536 keys); else the full sort + thread-per-key update
     uint32_t bucket_shift = 0;    // the wide pass partitions on (slot >> bucket_shift) & 1023
@@ -647,7 +584,6 @@ int wfb_engine_destroy(wfb_engine_t *e)
     if (!e) return 0;
     cudaDeviceSynchronize();
     e->ts.destroy();
-    e->free_sort();
     delete e;
     return 0;
 }
@@ -809,24 +745,14 @@ int wfb_reduce_by_key_batches(wfb_engine_t *e, const wfb_batch_t *in_h, const wf
     const uint32_t n = static_cast<uint32_t>(total);
     rc = e->ensure_sort(n, s); if (rc) return rc;
     rc = e->ts.ensure_batches(nbatches); if (rc) return rc;
-    if (nbatches > e->rb_cap) {
-        CK(cudaStreamSynchronize(s));
-        cudaFree(e->rb_off); cudaFree(e->rb_first);
-        e->rb_cap = std::max(nbatches, 2 * e->rb_cap);
-        CK(cudaMalloc(&e->rb_off, sizeof(uint32_t) * (static_cast<size_t>(e->rb_cap) + 1)));
-        CK(cudaMalloc(&e->rb_first, sizeof(uint32_t) * e->rb_cap));
-        if (!e->rb_total) CK(cudaMalloc(&e->rb_total, sizeof(uint32_t) * 2));
-    }
+    CK(e->rb_first.ensure(nbatches, s));
+    CK(e->rb_off.ensure(nbatches + 1ull, s, e->rb_first.capacity() + 1));
+    CK(e->rb_total.ensure(2));
     { int rc_ = e->ts.stage.h2d(e->ts.d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
     { int rc_ = e->ts.stage.h2d(e->rb_off, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
     CK(cudaMemsetAsync(e->rb_first, 0xff, sizeof(uint32_t) * nbatches, s));
     CK(cudaMemsetAsync(e->rb_total, 0, sizeof(uint32_t) * 2, s));
-    if (n / RB_LONG + 1 > e->rb_long_cap) {
-        CK(cudaStreamSynchronize(s));
-        cudaFree(e->rb_long);
-        e->rb_long_cap = std::max(n / RB_LONG + 1, 2 * e->rb_long_cap);
-        CK(cudaMalloc(&e->rb_long, sizeof(uint32_t) * e->rb_long_cap));
-    }
+    CK(e->rb_long.ensure(n / RB_LONG + 1, s));
     const uint32_t kb = nbatches == 1 ? 64u : key_bits; // a single batch needs no composite key
     if (ranked) rc = e->rank_keys(e->ts.d_batches, e->rb_off, nbatches, nullptr, n, s);
     else rc = e->ops->extract_keys_batches(e->ts.d_batches, e->rb_off, nbatches, n, kb, e->keysA, s, e->pp());
@@ -939,14 +865,9 @@ static int shard_lift_impl(wfb_engine_t *e, const wfb_functors_t *pre, const wfb
     if (positions > 0x7fffffffull || (bucketed && positions > region_capacity)) return WFB_E_BADARG;
     nbatches = static_cast<uint32_t>(hb.size());
     const size_t RB = e->ops->result_bytes;
-    if (positions > e->sh_cap) {
-        CK(cudaStreamSynchronize(s));
-        cudaFree(e->sh_lifted); cudaFree(e->sh_dest);
-        e->sh_cap = std::max<uint64_t>(positions, 2 * e->sh_cap);
-        CK(cudaMalloc(&e->sh_lifted, e->sh_cap * RB));
-        CK(cudaMalloc(&e->sh_dest, e->sh_cap * sizeof(uint32_t)));
-    }
-    if (!e->sh_ctl) CK(cudaMalloc(&e->sh_ctl, sizeof(uint32_t) * RadixSorter::CTL_WORDS));
+    CK(e->sh_dest.ensure(positions, s));
+    CK(e->sh_lifted.ensure(positions * RB, s, e->sh_dest.capacity() * RB));
+    CK(e->sh_ctl.ensure(RadixSorter::CTL_WORDS));
     rc = e->ts.ensure_tiles(tiles); if (rc) return rc;
     rc = e->ts.ensure_batches(nbatches); if (rc) return rc;
     { int rc_ = e->ts.stage.h2d(e->ts.d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
@@ -998,10 +919,9 @@ struct wfb_kstate {
     RadixSorter sorter;
     bool buckets = true;          // at most 65536 keys: buckets of at most 64 keys (k_ks_apply); else a full sort (k_ks_apply_runs)
     uint32_t bucket_shift = 0, sort_passes = 0;
-    DevBatch *d_batches = nullptr; uint32_t *d_boff = nullptr; uint32_t batch_cap = 0;
-    uint32_t cap = 0;             // tuples per call
-    uint32_t *slotsA = nullptr, *slotsB = nullptr, *posA = nullptr, *posB = nullptr, *tile_cnt = nullptr, *rank_start = nullptr;
-    unsigned char *keep = nullptr;
+    Scratch<DevBatch> d_batches; Scratch<uint32_t> d_boff, rank_start; // capacity in batches: d_batches'
+    Scratch<uint32_t> slotsA, slotsB, posA, posB, tile_cnt;           // capacity in tuples per call: slotsA's
+    Scratch<unsigned char> keep;
     uint64_t launches = 0;
     PinnedStage stage;
     GrowCheck growc;              // WFB_KEYS_GROW (ff.grow)
@@ -1057,9 +977,7 @@ int wfb_kstate_destroy(wfb_kstate_t *h)
     if (!h) return 0;
     cudaDeviceSynchronize();
     cudaFree(h->ff.ht_keys); cudaFree(h->ff.ht_slots); cudaFree(h->ff.n_slots); cudaFree(h->ff.slot_key); cudaFree(h->states);
-    cudaFree(h->d_batches); cudaFree(h->d_boff); cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posA); cudaFree(h->posB); cudaFree(h->tile_cnt);
-    cudaFree(h->rank_start); cudaFree(h->keep);
-    h->sorter.destroy(); h->stage.destroy(); h->growc.destroy();
+    h->stage.destroy(); h->growc.destroy();
     delete h;
     cudaGetLastError();
     return 0;
@@ -1091,22 +1009,14 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
     if (total == 0) return 0;
     if (total > 0x7fffffffull) return WFB_E_BADARG;
     const uint32_t n = static_cast<uint32_t>(total);
-    if (nbatches > h->batch_cap) {
-        CK(cudaStreamSynchronize(s));
-        cudaFree(h->d_batches); cudaFree(h->d_boff); cudaFree(h->rank_start);
-        h->batch_cap = std::max(nbatches, 2 * h->batch_cap);
-        CK(cudaMalloc(&h->d_batches, sizeof(DevBatch) * h->batch_cap));
-        CK(cudaMalloc(&h->d_boff, sizeof(uint32_t) * (static_cast<size_t>(h->batch_cap) + 1)));
-        CK(cudaMalloc(&h->rank_start, sizeof(uint32_t) * (static_cast<size_t>(h->batch_cap) + 1)));
-    }
-    if (n > h->cap) {
-        CK(cudaStreamSynchronize(s));
-        cudaFree(h->slotsA); cudaFree(h->slotsB); cudaFree(h->posA); cudaFree(h->posB); cudaFree(h->tile_cnt); cudaFree(h->keep);
-        h->cap = std::max(n, 2 * h->cap);
-        CK(cudaMalloc(&h->slotsA, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->slotsB, sizeof(uint32_t) * h->cap));
-        CK(cudaMalloc(&h->posA, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->posB, sizeof(uint32_t) * h->cap)); CK(cudaMalloc(&h->keep, h->cap));
-        CK(cudaMalloc(&h->tile_cnt, sizeof(uint32_t) * ((h->cap + SEGT - 1) / SEGT + 1)));
-    }
+    CK(h->d_batches.ensure(nbatches, s));
+    const size_t bcap = h->d_batches.capacity();
+    CK(h->d_boff.ensure(nbatches + 1ull, s, bcap + 1)); CK(h->rank_start.ensure(nbatches + 1ull, s, bcap + 1));
+    CK(h->slotsA.ensure(n, s));
+    const size_t cap = h->slotsA.capacity();
+    CK(h->slotsB.ensure(n, s, cap)); CK(h->posA.ensure(n, s, cap)); CK(h->posB.ensure(n, s, cap)); CK(h->keep.ensure(n, s, cap));
+    const size_t cnt_cap = (cap + SEGT - 1) / SEGT + 1;
+    CK(h->tile_cnt.ensure(cnt_cap, s, cnt_cap));
     { int rc_ = h->stage.h2d(h->d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
     { int rc_ = h->stage.h2d(h->d_boff, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
     // 1. slots; 2. one wide partition pass into 1024 buckets of consecutive slots; 3. per-bucket CTAs, one thread per key
@@ -1214,14 +1124,11 @@ static void ffat_plan_state(wfb_ffat *h, GrowPlan &plan, uint32_t cap)
     plan.add(ff.heavy, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, false, -1);
     SegScratch &g = h->seg[0]; // (growing handles are not pipelined: one segment scratch)
     plan.add(g.seg_cnt, sizeof(uint32_t) * old, sizeof(uint32_t) * cap, false, 0); // (a rerun pass counts the segment's items again)
-    if (g.trig) plan.add(g.trig, sizeof(Trigger) * g.trig_cap, sizeof(Trigger) * ffat_trig_cap(h, g.cap, cap), false, -1, false);
 }
 static void ffat_derive(wfb_ffat *h, uint32_t cap)
 {
     h->ff.max_keys = cap;
-    SegScratch &g = h->seg[0];
-    if (g.trig) g.trig_cap = ffat_trig_cap(h, g.cap, cap);
-    ffat_derive_paths(h);
+    ffat_derive_paths(h); // (the rerun pass sizes the window groups for the new capacity: ffat_ensure_segment)
 }
 static int ffat_grow(wfb_ffat *h, cudaStream_t s, bool *grew)
 {
@@ -1327,16 +1234,11 @@ static int tb_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, ui
 
 static int tb_ensure(wfb_ffat *h, uint32_t n, cudaStream_t s)
 {
-    if (n <= h->tb_cap) return 0;
-    CK(cudaStreamSynchronize(s));
-    cudaFree(h->tb_kA); cudaFree(h->tb_kB); cudaFree(h->tb_iA); cudaFree(h->tb_iB); cudaFree(h->tb_lifted); cudaFree(h->tb_part);
-    cudaFree(h->tb_head); cudaFree(h->tb_seg);
-    h->tb_cap = std::max(n, 2 * h->tb_cap);
-    const size_t RB = h->ops->result_bytes, c = h->tb_cap;
-    CK(cudaMalloc(&h->tb_kA, sizeof(uint64_t) * c)); CK(cudaMalloc(&h->tb_kB, sizeof(uint64_t) * c));
-    CK(cudaMalloc(&h->tb_iA, sizeof(uint32_t) * c)); CK(cudaMalloc(&h->tb_iB, sizeof(uint32_t) * c));
-    CK(cudaMalloc(&h->tb_lifted, RB * c)); CK(cudaMalloc(&h->tb_part, RB * c));
-    CK(cudaMalloc(&h->tb_head, sizeof(uint32_t) * ((c + SEGT - 1) / SEGT + 1))); CK(cudaMalloc(&h->tb_seg, sizeof(uint32_t) * (c + 1)));
+    CK(h->tb_kA.ensure(n, s));
+    const size_t RB = h->ops->result_bytes, c = h->tb_kA.capacity(), head_cap = (c + SEGT - 1) / SEGT + 1;
+    CK(h->tb_kB.ensure(n, s, c)); CK(h->tb_iA.ensure(n, s, c)); CK(h->tb_iB.ensure(n, s, c));
+    CK(h->tb_lifted.ensure(RB * n, s, RB * c)); CK(h->tb_part.ensure(RB * n, s, RB * c));
+    CK(h->tb_head.ensure(head_cap, s, head_cap)); CK(h->tb_seg.ensure(n + 1ull, s, c + 1));
     return 0;
 }
 
@@ -1411,13 +1313,10 @@ int wfb_ffat_process_tb(wfb_ffat_t *h, const wfb_functors_t *pre, const wfb_batc
         uint32_t total = 0;
         CK(cudaMemcpyAsync(&total, misc + 3, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));                           // (the reference synchronises here as well, :962)
-        if (total > h->tb_pop_cap) {
-            cudaFree(h->tb_popped); cudaFree(h->tb_popped_slots);
-            h->tb_pop_cap = std::max(total, 2 * h->tb_pop_cap);
-            CK(cudaMalloc(&h->tb_popped, RB * h->tb_pop_cap));
-            CK(cudaMalloc(&h->tb_popped_slots, sizeof(uint32_t) * ((static_cast<size_t>(h->tb_pop_cap) + TILE - 1) / TILE * TILE)));
-        }
-        rc = h->ops->tb_pop_write(h->ff, h->tb, F, h->tb.cnt, h->tb_popped, h->tb_popped_slots, h->tb_pop_cap, maxp, s, prm); if (rc) return rc;
+        CK(h->tb_popped.ensure(RB * total));
+        const size_t pop_cap = h->tb_popped.capacity() / RB, slots_cap = (pop_cap + TILE - 1) / TILE * TILE;
+        CK(h->tb_popped_slots.ensure(slots_cap, ScratchWaits(), slots_cap));
+        rc = h->ops->tb_pop_write(h->ff, h->tb, F, h->tb.cnt, h->tb_popped, h->tb_popped_slots, static_cast<uint32_t>(pop_cap), maxp, s, prm); if (rc) return rc;
         h->launches += 10 + (h->sorter.launches - before);
         // 7. the count-based back end consumes the popped panes as one batch with this batch's watermark
         if (total) {
@@ -1504,7 +1403,7 @@ int wfb_ffat_create(wfb_ffat_t **hh, int prog, uint64_t win, uint64_t slide, uin
         CK(cudaMemset(g.seg_cnt, 0, sizeof(uint32_t) * max_keys));
         ALLOC(g.n_total, sizeof(uint32_t) * 4);
         CK(cudaMemset(g.n_total, 0, sizeof(uint32_t) * 4));
-        g.n_trig = g.n_total + 1; g.res_n = nullptr; g.n_heavy = g.n_total + 3;
+        g.n_trig = g.n_total + 1; g.res_n = h->pipelined ? g.n_total + 2 : nullptr; g.n_heavy = g.n_total + 3;
         ALLOC(g.sort_ctl, sizeof(uint32_t) * RadixSorter::CTL_WORDS);
         CK(cudaEventCreateWithFlags(&g.ev_ingest, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&g.ev_done, cudaEventDisableTiming));
@@ -1533,14 +1432,11 @@ int wfb_ffat_destroy(wfb_ffat_t *h)
     cudaDeviceSynchronize();
     FfatDev &ff = h->ff;
     cudaFree(ff.ht_keys); cudaFree(ff.ht_slots); cudaFree(h->own_n_slots); if (!h->shares_slot_key) cudaFree(ff.slot_key); cudaFree(ff.cnt);
-    cudaFree(ff.acc); cudaFree(ff.tree); cudaFree(ff.seg_off); cudaFree(ff.heavy); cudaFree(h->mg_scratch);
-    for (int p = 0; p < 2; p++) h->seg[p].destroy();
-    h->sorter.destroy();
+    cudaFree(ff.acc); cudaFree(ff.tree); cudaFree(ff.seg_off); cudaFree(ff.heavy);
+    for (SegScratch &g : h->seg) { cudaFree(g.n_total); cudaFree(g.seg_cnt); cudaFree(g.sort_ctl); g.destroy(); } // (n_trig, n_heavy, res_n: inside n_total)
     if (h->cb) wfb_ffat_destroy(h->cb);
     cudaFree(h->tb.first); cudaFree(h->tb.num); cudaFree(h->tb.num_new); cudaFree(h->tb.trig); cudaFree(h->tb.done); cudaFree(h->tb.ring);
     cudaFree(h->tb.present); cudaFree(h->tb.cnt); cudaFree(h->tb_misc);
-    cudaFree(h->tb_kA); cudaFree(h->tb_kB); cudaFree(h->tb_iA); cudaFree(h->tb_iB); cudaFree(h->tb_lifted); cudaFree(h->tb_part);
-    cudaFree(h->tb_popped); cudaFree(h->tb_popped_slots); cudaFree(h->tb_head); cudaFree(h->tb_seg);
     if (h->s2) cudaStreamDestroy(h->s2);
     for (auto &e : h->tev) cudaEventDestroy(e);
     h->ts.destroy(); h->growc.destroy();
@@ -1574,34 +1470,21 @@ int wfb_ffat_set_key_shard(wfb_ffat_t *h, uint32_t num_shards, uint32_t shard)
 static double host_now_us() { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e6 + t.tv_nsec * 1e-3; }
 static int ffat_ensure_segment(wfb_ffat *h, SegScratch &g, uint32_t total, uint32_t nbatches, cudaStream_t s)
 {
-    if (total > g.cap) {
-        CK(cudaStreamSynchronize(s));
-        if (h->s2) CK(cudaStreamSynchronize(h->s2));
-        cudaFree(g.lifted); cudaFree(g.lifted_sorted); cudaFree(g.slotsA); cudaFree(g.slotsB); cudaFree(g.posA); cudaFree(g.posB);
-        cudaFree(g.trig); cudaFree(g.res); cudaFree(g.res_ts);
-        g.cap = std::max(total, 2 * g.cap);
-        const size_t RB = h->ops->result_bytes;
-        CK(cudaMalloc(&g.lifted, static_cast<size_t>(g.cap) * RB));
-        if (h->bucket_move) CK(cudaMalloc(&g.lifted_sorted, static_cast<size_t>(g.cap) * RB));
-        CK(cudaMalloc(&g.slotsA, sizeof(uint32_t) * g.cap)); CK(cudaMalloc(&g.slotsB, sizeof(uint32_t) * g.cap));
-        CK(cudaMalloc(&g.posA, sizeof(uint32_t) * g.cap)); CK(cudaMalloc(&g.posB, sizeof(uint32_t) * g.cap));
-        g.trig_cap = ffat_trig_cap(h, g.cap, h->ff.max_keys);
-        CK(cudaMalloc(&g.trig, sizeof(Trigger) * g.trig_cap));
-        if (h->pipelined) { // every group that can fire in one segment: trig_cap groups of Nb results
-            g.res_cap = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(g.trig_cap) * h->ff.nb, 0x7fffffffull));
-            CK(cudaMalloc(&g.res, static_cast<size_t>(g.res_cap) * RB));
-            CK(cudaMalloc(&g.res_ts, sizeof(uint64_t) * g.res_cap));
-            g.res_n = g.n_total + 2;
-        }
+    const ScratchWaits w = h->s2 ? ScratchWaits(s, h->s2) : ScratchWaits(s);
+    CK(g.slotsA.ensure(total, w));
+    const size_t cap = g.slotsA.capacity(), RB = h->ops->result_bytes;
+    CK(g.slotsB.ensure(total, w, cap)); CK(g.posA.ensure(total, w, cap)); CK(g.posB.ensure(total, w, cap));
+    CK(g.lifted.ensure(RB * total, w, RB * cap));
+    if (h->bucket_move) CK(g.lifted_sorted.ensure(RB * total, w, RB * cap));
+    // the window groups the segment can fire, for the current key capacity (key growth raises it before the pass runs again)
+    const uint32_t trig_cap = ffat_trig_cap(h, static_cast<uint32_t>(cap), h->ff.max_keys);
+    CK(g.trig.ensure(trig_cap, w, trig_cap));
+    if (h->pipelined) { // every group that can fire in one segment: trig_cap groups of Nb results
+        const size_t res_cap = std::min<uint64_t>(static_cast<uint64_t>(trig_cap) * h->ff.nb, 0x7fffffffull);
+        CK(g.res_ts.ensure(res_cap, w, res_cap)); CK(g.res.ensure(RB * res_cap, w, RB * res_cap));
     }
-    if (nbatches + 1 > g.batch_off_cap) {
-        CK(cudaStreamSynchronize(s));
-        if (h->s2) CK(cudaStreamSynchronize(h->s2));
-        cudaFree(g.batch_off); cudaFree(g.d_batches);
-        g.batch_off_cap = std::max(nbatches + 1, 2 * g.batch_off_cap);
-        CK(cudaMalloc(&g.batch_off, sizeof(uint32_t) * g.batch_off_cap));
-        CK(cudaMalloc(&g.d_batches, sizeof(DevBatch) * g.batch_off_cap));
-    }
+    CK(g.batch_off.ensure(nbatches + 1ull, w));
+    CK(g.d_batches.ensure(nbatches + 1ull, w, g.batch_off.capacity()));
     return 0;
 }
 
@@ -1616,8 +1499,9 @@ static int ffat_window_phase(wfb_ffat *h, SegScratch &g, const FfatDev &ff, unsi
         // ONE wide radix pass on the top 10 slot bits: 1024 buckets of consecutive keys, arrival order inside a bucket ...
         const uint32_t *counts = nullptr;
         rc = h->sorter.sort_wide<uint32_t>(g.slotsA, g.slotsB, g.posB, nullptr, g.total, g.total, h->bucket_shift, s, g.sort_ctl, &counts,
-                                           h->bucket_move ? g.lifted : nullptr, h->bucket_move ? g.lifted_sorted : nullptr,
-                                           static_cast<uint32_t>(h->ops->result_bytes), true, 0, 0, h->pipelined ? g.h16 : nullptr);
+                                           h->bucket_move ? static_cast<unsigned char *>(g.lifted) : nullptr,
+                                           h->bucket_move ? static_cast<unsigned char *>(g.lifted_sorted) : nullptr,
+                                           static_cast<uint32_t>(h->ops->result_bytes), true, 0, 0, h->pipelined ? static_cast<uint16_t *>(g.h16) : nullptr);
         if (rc) return rc;
         h->launches += h->sorter.launches - before;
         h->mark(2, s);
@@ -1722,7 +1606,7 @@ static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_
         }
 
         ff = h->ff;
-        ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = g.trig_cap; ff.n_heavy = g.n_heavy;
+        ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = static_cast<uint32_t>(g.trig.capacity()); ff.n_heavy = g.n_heavy;
 
         // the streaming pass also counts the digits of the slot sort that follows
         const uint32_t npasses = h->buckets ? 1u : h->sort_passes;
@@ -1758,16 +1642,11 @@ static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_
             // a CTA claims the 16 tiles of a wide tile at once, counts its digits in shared memory and files the row itself, and packs a
             // rank with every slot (bucket-path slots fit 16 bits): the partition that follows needs neither a counting pass nor the
             // per-CTA global digit counts
-            if (h->pipelined && (g.total + OSW_TILE - 1) / OSW_TILE > h->sorter.wide_tiles) CK(cudaStreamSynchronize(h->s2)); // (the rows are about to be re-allocated)
-            rc = h->sorter.ensure_wide(g.total, s, &a.wide_h16); if (rc) return rc; // (also sizes the chunk rows the partition needs)
+            const ScratchWaits w = h->pipelined ? ScratchWaits(s, h->s2) : ScratchWaits(s);
+            rc = h->sorter.ensure_wide(g.total, w, &a.wide_h16); if (rc) return rc; // (also sizes the chunk rows the partition needs)
             if (h->pipelined) {
-                const uint32_t wt = (g.total + OSW_TILE - 1) / OSW_TILE;
-                if (wt > g.h16_tiles) {
-                    CK(cudaStreamSynchronize(s)); CK(cudaStreamSynchronize(h->s2));
-                    cudaFree(g.h16);
-                    g.h16_tiles = std::max(wt, 2 * g.h16_tiles);
-                    CK(cudaMalloc(&g.h16, sizeof(uint16_t) * OSW_DIGITS * g.h16_tiles));
-                }
+                const size_t wt = (g.total + OSW_TILE - 1) / OSW_TILE;
+                CK(g.h16.ensure(OSW_DIGITS * wt, w));
                 a.wide_h16 = g.h16;
             }
             a.tiles_per_ticket = OSW_TILE_POS / TILE;
@@ -1804,7 +1683,7 @@ static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_
         rc = ffat_deliver(h, prev, out, out_ts, out_capacity, n_out_dev, s); if (rc) return rc;
         CK(cudaStreamWaitEvent(h->s2, g.ev_ingest, 0));
         CK(cudaMemsetAsync(g.res_n, 0, sizeof(uint32_t), h->s2));
-        rc = ffat_window_phase(h, g, ff, g.res, g.res_ts, g.res_cap, g.res_n, h->s2); if (rc) return rc;
+        rc = ffat_window_phase(h, g, ff, g.res, g.res_ts, static_cast<uint32_t>(g.res_ts.capacity()), g.res_n, h->s2); if (rc) return rc;
         h->mark(3, h->s2);
         CK(cudaEventRecord(g.ev_done, h->s2));
         g.pending = true;
@@ -1839,7 +1718,7 @@ static int ffat_process_prebucketed(wfb_ffat *h, const unsigned char *records, c
     { int rc_ = h->ts.stage.h2d(g.batch_off, offs_h, sizeof(uint32_t) * (nsrc + 1), s); if (rc_) return rc_; }
     g.nbatches = nsrc; g.total = total; g.lifted_src = records;
     FfatDev ff = h->ff;
-    ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = g.trig_cap; ff.n_heavy = g.n_heavy;
+    ff.seg_cnt = g.seg_cnt; ff.trig = g.trig; ff.n_trig = g.n_trig; ff.trig_cap = static_cast<uint32_t>(g.trig.capacity()); ff.n_heavy = g.n_heavy;
     rc = RadixSorter::prepare_wide(g.sort_ctl, s); if (rc) return rc; // (buckets at or above bps stay empty)
     h->mark(0, s); h->mark(1, s);
     MgRuns runs;
@@ -1847,7 +1726,7 @@ static int ffat_process_prebucketed(wfb_ffat *h, const unsigned char *records, c
     // the sources' 1024 bins are shared by all destinations: split every coarse bucket so that the update kernel gets (up to) 1024 buckets
     uint32_t nsub = 1, shift2 = shift;
     while (nsub * 2 * bps <= OSW_DIGITS && nsub * 2 <= MAX_SHARDS && shift2 > 0) { nsub *= 2; shift2--; }
-    if (!h->mg_scratch) CK(cudaMalloc(&h->mg_scratch, sizeof(uint32_t) * 3 * OSW_DIGITS * MAX_SHARDS));
+    CK(h->mg_scratch.ensure(3 * OSW_DIGITS * MAX_SHARDS));
     uint32_t *cnt3 = h->mg_scratch, *off3 = cnt3 + OSW_DIGITS * MAX_SHARDS, *run_starts = off3 + OSW_DIGITS * MAX_SHARDS;
     const dim3 grid(bps, nsrc);
     k_mg_count<<<grid, MG_THREADS, 0, s>>>(bins, nsrc, bps, runs, recv_slots, slot_mask, shift2, nsub, cnt3, run_starts, g.n_trig, g.n_heavy);
@@ -1976,8 +1855,9 @@ __global__ void k_mg_meta(const uint32_t *__restrict__ counts, uint64_t watermar
 __global__ void k_mg_pre_append(unsigned long long *results_total, const uint32_t *n_out) { if (results_total) *results_total -= *n_out; }
 
 struct MgSlot { // buffers of one step in flight (three: the exchange of step i-2 overlaps the source pass of step i)
-    unsigned char *regions = nullptr; uint32_t region_cap = 0; // records by destination (bucketed: bin after bin, region_cap = the segment's positions)
-    uint32_t *vslots = nullptr;                // bucketed: virtual slot of every record of `regions`
+    Scratch<unsigned char> regions;            // records by destination (bucketed: bin after bin, as many as the segment's positions)
+    uint32_t region_cap = 0;                   // not bucketed: records per destination region (the stride of `regions`)
+    Scratch<uint32_t> vslots;                  // bucketed: virtual slot of every record of `regions`
     uint32_t *bins = nullptr;                  // bucketed: OSW_DIGITS + 1 words, the bin sizes of this step's partition
     uint32_t *recv_slots = nullptr, *recv_bins = nullptr; size_t recv_slots_cap = 0; // bucketed: what the sources delivered ([nranks][bps] run lengths)
     unsigned char *ce_buf = nullptr;           // copy-engine exchange: the receive buffers of this slot in ONE allocation other ranks map (cudaIpc):
@@ -2040,8 +1920,8 @@ int wfb_mg_destroy(wfb_mg_t *h)
     if (h->eng) wfb_engine_destroy(h->eng);
     if (h->ffat) wfb_ffat_destroy(h->ffat);
     for (MgSlot &sl : h->slot) {
-        cudaFree(sl.regions); cudaFree(sl.counts); cudaFree(sl.send_meta); cudaFree(sl.recv_meta); if (!sl.ce_buf) cudaFree(sl.recv);
-        cudaFree(sl.vslots); cudaFree(sl.bins);
+        cudaFree(sl.counts); cudaFree(sl.send_meta); cudaFree(sl.recv_meta); if (!sl.ce_buf) cudaFree(sl.recv);
+        cudaFree(sl.bins);
         if (sl.ce_buf) { // (recv / recv_slots / recv_bins point into ce_buf)
             for (int p = 0; p < h->nranks; p++) if (p != h->rank && sl.peer[p]) cudaIpcCloseMemHandle(sl.peer[p]);
             cudaFree(sl.ce_buf); sl.recv = nullptr;
@@ -2223,26 +2103,19 @@ static int mg_source(wfb_mg *h, MgSlot &sl, const wfb_functors_t *pre, const wfb
         }
         CK(cudaEventRecord(sl.tr[0], s));
     }
+    const ScratchWaits waits = sl.used ? ScratchWaits::device() : ScratchWaits(); // (the exchange of the slot's last step reads the regions)
     if (h->bucketed) {
         uint64_t positions = 0;
         for (uint32_t i = 0; i < nbatches; i++) positions += static_cast<uint64_t>(tiles_of(batches_h[i].n)) * TILE;
         if (!h->ce_tried) { rc = mg_ce_setup(h, std::max<uint64_t>(positions, 1)); if (rc) return rc; } // (collective: every rank is in its first step)
-        if (sl.region_cap < positions) {
-            if (sl.used) CK(cudaDeviceSynchronize());
-            cudaFree(sl.regions); cudaFree(sl.vslots);
-            sl.region_cap = static_cast<uint32_t>(positions);
-            CK(cudaMalloc(&sl.regions, static_cast<size_t>(sl.region_cap) * h->rb));
-            CK(cudaMalloc(&sl.vslots, sizeof(uint32_t) * sl.region_cap));
-        }
-        rc = shard_lift_impl(h->eng, pre, batches_h, nbatches, static_cast<uint32_t>(h->nranks), sl.regions, sl.region_cap, sl.counts, s,
+        CK(sl.vslots.ensure(positions, waits, positions));
+        CK(sl.regions.ensure(positions * h->rb, waits, positions * h->rb));
+        rc = shard_lift_impl(h->eng, pre, batches_h, nbatches, static_cast<uint32_t>(h->nranks), sl.regions, static_cast<uint32_t>(sl.vslots.capacity()), sl.counts, s,
                              h->shard_slots, h->shard_keys, h->shift, sl.vslots, sl.bins, n ? sl.send_meta : nullptr, watermark);
     } else {
-        if (sl.region_cap < n) { // worst case: every item of the segment survives and goes to one shard
-            if (sl.used) CK(cudaDeviceSynchronize());
-            cudaFree(sl.regions);
-            sl.region_cap = static_cast<uint32_t>(n);
-            CK(cudaMalloc(&sl.regions, static_cast<size_t>(h->nranks) * sl.region_cap * h->rb));
-        }
+        const size_t region_bytes = static_cast<size_t>(h->nranks) * h->rb; // worst case: every item of the segment survives and goes to one shard
+        CK(sl.regions.ensure(n * region_bytes, waits, n * region_bytes));
+        sl.region_cap = static_cast<uint32_t>(sl.regions.capacity() / region_bytes);
         rc = wfb_shard_lift(h->eng, pre, batches_h, nbatches, static_cast<uint32_t>(h->nranks), sl.regions, sl.region_cap, sl.counts, s);
     }
     if (rc) return rc;
@@ -2364,9 +2237,10 @@ static int mg_exchange(wfb_mg *h, MgSlot &sl)
         if (sl.recv_bytes < need * h->rb || sl.recv_slots_cap < need) {
             CK(cudaDeviceSynchronize());
             cudaFree(sl.recv); cudaFree(sl.recv_slots);
-            sl.recv_slots_cap = need * 5 / 4; sl.recv_bytes = sl.recv_slots_cap * h->rb;
-            CK(cudaMalloc(&sl.recv, sl.recv_bytes));
-            CK(cudaMalloc(&sl.recv_slots, sizeof(uint32_t) * sl.recv_slots_cap));
+            sl.recv = nullptr; sl.recv_slots = nullptr; sl.recv_bytes = 0; sl.recv_slots_cap = 0; // (as a failed allocation leaves them)
+            const size_t cap = need * 5 / 4;
+            CK(cudaMalloc(&sl.recv, cap * h->rb)); sl.recv_bytes = cap * h->rb;
+            CK(cudaMalloc(&sl.recv_slots, sizeof(uint32_t) * cap)); sl.recv_slots_cap = cap;
         }
         if (sl.done_recorded) CK(cudaStreamWaitEvent(h->cs, sl.ev_done, 0)); // the window update that read these receive buffers two steps ago
         if (h->trace) CK(cudaEventRecord(sl.tr[4], h->cs));
@@ -2410,8 +2284,8 @@ static int mg_exchange(wfb_mg *h, MgSlot &sl)
     if (sl.recv_bytes < need) {
         CK(cudaDeviceSynchronize());
         cudaFree(sl.recv);
-        sl.recv_bytes = need * 5 / 4;
-        CK(cudaMalloc(&sl.recv, sl.recv_bytes));
+        sl.recv = nullptr; sl.recv_bytes = 0; // (as a failed allocation leaves them)
+        CK(cudaMalloc(&sl.recv, need * 5 / 4)); sl.recv_bytes = need * 5 / 4;
     }
     if (sl.done_recorded) CK(cudaStreamWaitEvent(h->cs, sl.ev_done, 0)); // the window update that read this receive buffer two steps ago
     if (h->trace) CK(cudaEventRecord(sl.tr[4], h->cs));
