@@ -190,6 +190,24 @@ struct FacadeStatefulProgram {
     __host__ __device__ static void map_stateful(tuple_t &t, state_t &st, const params_t &p) { MapF2 f = p.map; f(t, st); }
     __host__ __device__ static bool filter_stateful(tuple_t &t, state_t &st, const params_t &p) { FiltF2 f = p.filt; return f(t, st); }
 };
+// The program of a FlatMap_GPU: func(const tuple_t &, Shipper_GPU<result_t> &) after the fused run of stateless operators in front
+// (the filter slot runs maps and predicates in order). The window slots are never launched for it.
+template <class R> using Shipper_GPU = wfb::Shipper<R>; // push(const result_t &): the shipper of a FlatMap_GPU functor (wf/shipper.hpp)
+template <class T, class R, class FlatF>
+struct FacadeFlatMapProgram {
+    using tuple_t = T; using result_t = R; using key_t = uint64_t;
+    struct params_t { ChainStages<T> map; ChainStages<T> filt; FlatF fm; };
+    static_assert(std::is_trivially_copyable<T>::value && std::is_trivially_copyable<R>::value, "tuple_t / result_t must be trivially copyable");
+    static_assert(sizeof(T) % 8 == 0 && sizeof(R) % 8 == 0, "tuple_t / result_t sizes must be multiples of 8 bytes");
+    __host__ __device__ static void map(tuple_t &t, const params_t &p) { p.map(t); }
+    __host__ __device__ static bool filter(tuple_t &t, const params_t &p) { return p.filt(t); }
+    __host__ __device__ static void flatmap(const tuple_t &t, Shipper_GPU<result_t> &sh, const params_t &p) { FlatF f = p.fm; f(t, sh); }
+    __host__ __device__ static key_t key(const tuple_t &, const params_t &) { return 0; }
+    __host__ __device__ static void lift(const tuple_t &, result_t &, const params_t &) {}
+    __host__ __device__ static void comb(const result_t &, const result_t &, result_t &, const params_t &) {}
+    __host__ __device__ static result_t make_result(key_t, uint64_t, const params_t &) { return result_t(); }
+    __host__ __device__ static tuple_t reduce(const tuple_t &a, const tuple_t &, const params_t &) { return a; }
+};
 template <class T, class S> struct StatefulIdMap { __host__ __device__ void operator()(T &, S &) const {} };
 template <class T, class S> struct StatefulKeepAll { __host__ __device__ bool operator()(T &, S &) const { return true; } };
 
@@ -641,6 +659,130 @@ public:
 template <class F> using Map_GPU = Stateless_GPU<F, false>;
 template <class F> using Filter_GPU = Stateless_GPU<F, true>;
 
+// FlatMap_GPU (wf/flatmap.hpp with wf/shipper.hpp on the GPU): func(const tuple_t &, Shipper_GPU<result_t> &) pushes 0..m records per
+// tuple, m = withMaxOutputsPerTuple(m). ONE wfb_flatmap_batches call per svc() over the K batches found queued, with the fused run of
+// stateless operators in front of it: input batch i becomes output batch i (records in input order, per tuple in push order, each
+// with its tuple's timestamp), of capacity original_size * m, whose size stays on the device. The functor may run more than once per
+// tuple (it must push the same records every time). Pushes beyond the m-th of a tuple are dropped and counted on the device; a
+// non-zero count stops the program at the end of the stream with the operator's name and m.
+template <class shipper_t> struct shipper_result;
+template <class R> struct shipper_result<wfb::Shipper<R>> { using type = R; };
+
+template <class tuple_t, class result_t, class func_t>
+class FlatMapReplica: public Basic_Replica {
+    using prog_t = FacadeFlatMapProgram<tuple_t, result_t, func_t>;
+    using batch_t = Batch_GPU_t<tuple_t>;
+    wfb_engine_t *eng = nullptr; typename prog_t::params_t prm{};
+    uint32_t max_out; size_t maxk;
+    BatchPool<result_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
+    uint32_t *counts_d = nullptr, *counts_h = nullptr; size_t ring = 0; // deferred sizes + the drop count of every call
+    static constexpr size_t RING = 16 * (WF_MAX_BATCHES_PER_CALL + 1);
+    struct Pending { size_t word; cudaEvent_t ev; };
+    std::vector<Pending> pending; uint64_t dropped = 0; // drop counts of calls the host has not read yet / the sum of those it read
+    std::vector<batch_t *> in;
+    std::vector<wfb_batch_t> bi, bo;
+public:
+    FlatMapReplica(std::string n, const StageChain &pre, func_t f, uint32_t m, size_t maxk_): Basic_Replica(std::move(n)), max_out(m), maxk(maxk_ ? maxk_ : 1)
+    {
+        prm.filt.c = pre; prm.fm = f;
+    }
+    ~FlatMapReplica() override { if (eng) wfb_engine_destroy(eng); cudaFree(counts_d); cudaFreeHost(counts_h); }
+    int svc_init() override
+    {
+        Basic_Replica::svc_init();
+        wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
+        gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING));
+        return 0;
+    }
+    void *svc(void *msg) override
+    {
+        drain(msg, maxk, in);
+        std::vector<batch_t *> work;
+        for (auto *b : in) {
+            if (!b->isPunct()) { work.push_back(b); continue; }
+            flush_work(work);
+            Batch_GPU_t<result_t> *p = pool.get(1); // (a punctuation of the output type)
+            p->isPunctuation = true; p->size = 0; p->watermarks = b->watermarks;
+            recycleBatch(b);
+            this->ff_send_out(p);
+        }
+        flush_work(work);
+        return this->GO_ON;
+    }
+    void eosnotify(ssize_t id) override
+    {
+        read_drops(true);
+        if (dropped) wf_fatal("FlatMap_GPU [" + opName + "]: " + std::to_string(dropped) + " records pushed beyond withMaxOutputsPerTuple(" +
+                              std::to_string(max_out) + ") were dropped");
+        Basic_Replica::eosnotify(id);
+    }
+private:
+    // adds the drop counts of finished calls (all of them with `wait`); the words of a call are reused only after it was read
+    void read_drops(bool wait)
+    {
+        size_t i = 0;
+        for (; i < pending.size(); i++) {
+            if (wait || pending.size() - i > 8) { gpuErrChk(cudaEventSynchronize(pending[i].ev)); } // (events of the ring are re-recorded after 16 calls)
+            else if (cudaEventQuery(pending[i].ev) != cudaSuccess) { cudaGetLastError(); break; }
+            dropped += counts_h[pending[i].word];
+        }
+        pending.erase(pending.begin(), pending.begin() + static_cast<std::ptrdiff_t>(i));
+    }
+    void flush_work(std::vector<batch_t *> &work)
+    {
+        if (work.empty()) return;
+        wait_inputs(work);
+        read_drops(false);
+        const size_t k = work.size();
+        if (ring + k + 1 > RING) { read_drops(true); ring = 0; }
+        bi.resize(k); bo.resize(k);
+        std::vector<Batch_GPU_t<result_t> *> outs(k);
+        for (size_t i = 0; i < k; i++) {
+            batch_t *b = work[i];
+            b->getSize();
+            Batch_GPU_t<result_t> *o = pool.get(b->original_size * max_out);
+            o->watermarks = b->watermarks;
+            if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
+            bi[i] = wfb_batch_t{b->tuples_gpu, b->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
+            bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(o->original_size), 0};
+            outs[i] = o;
+        }
+        wfbErrChk(wfb_flatmap_batches(eng, reinterpret_cast<const wfb_functors_t *>(&prm), bi.data(), bo.data(), static_cast<uint32_t>(k), max_out,
+                                      counts_d + ring, stream));
+        gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
+        cudaEvent_t e = next_event();
+        gpuErrChk(cudaEventRecord(e, stream));
+        pending.push_back(Pending{ring + k, e});
+        for (size_t i = 0; i < k; i++) {
+            Batch_GPU_t<result_t> *o = outs[i];
+            o->size = work[i]->size * max_out; o->deferred = true; o->count_h = counts_h + ring + i; o->valid_after = e;
+            work[i]->reuse_after = e; recycleBatch(work[i]);
+            this->ff_send_out(o);
+        }
+        ring += k + 1;
+        work.clear();
+    }
+};
+
+template <class func_t>
+class FlatMap_GPU: public Basic_Operator {
+public:
+    using tuple_t = fn_arg_t<func_t, 0>;
+    using result_t = typename shipper_result<fn_arg_t<func_t, 1>>::type;
+    static constexpr op_type_t op_type = op_type_t::BASIC_GPU;
+    func_t func; uint32_t max_outputs;
+    FlatMap_GPU(func_t f, size_t p, std::string n, Routing_Mode_t r, uint32_t m): Basic_Operator(std::move(n), p, r, 1), func(f), max_outputs(m)
+    {
+        static_assert(std::is_trivially_copyable<func_t>::value, "GPU functors must be trivially copyable");
+    }
+    std::string getType() const override { return "FlatMap_GPU"; }
+    // a replica with the fused run `pre` of stateless operators over tuple_t in front (empty: none)
+    FlatMapReplica<tuple_t, result_t, func_t> *make_replica(const StageChain &pre) const
+    {
+        return new FlatMapReplica<tuple_t, result_t, func_t>(name, pre, func, max_outputs, parallelism > 1 ? 1 : WF_MAX_BATCHES_PER_CALL);
+    }
+};
+
 // Map_GPU / Filter_GPU, keyed-stateful (wf/map_gpu.hpp:104-310, wf/filter_gpu.hpp:120-399): func(tuple, state_of_key) in per-key arrival
 // order. The key -> state table is one wfb_kstate_t per operator, shared by its replicas behind a mutex (the reference's TBB map +
 // spinlock, wf/map_gpu.hpp:551-559); a replica hands the K batches it finds queued to one launch sequence.
@@ -1012,6 +1154,30 @@ public:
     }
 };
 
+template <class flatmap_func_gpu_t>
+class FlatMapGPU_Builder {
+    flatmap_func_gpu_t func; std::string name = "flatmap_gpu"; size_t parallelism = 1; Routing_Mode_t mode = Routing_Mode_t::FORWARD;
+    uint32_t max_outputs = 0;
+public:
+    explicit FlatMapGPU_Builder(flatmap_func_gpu_t f): func(f)
+    {
+        static_assert(std::tuple_size<typename fn_sig<flatmap_func_gpu_t>::args>::value == 2 &&
+                      std::is_same<fn_ret_t<flatmap_func_gpu_t>, void>::value &&
+                      std::is_same<std::tuple_element_t<1, typename fn_sig<flatmap_func_gpu_t>::args>,
+                                   Shipper_GPU<typename shipper_result<fn_arg_t<flatmap_func_gpu_t, 1>>::type> &>::value,
+                      "WindFlow Compilation Error - FlatMapGPU_Builder: __host__ __device__ void(const tuple_t &, Shipper_GPU<result_t> &)");
+    }
+    auto &withName(std::string n) { name = std::move(n); return *this; }
+    auto &withParallelism(size_t p) { parallelism = p; return *this; }
+    auto &withRebalancing() { mode = Routing_Mode_t::REBALANCING; return *this; }
+    auto &withMaxOutputsPerTuple(uint32_t m) { max_outputs = m; return *this; } // required: the output batches hold original_size * m records
+    auto build()
+    {
+        if (max_outputs == 0) wf_fatal("FlatMapGPU_Builder [" + name + "]: withMaxOutputsPerTuple(m >= 1) is required");
+        return FlatMap_GPU<flatmap_func_gpu_t>(func, parallelism, name, mode, max_outputs);
+    }
+};
+
 template <class reduce_func_gpu_t, class keyextr_func_gpu_t = NoKey<fn_arg_t<reduce_func_gpu_t, 0>>>
 class ReduceGPU_Builder {
     template <class A, class B> friend class ReduceGPU_Builder;
@@ -1138,6 +1304,21 @@ public:
     template <class F, class K> MultiPipe &chain(Map_GPU_KB<F, K> op) { return add_replicated(op); }
     template <class F, class K> MultiPipe &chain(Filter_GPU_KB<F, K> op) { return add_replicated(op); }
     template <class F, class K> MultiPipe &chain(Reduce_GPU<F, K> op) { return add_replicated(op); }
+    template <class F> MultiPipe &chain(FlatMap_GPU<F> op)
+    {
+        using T = typename FlatMap_GPU<F>::tuple_t;
+        attach(op);
+        StageChain pre{}; // a pending run over the same tuples with the same parallelism runs in the FlatMap's own pass
+        if (pending.n && pending_type == std::type_index(typeid(T)) && pending_par == op.getParallelism()) {
+            pre = pending;
+            pending = StageChain{}; pending_type = std::type_index(typeid(void)); materialize_pending = nullptr;
+        } else flush_pending();
+        auto *g = new ff::ff_group();
+        for (size_t i = 0; i < op.getParallelism(); i++) g->add(op.make_replica(pre), true);
+        add_stage(g);
+        tail_is_gpu = true;
+        return *this;
+    }
     template <class L, class C, class K> MultiPipe &chain(Ffat_Windows_GPU<L, C, K> op)
     {
         using T = typename Ffat_Windows_GPU<L, C, K>::tuple_t;

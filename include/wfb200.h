@@ -135,6 +135,17 @@ int wfb_map_filter(wfb_engine_t *e, const wfb_functors_t *f,
 int wfb_map_filter_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h,
                            uint32_t nbatches, uint32_t *n_out_dev, void *stream);
 
+/* ---- FlatMap_GPU: [map ->] [filter ->] flatmap(tuple, shipper) pushing 0..max_per_tuple result_t records per tuple ---------
+ * (wf/flatmap.hpp, wf/shipper.hpp). K queued batches in ONE launch: batch i expands into out[i] (capacity >= in[i].n *
+ * max_per_tuple result records; out[i].ts written when in[i].ts and out[i].ts are both non-null, every record with the timestamp
+ * of the tuple that pushed it), in input order and, per tuple, in push order; the results are identical to K single-batch calls.
+ * n_out_dev[i] = records of batch i, n_out_dev[nbatches] = pushes dropped because a tuple exceeded max_per_tuple (0 when none):
+ * n_out_dev holds nbatches + 1 words. max_per_tuple >= 1 and in[i].n * max_per_tuple < 2^31 (WFB_E_BADARG otherwise). The
+ * functor may run more than once per tuple: it must push the same records every time. `f` is the program's params_t, whose
+ * map / filter run in front as in wfb_map_filter_batches. Programs without a flatmap functor: WFB_E_UNSUPPORTED. */
+int wfb_flatmap_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
+                        uint32_t max_per_tuple, uint32_t *n_out_dev, void *stream);
+
 /* ---- Map_GPU / Filter_GPU, keyed-stateful ------------------------------------------------------------------------
  * func(tuple, state_of_key) applied in per-key arrival order; a key's state (the program's state_t, zero-initialised) lives
  * in the handle, which the replicas of one operator share (they see disjoint keys). K queued batches per call; arrival

@@ -54,6 +54,7 @@ SYMBOLS = {
     "wfb_filter_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_reduce_by_key_batches": (C.c_int, [vp, C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_map_filter_batches": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
+    "wfb_flatmap_batches": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, u32, vp, vp]),
     "wfb_reduce_by_key": (C.c_int, [vp, vp, vp, u32, vp, vp, vp, vp]),
     "wfb_reduce_all": (C.c_int, [vp, vp, vp, u32, vp, vp, vp]),
     "wfb_keyby_group": (C.c_int, [vp, vp, u32, vp, vp, vp, vp, vp]),

@@ -10,6 +10,8 @@
 //                                           (wf/filter_gpu.hpp:72-88, :555-570)
 //                              MODE_INGEST  [Map -> Filter ->] lift + key->slot for Ffat_Windows_GPU, or -> destination for
 //                                           wfb_shard_lift (wf/ffat_replica_gpu.hpp:94-121); chain-free ("sparse") on the bucket path
+//                              MODE_FLATMAP [Map -> Filter ->] FlatMap_GPU: 0..m result records per tuple, stable per batch
+//                                           (count pass, CTA scan, decoupled look-back, emit pass; wf/flatmap.hpp, wf/shipper.hpp)
 //   k_wide_tile_hist / k_wide_scatter / k_shard_scatter   one stable partition pass on a 10-bit digit (window path: 1024
 //                            buckets of slots; multi-GPU: destinations, with the records)
 //   k_ffat_update_buckets<P> one CTA per bucket: split by key, ordered pane folds, FlatFAT leaf + path update, fired
@@ -22,6 +24,7 @@
 #pragma once
 #include <type_traits>
 #include <cstdint>
+#include <cstring>
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include "wfb_ptx.cuh"
@@ -46,7 +49,7 @@ constexpr uint32_t OSW_TILE_POS = 4096; // positions per tile of the wide partit
 constexpr int STAGES = WFB_STAGES;    // TMA ring depth per CTA
 constexpr uint32_t FULL = 0xffffffffu;
 
-enum { MODE_MAP = 0, MODE_FILTER = 1, MODE_INGEST = 2 };
+enum { MODE_MAP = 0, MODE_FILTER = 1, MODE_INGEST = 2, MODE_FLATMAP = 3 };
 constexpr uint32_t MAX_SHARDS = 8;
 
 // decoupled look-back tile state: [63:34] epoch, [33:32] status, [31:0] value
@@ -155,12 +158,46 @@ struct TileArgs {
     uint32_t *shard_err;
     // MODE_INGEST: digit histograms of the slot sort that follows (RadixSorter ctl), accumulated per CTA in shared memory
     uint32_t *sort_ctl; uint32_t sort_passes, sort_shift, sort_dbits; // sort_dbits: digit width of a pass (8, or 10 for the wide pass)
+    uint32_t max_per_tuple;    // MODE_FLATMAP: records kept per tuple (m >= 1; the word fills the padding before `lifted`)
     // MODE_INGEST outputs (compacted over the whole segment, arrival order)
     unsigned char *lifted;     // result_t per surviving tuple
     uint32_t *slots;           // slot per surviving tuple
     uint32_t *batch_off;       // nbatches+1: compact offset of the first survivor of each batch; [nbatches]=total
-    uint32_t *n_total;         // == batch_off[nbatches]
+    uint32_t *n_total;         // == batch_off[nbatches]; MODE_FLATMAP: pushes dropped beyond max_per_tuple (added once per tile)
     FfatDev ff;
+};
+
+// The Shipper of a FlatMap functor: push(r) places record j (the j-th push of the tuple) at out[j] with the tuple's timestamp,
+// for j < m; later pushes are only counted. With out == nullptr it only counts (the count pass of MODE_FLATMAP: the functor is
+// inlined, so the stores vanish from that instance).
+template <class R>
+class Shipper {
+    unsigned char *out; uint64_t *ts_out; uint64_t ts; uint32_t m, n;
+public:
+    __host__ __device__ Shipper(unsigned char *out_, uint64_t *ts_out_, uint64_t ts_, uint32_t m_): out(out_), ts_out(ts_out_), ts(ts_), m(m_), n(0) {}
+    __host__ __device__ void push(const R &r)
+    {
+        if (out != nullptr && n < m) {
+            store(out + static_cast<size_t>(n) * sizeof(R), r);
+            if (ts_out != nullptr) ts_out[n] = ts;
+        }
+        n++;
+    }
+    __host__ __device__ uint32_t pushes() const { return n; } // every push, the dropped ones included
+private:
+    __host__ __device__ static void store(unsigned char *p, const R &r)
+    {
+        const unsigned char *src = reinterpret_cast<const unsigned char *>(&r);
+        if constexpr (sizeof(R) % 16 == 0) {
+            if ((reinterpret_cast<uintptr_t>(p) & 15u) == 0) { // (records of 16 * k bytes from a 16-byte aligned base: vector stores)
+#pragma unroll
+                for (uint32_t k = 0; k < sizeof(R) / 16; k++) { uint4 v; memcpy(&v, src + 16 * k, 16); reinterpret_cast<uint4 *>(p)[k] = v; }
+                return;
+            }
+        }
+#pragma unroll
+        for (uint32_t k = 0; k < sizeof(R) / 8; k++) { uint64_t v; memcpy(&v, src + 8 * k, 8); reinterpret_cast<uint64_t *>(p)[k] = v; }
+    }
 };
 
 // ------------------------------------------------------------------------------------------------------
@@ -409,7 +446,7 @@ struct TilePassSmem {
     using R = typename P::result_t;
     static constexpr uint32_t rec_bytes = (MODE == MODE_INGEST && sizeof(R) > sizeof(T)) ? sizeof(R) : sizeof(T);
     static constexpr uint32_t tile_bytes = (TILE * rec_bytes + 1023u) & ~1023u; // swizzled stages need 512-B alignment
-    static constexpr uint32_t aux_bytes = (MODE == MODE_INGEST) ? TILE * 4u : (MODE == MODE_FILTER ? TILE * 16u : 0u); // slots | ts in + ts out
+    static constexpr uint32_t aux_bytes = (MODE == MODE_INGEST) ? TILE * 4u : (MODE == MODE_FILTER ? TILE * 16u : (MODE == MODE_FLATMAP ? TILE * 8u : 0u)); // slots | ts in + ts out | ts in
     static constexpr uint32_t stage_bytes = tile_bytes + aux_bytes;
     static constexpr uint32_t hist_bytes = (MODE == MODE_INGEST) ? 4u * 256u * 4u : 0u; // up to 4 sort passes of 8 bits or one of 10 | two buffers of 1024 packed 16-bit per-wide-tile counts
     static constexpr uint32_t total = STAGES * stage_bytes + 1024 /*alignment slack*/ + 1024 /*barriers, meta, scan*/ + hist_bytes;
@@ -436,6 +473,34 @@ __device__ __forceinline__ void tma_store_2d(const void *tmap, int32_t c0, int32
 }
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(TILE) : "memory"); }
 
+// decoupled look-back of tile t > chain_begin (one whole warp): adds the sum of the published counts of tiles [chain_begin, t) to
+// excl, read back from the nearest PREFIX (the chain's start acts as a PREFIX of 0)
+__device__ __forceinline__ void lookback_exclusive(const TileArgs &a, uint32_t t, uint32_t chain_begin, uint32_t lane, uint32_t &excl)
+{
+    int64_t idx = static_cast<int64_t>(t) - 1;
+    while (true) {
+        const int64_t my = idx - lane;
+        uint64_t w = pack_state(a.epoch, ST_PREFIX, 0); // virtual terminator below the chain start
+        bool valid;
+        do {
+            valid = true;
+            if (my >= static_cast<int64_t>(chain_begin)) {
+                w = ld_relaxed_u64(&a.tile_state[my]);
+                valid = ((w >> 34) == (a.epoch & 0x3fffffffu)) && (((w >> 32) & 3u) != 0);
+            }
+        } while (!__all_sync(FULL, valid));
+        const uint32_t status = static_cast<uint32_t>(w >> 32) & 3u;
+        const uint32_t pmask = __ballot_sync(FULL, status == ST_PREFIX);
+        const uint32_t firstp = pmask ? (__ffs(pmask) - 1) : 32;
+        uint32_t v = (lane <= firstp) ? static_cast<uint32_t>(w) : 0u;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+        excl += v;
+        if (pmask) break;
+        idx -= 32;
+    }
+}
+
 template <class P, int MODE>
 __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant__ CUtensorMap tmap, const TileArgs a,
                                                           const __grid_constant__ typename P::params_t prm)
@@ -456,6 +521,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
     uint64_t *empty = staged + STAGES;                           // STAGES  epilogue -> producer
     StageMeta *meta = reinterpret_cast<StageMeta *>(empty + STAGES);  // STAGES
     uint32_t *warp_tot = reinterpret_cast<uint32_t *>(meta + STAGES); // 2 x 8 warp totals (double-buffered by iteration parity)
+    uint32_t *fm_words = warp_tot + 2 * (TILE / 32);                  // MODE_FLATMAP: 2 x 8 warp drop counts, then 2 tile bases
     uint32_t *s_hist = reinterpret_cast<uint32_t *>(ctl + 1024);      // MODE_INGEST: [pass][1 << sort_dbits] digit counts of this CTA (1024 words)
 
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -504,7 +570,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
                 if (CAN_SWZ && a.use_tmap && cnt == TILE && (off & 63u) == 0 && (off >> 6) < 0x7fffff00ull) flags = TF_SWZ;
                 else if (!bulk_ok(src, cnt * TB)) flags = TF_FALLBACK;
                 if (!(flags & TF_FALLBACK)) tx += cnt * TB;
-                const uint64_t *tsp = (MODE == MODE_FILTER && b.ts != nullptr) ? b.ts + first : nullptr;
+                const uint64_t *tsp = ((MODE == MODE_FILTER || MODE == MODE_FLATMAP) && b.ts != nullptr) ? b.ts + first : nullptr;
                 if (tsp != nullptr && bulk_ok(tsp, cnt * 8u)) { flags |= TF_TS_SMEM; tx += cnt * 8u; }
                 if (t_next == t_end) flags |= TF_WIDE_LAST;
                 m.tile = t; m.batch = bi; m.first = first; m.cnt = cnt; m.flags = flags; m.wide = claim;
@@ -561,7 +627,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
                         for (uint32_t jj = 0; jj < 4; jj++) o[jj] = p[jj ^ x];
                     } else TileIO<T>::load(buf, ctid, tup);
                 } else TileIO<T>::load(buf, ctid, tup);
-                if constexpr (MODE == MODE_FILTER) {
+                if constexpr (MODE == MODE_FILTER || MODE == MODE_FLATMAP) {
                     if (b.ts != nullptr)
                         ts = (m.flags & TF_TS_SMEM) ? reinterpret_cast<const uint64_t *>(stage_aux(s))[ctid] : b.ts[m.first + ctid];
                 }
@@ -610,6 +676,48 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
                     } else TileIO<T>::store(buf, ctid, tup);
                 }
                 if (ctid == 0) meta[s].count = cnt;
+            } else if constexpr (MODE == MODE_FLATMAP) {
+                // ---- count pass: the functor with a counting shipper, capped at m ------------------------------------
+                const uint32_t mpt = a.max_per_tuple;
+                uint32_t cnt_t = 0;
+                if (keep) { Shipper<R> sh(nullptr, nullptr, 0, mpt); P::flatmap(tup, sh, prm); cnt_t = sh.pushes(); }
+                const uint32_t dropped = cnt_t > mpt ? cnt_t - mpt : 0u;
+                cnt_t -= dropped;
+                // ---- CTA scan: warp inclusive scan + warp totals (double-buffered by iteration parity) ---------------
+                uint32_t incl = cnt_t;
+#pragma unroll
+                for (uint32_t o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if (lane >= o) incl += v; }
+                uint32_t *wt = warp_tot + (it & 1u) * (TILE / 32);
+                uint32_t *wd = fm_words + (it & 1u) * (TILE / 32);
+                const uint32_t wdrop = __reduce_add_sync(FULL, dropped);
+                if (lane == 31) { wt[cwarp] = incl; wd[cwarp] = wdrop; }
+                consumer_bar(); // warp totals visible; every consumer has read its tuple and timestamp
+                uint32_t wbase = 0, total = 0, tdrop = 0;
+#pragma unroll
+                for (uint32_t w = 0; w < TILE / 32; w++) { const uint32_t c = wt[w]; if (w < cwarp) wbase += c; total += c; tdrop += wd[w]; }
+                // ---- the tile's base in its batch's output: consumer warp 0 publishes the aggregate and looks back ----
+                uint32_t *tile_base = fm_words + 2 * (TILE / 32) + (it & 1u);
+                if (cwarp == 0) {
+                    if (lane == 0) {
+                        meta[s].count = total;
+                        if (m.tile != b.tile_begin) st_relaxed_u64(&a.tile_state[m.tile], pack_state(a.epoch, ST_AGG, total));
+                    }
+                    uint32_t excl = 0;
+                    if (m.tile != b.tile_begin) lookback_exclusive(a, m.tile, b.tile_begin, lane, excl);
+                    if (lane == 0) {
+                        st_relaxed_u64(&a.tile_state[m.tile], pack_state(a.epoch, ST_PREFIX, excl + total));
+                        if (m.tile == b.tile_begin + (b.n + TILE - 1) / TILE - 1 && b.n_out != nullptr) *b.n_out = excl + total;
+                        if (tdrop) atomicAdd(a.n_total, tdrop); // (one atomic per tile that dropped pushes)
+                        *tile_base = excl;
+                    }
+                }
+                consumer_bar(); // tile base visible
+                // ---- emit pass: the functor again, record j of this tuple at batch base + tile excl + thread excl + j ---
+                if (cnt_t) {
+                    const uint32_t pos = *tile_base + wbase + incl - cnt_t;
+                    Shipper<R> sh(b.out + static_cast<size_t>(pos) * RB, b.ts_out != nullptr ? b.ts_out + pos : nullptr, ts, mpt);
+                    P::flatmap(tup, sh, prm);
+                }
             } else {
                 // ---- stable local offsets: ballot + warp totals (double-buffered), ONE named barrier ------------
                 const uint32_t bal = __ballot_sync(FULL, keep);
@@ -658,6 +766,11 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
             mbar_wait(&staged[s], par);
             const StageMeta m = meta[s];
             if (m.tile == TILE_SENTINEL) break;
+            if constexpr (MODE == MODE_FLATMAP) { // the consumers placed the records themselves: only release the stage
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);
+                continue;
+            }
             DevBatch b;
             if (a.batches == nullptr) b = a.one; else b = a.batches[m.batch];
             const uint32_t t = m.tile, tile_count = m.count;
@@ -667,30 +780,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
                 if (lane == 0 && t == 0 && a.ff.n_trig != nullptr) { *a.ff.n_trig = 0; *a.ff.n_heavy = 0; } // per-segment lists filled by the update kernels
             } else if constexpr (MODE != MODE_MAP) {
                 const uint32_t chain_begin = (MODE == MODE_FILTER) ? b.tile_begin : 0u;
-                if (t != chain_begin) {
-                    int64_t idx = static_cast<int64_t>(t) - 1;
-                    while (true) {
-                        const int64_t my = idx - lane;
-                        uint64_t w = pack_state(a.epoch, ST_PREFIX, 0); // virtual terminator below the chain start
-                        bool valid;
-                        do {
-                            valid = true;
-                            if (my >= static_cast<int64_t>(chain_begin)) {
-                                w = ld_relaxed_u64(&a.tile_state[my]);
-                                valid = ((w >> 34) == (a.epoch & 0x3fffffffu)) && (((w >> 32) & 3u) != 0);
-                            }
-                        } while (!__all_sync(FULL, valid));
-                        const uint32_t status = static_cast<uint32_t>(w >> 32) & 3u;
-                        const uint32_t pmask = __ballot_sync(FULL, status == ST_PREFIX);
-                        const uint32_t firstp = pmask ? (__ffs(pmask) - 1) : 32;
-                        uint32_t v = (lane <= firstp) ? static_cast<uint32_t>(w) : 0u;
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-                        excl += v;
-                        if (pmask) break;
-                        idx -= 32;
-                    }
-                }
+                if (t != chain_begin) lookback_exclusive(a, t, chain_begin, lane, excl);
                 if (lane == 0) {
                     st_relaxed_u64(&a.tile_state[t], pack_state(a.epoch, ST_PREFIX, excl + tile_count));
                     if constexpr (MODE == MODE_FILTER) {

@@ -118,6 +118,8 @@ struct ProgramOps {
     // Reduce_GPU over keys that are not integers: the order words of every element (k_key_order_words; batches null: `tuples` is the batch)
     int (*key_order_words)(const DevBatch *batches, const uint32_t *boff, uint32_t nb, const unsigned char *tuples, uint32_t total, uint64_t *lo,
                            uint64_t *hi, cudaStream_t s, const void *params);
+    // FlatMap_GPU: the tile pass in MODE_FLATMAP (null when the program has no flatmap)
+    int (*flatmap)(TileArgs &a, const void *params, uint32_t want_grid, cudaStream_t s, uint32_t *grid_used, uint64_t span_begin, uint64_t span_end);
 };
 
 // P::passthrough (optional): map is a no-op and lift the identity (tuple_t == result_t)
@@ -285,6 +287,16 @@ int flag_scatter_dispatch(const unsigned char *keep, const uint32_t *tile_base, 
 }
 template <class P> constexpr uint32_t program_state_bytes() { if constexpr (program_has_state<P>::value) return sizeof(typename P::state_t); else return 0; }
 
+// P::flatmap(const tuple_t &, Shipper<result_t> &, const params_t &) (optional: FlatMap_GPU)
+template <class P, class = void> struct program_has_flatmap : std::false_type {};
+template <class P> struct program_has_flatmap<P, std::void_t<decltype(P::flatmap(std::declval<const typename P::tuple_t &>(),
+    std::declval<Shipper<typename P::result_t> &>(), std::declval<const typename P::params_t &>()))>> : std::true_type {};
+template <class P>
+int flatmap_dispatch(TileArgs &a, const void *params, uint32_t want_grid, cudaStream_t s, uint32_t *grid_used, uint64_t span_begin, uint64_t span_end)
+{
+    return launch_tile_pass<P, MODE_FLATMAP>(a, params, want_grid, s, grid_used, span_begin, span_end);
+}
+
 template <class P>
 int tb_lift_dispatch(const unsigned char *tuples, const uint64_t *ts, uint32_t n, const FfatDev &ff, const TbDev &tb, uint64_t first_incomplete,
                      unsigned char *lifted, uint64_t *ckeys, cudaStream_t s, const void *params)
@@ -437,6 +449,7 @@ ProgramOps make_ops()
     o.key_bytes = 8u * key_codec<P>::words; o.key_kind = key_codec<P>::kind; o.key_size = sizeof(typename P::key_t);
     o.key_order_words = &key_order_words_dispatch<P>;
     if constexpr (program_is_lifted<P>::value) o.lifted_ops = nullptr; else o.lifted_ops = &lifted_ops_of<P>;
+    if constexpr (program_has_flatmap<P>::value) o.flatmap = &flatmap_dispatch<P>; else o.flatmap = nullptr;
     return o;
 }
 

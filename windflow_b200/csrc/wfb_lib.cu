@@ -671,6 +671,45 @@ int wfb_map_filter_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_b
     return 0;
 }
 
+int wfb_flatmap_batches(wfb_engine_t *e, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
+                        uint32_t max_per_tuple, uint32_t *n_out_dev, void *stream)
+{
+    if (!e || !f || !n_out_dev || max_per_tuple == 0 || (nbatches && (!in_h || !out_h))) return WFB_E_BADARG;
+    if (!e->ops->flatmap) return WFB_E_UNSUPPORTED;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    int rc = e->ts.enter(s); if (rc) return rc;
+    std::vector<DevBatch> hb; hb.reserve(nbatches);
+    uint32_t tiles = 0; uint64_t span_begin = ~0ull, span_end = 0;
+    for (uint32_t i = 0; i < nbatches; i++) {
+        if (in_h[i].n == 0) continue;
+        if (!in_h[i].tuples || !out_h[i].tuples) return WFB_E_BADARG;
+        if (static_cast<uint64_t>(in_h[i].n) * max_per_tuple >= (1ull << 31)) return WFB_E_BADARG; // (positions of a batch are 32-bit)
+        DevBatch b; std::memset(&b, 0, sizeof(b));
+        b.tuples = static_cast<const unsigned char *>(in_h[i].tuples); b.ts = in_h[i].ts;
+        b.out = static_cast<unsigned char *>(const_cast<void *>(out_h[i].tuples));
+        b.ts_out = in_h[i].ts ? const_cast<uint64_t *>(out_h[i].ts) : nullptr;
+        b.n_out = n_out_dev + i; b.n = in_h[i].n; b.tile_begin = tiles;
+        tiles += tiles_of(b.n);
+        const uint64_t p0 = reinterpret_cast<uint64_t>(b.tuples);
+        span_begin = std::min(span_begin, p0); span_end = std::max(span_end, p0 + static_cast<uint64_t>(b.n) * e->ops->tuple_bytes);
+        hb.push_back(b);
+    }
+    CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t) * (nbatches + 1), s)); // empty batches keep 0; the drop counter starts at 0
+    if (hb.empty()) return 0;
+    rc = e->ts.ensure_tiles(tiles); if (rc) return rc;
+    rc = e->ts.ensure_batches(static_cast<uint32_t>(hb.size())); if (rc) return rc;
+    { int rc_ = e->ts.stage.h2d(e->ts.d_batches, hb.data(), sizeof(DevBatch) * hb.size(), s); if (rc_) return rc_; }
+    TileArgs a; std::memset(&a, 0, sizeof(a));
+    a.batches = e->ts.d_batches; a.nbatches = static_cast<uint32_t>(hb.size()); a.num_tiles = tiles; a.l2_hints = 1;
+    a.max_per_tuple = max_per_tuple; a.n_total = n_out_dev + nbatches;
+    e->ts.next_launch(a);
+    uint32_t grid = 0;
+    rc = e->ops->flatmap(a, f, tiles, s, &grid, span_begin, span_end); if (rc) return rc;
+    e->ts.launched(tiles, grid);
+    e->launches++;
+    return 0;
+}
+
 int wfb_engine_set_key_bits(wfb_engine_t *e, uint32_t bits)
 {
     if (!e || bits == 0 || bits > 64 || e->ops->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG;

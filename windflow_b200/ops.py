@@ -143,6 +143,13 @@ class Engine:
                                             _stream_ptr(stream)), "wfb_map_filter_batches")
         return outs, n_out
 
+    def flatmap_batches(self, batches, f, outs, n_out, max_per_tuple, stream=None):
+        """[Map_GPU ->] [Filter_GPU ->] FlatMap_GPU over K queued batches in one launch: batch i expands into outs[i] (room for
+        batches[i].n * max_per_tuple result records), n_out[i] records; n_out[K] = pushes dropped beyond max_per_tuple per tuple."""
+        check(self.L.wfb_flatmap_batches(self.h, C.byref(f), _cbatches(batches), _cbatches(outs), len(batches), max_per_tuple, _ptr(n_out),
+                                         _stream_ptr(stream)), "wfb_flatmap_batches")
+        return outs, n_out
+
     def reduce_by_key(self, batch, out=None, n_out=None, stream=None):
         if out is None:
             out = DeviceBatch(torch.empty_like(batch.tuples), torch.empty_like(batch.ts), batch.n, batch.watermark)
