@@ -1128,6 +1128,8 @@ __global__ void __launch_bounds__(256) k_slots_inplace(const TileArgs a, const t
 constexpr uint32_t OSW_BITS = 10, OSW_DIGITS = 1u << OSW_BITS;
 constexpr uint32_t OSW_THREADS = 256, OSW_ITEMS = 16, OSW_TILE = OSW_THREADS * OSW_ITEMS; // 4096 elements per tile
 static_assert(OSW_TILE == OSW_TILE_POS, "the tile pass files its digit counts per wide tile");
+// wide tiles per CTA of k_wide_scatter_ranked (and per offset row T of k_wide_tile_bases): a chunk is a whole number of groups
+constexpr uint32_t OSR_GROUP = 4, OSR_GROUP_POS = OSR_GROUP * OSW_TILE;
 
 template <class K>
 __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_hist(const K *__restrict__ keys, const uint32_t *__restrict__ n_ptr, uint32_t n_host,
@@ -1184,15 +1186,15 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_chunk_sums16(const 
     }
 }
 
-// The first output position of every (wide tile, digit), in one launch, from the 16-bit rows the tile pass filed. CTA c adds the rows
-// of chunk c and files, for every tile of the chunk, the sum of the chunk's earlier rows (T[tile][digit], 32-bit). The last CTA to
+// The first output position of every (group of 2^gshift wide tiles, digit), in one launch, from the 16-bit rows the tile pass filed.
+// CTA c adds the rows of chunk c and files, for every group of the chunk, the sum of the chunk's earlier rows (T[group][digit], 32-bit). The last CTA to
 // finish turns the chunk sums C[chunk][digit] into the first output position of every (chunk, digit) -- exclusive scan over the digits
-// of the totals + exclusive scan over the chunks, in place -- and sets ctl_counts[digit] = total of the digit. A tile's first output
-// position of digit d is then C[chunk][d] + T[tile][d]: two rows per scatter CTA, whatever the tile's place in its chunk.
+// of the totals + exclusive scan over the chunks, in place -- and sets ctl_counts[digit] = total of the digit. A group's first output
+// position of digit d is then C[chunk][d] + T[group][d]: two rows per scatter CTA, whatever the group's place in its chunk.
 // `done` (one word, zero between launches: the last CTA clears it) counts the finished chunks.
 static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const uint16_t *__restrict__ H, uint32_t tiles, uint32_t chunk_shift, uint32_t chunks,
                                                                         uint32_t *__restrict__ C, uint32_t *__restrict__ T, uint32_t *__restrict__ ctl_counts,
-                                                                        uint32_t *__restrict__ done)
+                                                                        uint32_t *__restrict__ done, uint32_t gshift)
 {
     static_assert(OSW_THREADS * 4 == OSW_DIGITS, "four digits per thread");
     constexpr uint32_t NW = OSW_THREADS / 32;
@@ -1206,7 +1208,7 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const ui
 #pragma unroll 8
     for (uint32_t t = t0; t < t1; t++) {
         const ushort4 v = row[static_cast<size_t>(t) * (OSW_DIGITS / 4)];
-        trow[static_cast<size_t>(t) * (OSW_DIGITS / 4)] = acc;
+        if ((t & ((1u << gshift) - 1u)) == 0) trow[static_cast<size_t>(t >> gshift) * (OSW_DIGITS / 4)] = acc;
         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
     }
     uint4 *C4 = reinterpret_cast<uint4 *>(C);
@@ -1242,7 +1244,118 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const ui
 }
 
 // The scatter of the wide partition when the tile pass packed a rank with every slot (TileArgs::pack_rank): word = slot | rank << 16,
-// rank = any numbering 0 .. count-1 of the survivors of one (wide tile, digit) cell. One CTA per wide tile, everything on chip:
+// rank = any numbering 0 .. count-1 of the survivors of one (wide tile, digit) cell. One CTA per GROUP of OSR_GROUP consecutive wide
+// tiles, everything on chip:
+//   1. the group's rows; the group's cells laid out back to back in shared memory (exclusive scan of the group's digit counts). The
+//      cell of (group, digit) is the group's (wide tile, digit) cells -- its "parts" -- in tile order, which is arrival order, and it is
+//      where they sit in the output as well,
+//   2. every item files its position within the group (and its slot, at the same index) at its part's start + rank -- no ranking
+//      rounds, no per-warp counters,
+//   3. a sweep over the laid-out cells, consecutive threads on consecutive entries of a cell: ARRIVAL order inside each part (the count
+//      windows need every key's items in stream order, and two items of one key may share a part; every entry of an earlier part is
+//      earlier, every entry of a later part later) -- an entry's place in its part is the number of the part's entries with a smaller
+//      position, two 16-bit compares per 4-byte load as in k_wide_scatter_ranked_tile -- and one write of (slot, position) to the final
+//      place: first output position of the group's cell (C[chunk] + T[group] of k_wide_tile_bases) + the earlier parts + that number.
+// Why groups: a (wide tile, digit) cell holds about 2 items at the bench step (4096 positions, half of them survivors, 1024 digits), so
+// with one wide tile per CTA a warp's store touched about 16 separate 32-byte sectors per array; a group cell of 4 tiles is about 8
+// items, whole sectors (tools/micro/bucket_store.cu replays both patterns). Used when there are enough groups to give every SM one
+// (osr_group in wfb_lib.cu) and no records travel; otherwise k_wide_scatter_ranked_tile below (one wide tile per CTA) runs.
+// Output: keys_out[i] = slot, vals_out[i] = arrival position, stable by (digit, position) -- what k_wide_scatter produces.
+// OSR_SMEM = 74 KB of dynamic shared memory: 3 resident CTAs per SM. Positions within a group are < 2^14, slots < 2^16.
+constexpr uint32_t OSR_SMEM = OSR_GROUP_POS * 2u * 2u + OSW_DIGITS * 8u + OSW_DIGITS * 2u;
+static_assert(OSR_GROUP == 4 && OSR_GROUP_POS <= 0x8000u, "one ushort4 of part sizes per digit; 16-bit packed position compare");
+static __global__ void __launch_bounds__(OSW_THREADS, 3) k_wide_scatter_ranked(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
+                                                                            uint32_t *__restrict__ vals_out, uint32_t n, uint32_t shift, uint32_t chunk_shift,
+                                                                            uint32_t tiles, const uint16_t *__restrict__ H, const uint32_t *__restrict__ Cx,
+                                                                            const uint32_t *__restrict__ T)
+{
+    constexpr uint32_t NW = OSW_THREADS / 32;
+    static_assert(OSW_THREADS * 4 == OSW_DIGITS, "four digits per thread");
+    extern __shared__ __align__(16) unsigned char osr_smem_buf[];
+    uint16_t *lpos = reinterpret_cast<uint16_t *>(osr_smem_buf);        // [OSR_GROUP_POS] position within the group, cells back to back
+    uint16_t *lslot = lpos + OSR_GROUP_POS;                               // [OSR_GROUP_POS] the slot of the same entry
+    ushort4 *part = reinterpret_cast<ushort4 *>(lslot + OSR_GROUP_POS);  // [OSW_DIGITS] sizes of the digit's parts, tile 0 .. 3
+    uint16_t *cell = reinterpret_cast<uint16_t *>(part + OSW_DIGITS);     // [OSW_DIGITS] start of the digit's cell in lpos / lslot
+    __shared__ uint32_t wsum[NW];
+    __shared__ uint32_t s_total;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, group = blockIdx.x, tile0 = group * OSR_GROUP;
+    const uint32_t start = tile0 * OSW_TILE;
+    if (start >= n) return;
+    {
+        ushort4 h[OSR_GROUP]; // the group's rows, digits 4 tid .. 4 tid + 3 (a group past the last tile has empty rows)
+#pragma unroll
+        for (uint32_t k = 0; k < OSR_GROUP; k++)
+            h[k] = tile0 + k < tiles ? reinterpret_cast<const ushort4 *>(H)[static_cast<size_t>(tile0 + k) * (OSW_DIGITS / 4) + tid] : make_ushort4(0, 0, 0, 0);
+        part[4 * tid + 0] = make_ushort4(h[0].x, h[1].x, h[2].x, h[3].x);
+        part[4 * tid + 1] = make_ushort4(h[0].y, h[1].y, h[2].y, h[3].y);
+        part[4 * tid + 2] = make_ushort4(h[0].z, h[1].z, h[2].z, h[3].z);
+        part[4 * tid + 3] = make_ushort4(h[0].w, h[1].w, h[2].w, h[3].w);
+        uint32_t c0 = 0, c1 = 0, c2 = 0, c3 = 0;
+#pragma unroll
+        for (uint32_t k = 0; k < OSR_GROUP; k++) { c0 += h[k].x; c1 += h[k].y; c2 += h[k].z; c3 += h[k].w; }
+        const uint32_t sum = c0 + c1 + c2 + c3;
+        uint32_t incl = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if (lane >= static_cast<uint32_t>(o)) incl += v; }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        uint32_t base = incl - sum;
+#pragma unroll
+        for (uint32_t q = 0; q < NW; q++) if (q < warp) base += wsum[q];
+        if (tid == OSW_THREADS - 1) s_total = base + sum;
+        reinterpret_cast<ushort4 *>(cell)[tid] = make_ushort4(static_cast<uint16_t>(base), static_cast<uint16_t>(base + c0), static_cast<uint16_t>(base + c0 + c1),
+                                                               static_cast<uint16_t>(base + c0 + c1 + c2));
+    }
+    __syncthreads();
+    // parts of tile k of digit d start at cell[d] + the sizes of the digit's parts of tiles 0 .. k-1
+    auto part_start = [&](uint32_t d, uint32_t k, uint32_t *size) {
+        const ushort4 p = part[d];
+        *size = k == 0 ? p.x : k == 1 ? p.y : k == 2 ? p.z : p.w;
+        return (k > 0 ? p.x : 0u) + (k > 1 ? p.y : 0u) + (k > 2 ? p.z : 0u);
+    };
+#pragma unroll 1
+    for (uint32_t k = 0; k < OSR_GROUP; k++) {
+        uint32_t w[OSW_ITEMS];
+#pragma unroll
+        for (uint32_t r = 0; r < OSW_ITEMS; r++) {
+            const uint32_t idx = start + k * OSW_TILE + r * OSW_THREADS + tid;
+            w[r] = idx < n ? packed[idx] : INVALID_SLOT;
+        }
+#pragma unroll
+        for (uint32_t r = 0; r < OSW_ITEMS; r++)
+            if (w[r] != INVALID_SLOT) {
+                const uint32_t slot = w[r] & 0xffffu, d = (slot >> shift) & (OSW_DIGITS - 1u);
+                uint32_t size;
+                const uint32_t i = cell[d] + part_start(d, k, &size) + (w[r] >> 16);
+                lpos[i] = static_cast<uint16_t>(k * OSW_TILE + r * OSW_THREADS + tid);
+                lslot[i] = static_cast<uint16_t>(slot);
+            }
+    }
+    __syncthreads();
+    const uint32_t total = s_total;
+    const uint32_t *cbase = Cx + static_cast<size_t>(tile0 >> chunk_shift) * OSW_DIGITS, *tbase = T + static_cast<size_t>(group) * OSW_DIGITS;
+#pragma unroll 2
+    for (uint32_t e = tid; e < total; e += OSW_THREADS) {
+        const uint32_t mine = lpos[e], slot = lslot[e], d = (slot >> shift) & (OSW_DIGITS - 1u);
+        uint32_t size;
+        const uint32_t before = part_start(d, mine / OSW_TILE, &size);
+        uint32_t j = cell[d] + before;
+        const uint32_t end = j + size;
+        // entries of the part below `mine`: an odd head and tail one by one, the rest two per load -- per 16-bit half, bit 15 of
+        // (0x8000 + mine - 1 - entry) says entry < mine (positions are < 2^14, so the halves never borrow from each other)
+        uint32_t less = 0;
+        if (j & 1u) { less += lpos[j] < mine ? 1u : 0u; j++; }
+        const uint32_t mm = (mine | (mine << 16)) + 0x7fff7fffu;
+        for (; j + 1 < end; j += 2) less += __popc((mm - *reinterpret_cast<const uint32_t *>(lpos + j)) & 0x80008000u);
+        if (j < end) less += lpos[j] < mine ? 1u : 0u;
+        const uint32_t dst = __ldg(cbase + d) + __ldg(tbase + d) + before + less;
+        keys_out[dst] = slot;
+        vals_out[dst] = start + mine;
+    }
+}
+
+// The same scatter with one CTA per wide tile (k_wide_tile_bases files one offset row per tile, gshift = 0): calls with fewer wide
+// tiles than 4 per SM and the payload variants (their L2 prefetch of a group's records would overrun the L2). Everything on chip:
 //   1. the tile's words to shared memory; first output position of every digit for this tile (C[chunk] + T[tile] of k_wide_tile_bases)
 //      and the tile's own cells laid out back to back in shared memory (exclusive scan of the tile's digit counts),
 //   2. every item files its position within the tile at cell start + rank -- no ranking rounds, no per-warp counters,
@@ -1260,7 +1373,7 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const ui
 #define WFB_OSR_MINBLOCKS 6
 #endif
 template <int RBYTES>
-static __global__ void __launch_bounds__(OSW_THREADS, WFB_OSR_MINBLOCKS) k_wide_scatter_ranked(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
+static __global__ void __launch_bounds__(OSW_THREADS, WFB_OSR_MINBLOCKS) k_wide_scatter_ranked_tile(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
                                                                             uint32_t *__restrict__ vals_out, uint32_t n, uint32_t shift, uint32_t chunk_shift,
                                                                             const uint16_t *__restrict__ H, const uint32_t *__restrict__ Cx, const uint32_t *__restrict__ T,
                                                                             const unsigned char *__restrict__ payload_in, unsigned char *__restrict__ payload_out)

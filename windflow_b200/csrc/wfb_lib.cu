@@ -8,6 +8,7 @@
 #include <mutex>
 #include <vector>
 #include <algorithm>
+#include <atomic>
 #include <new>
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -110,6 +111,24 @@ struct TileScratch {
 
 inline uint32_t tiles_of(uint32_t n) { return (n + TILE - 1) / TILE; }
 
+// wide tiles per CTA of k_wide_scatter_ranked (and per row T of k_wide_tile_bases): OSR_GROUP when no records travel and every SM gets a
+// group, else 1
+inline uint32_t osr_group(uint32_t tiles, bool payload) { return !payload && tiles >= OSR_GROUP * static_cast<uint32_t>(g_num_sms) ? OSR_GROUP : 1u; }
+
+// k_wide_scatter_ranked takes more than 48 KB of dynamic shared memory: opt in once per device (bit = device ordinal)
+cudaError_t osr_smem_attr()
+{
+    static std::atomic<uint64_t> done{0};
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    const uint64_t bit = 1ull << (dev & 63);
+    if (done.load(std::memory_order_relaxed) & bit) return cudaSuccess;
+    e = cudaFuncSetAttribute(k_wide_scatter_ranked, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(OSR_SMEM));
+    if (e == cudaSuccess) done.fetch_or(bit, std::memory_order_relaxed);
+    return e;
+}
+
 // scratch + launcher of the onesweep radix sort (one per engine / window handle)
 struct RadixSorter {
     Scratch<uint32_t> ctl;          // [passes][256] histograms + [passes] tickets
@@ -136,7 +155,7 @@ struct RadixSorter {
     // ONE stable partition pass of (kin[i], i) on the digit (key >> shift) & 1023 into (kout, vout): per-tile counts, then
     // the scatter (no chained scan). *counts = the 1024 digit counts (ready_ctl if the producer of the keys made them).
     Scratch<uint16_t> wideH; Scratch<uint32_t> wideC;
-    Scratch<uint32_t> wideT;    // [tiles][1024]: sum of the earlier rows of the tile's chunk (k_wide_tile_bases)
+    Scratch<uint32_t> wideT;    // [groups of osr_group() tiles][1024]: sum of the earlier rows of the group's chunk (k_wide_tile_bases)
     Scratch<uint32_t> wideDone; // finished chunks of k_wide_tile_bases (zero between launches)
     // tiles of the wide pass over `cap` positions and their chunks. prefix = false: about sqrt(tiles) chunks of >= 16 tiles, every
     // scatter CTA sums the rows of the earlier chunks itself; true (rows filed by the tile pass): chunks of 32 tiles; one kernel
@@ -156,7 +175,7 @@ struct RadixSorter {
     {
         const size_t rows = static_cast<size_t>(OSW_DIGITS) * tiles, chunk_rows = static_cast<size_t>(OSW_DIGITS) * chunks;
         CK(wideH.ensure(rows, waits, rows));
-        CK(wideT.ensure(rows, waits, rows));
+        CK(wideT.ensure(rows, waits, rows)); // (one row per group: as many as tiles at a group of 1)
         CK(wideC.ensure(chunk_rows, waits, chunk_rows));
         return 0;
     }
@@ -198,7 +217,8 @@ struct RadixSorter {
         if (!ready_ctl) { int rc = prepare_wide(c, s); if (rc) return rc; }
         if (ranked) { // first output position of every (chunk, digit) and (tile, digit) + digit counts
             CK(wideDone.ensure_zeroed(1, s));
-            k_wide_tile_bases<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, chunks, wideC, wideT, c, wideDone);
+            k_wide_tile_bases<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, chunks, wideC, wideT, c, wideDone,
+                                                             osr_group(tiles, payload_in != nullptr) == OSR_GROUP ? 2u : 0u); // (log2 OSR_GROUP)
         } else if (ready_ctl) { // a few bins (destinations): chunk sums + the global counts
             k_wide_chunk_sums16<<<chunks, OSW_THREADS, 0, s>>>(rows, tiles, chunk_shift, wideC, c);
         } else {
@@ -224,14 +244,19 @@ struct RadixSorter {
         }
         if (ranked) {
             if (sizeof(K) != 4 || !kout || (payload_in ? !payload_out || region_stride : !vout)) return WFB_E_UNSUPPORTED;
-#define WFB_WSR(RB_) k_wide_scatter_ranked<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, \
-                                                                             chunk_shift, rows, wideC, wideT, payload_in, payload_out)
-            if (!payload_in) WFB_WSR(0);
+            if (!payload_in && osr_group(tiles, false) == OSR_GROUP) {
+                CK(osr_smem_attr());
+                k_wide_scatter_ranked<<<(tiles + OSR_GROUP - 1) / OSR_GROUP, OSW_THREADS, OSR_SMEM, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout),
+                                                                                                       vout, n_host, shift, chunk_shift, tiles, rows, wideC, wideT);
+            }
+#define WFB_WSRT(RB_) k_wide_scatter_ranked_tile<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, \
+                                                                                  chunk_shift, rows, wideC, wideT, payload_in, payload_out)
+            else if (!payload_in) WFB_WSRT(0);
             else switch (payload_bytes) { // the records travel with their slots (bucketed exchange)
-                case 16: WFB_WSR(16); break; case 24: WFB_WSR(24); break; case 32: WFB_WSR(32); break; case 48: WFB_WSR(48); break; case 64: WFB_WSR(64); break;
+                case 16: WFB_WSRT(16); break; case 24: WFB_WSRT(24); break; case 32: WFB_WSRT(32); break; case 48: WFB_WSRT(48); break; case 64: WFB_WSRT(64); break;
                 default: return WFB_E_UNSUPPORTED;
             }
-#undef WFB_WSR
+#undef WFB_WSRT
             CK(cudaGetLastError());
             launches += 2;
             *counts = c;
