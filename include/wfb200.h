@@ -306,6 +306,10 @@ int wfb_mg_unique_id(void *id128_h);   /* rank 0: an ncclUniqueId (128 bytes) to
 int wfb_mg_create(wfb_mg_t **h, int prog, int nranks, int rank, const void *id128_h, uint64_t win, uint64_t slide, uint32_t wins_per_batch,
                   uint32_t max_keys_total /* keys 0 .. max_keys_total-1 over all ranks */);
 int wfb_mg_destroy(wfb_mg_t *h);
+/* params_t of the program (see wfb_engine_set_params), on every rank: used by the source side of a step that passes no `pre` and, always,
+ * by the destination side -- the key extractor on the received records and the window update's comb and make_result. Call before the
+ * first step; until then both sides use all-zero params. */
+int wfb_mg_set_params(wfb_mg_t *h, const void *params, size_t bytes);
 /* this rank's K batches of the next global step; the window results of the step three calls back go to out_results / out_ts (none on the first three calls).
  * `watermark`: the watermark of the segment (result timestamps carry the watermark of the source segment that held the triggering item). */
 int wfb_mg_step(wfb_mg_t *h, const wfb_functors_t *pre, const wfb_batch_t *batches_h, uint32_t nbatches, uint64_t watermark,

@@ -75,6 +75,7 @@ SYMBOLS = {
     "wfb_mg_unique_id": (C.c_int, [vp]),
     "wfb_mg_create": (C.c_int, [C.POINTER(vp), C.c_int, C.c_int, C.c_int, vp, u64, u64, u32, u32]),
     "wfb_mg_destroy": (C.c_int, [vp]),
+    "wfb_mg_set_params": (C.c_int, [vp, vp, C.c_size_t]),
     "wfb_mg_step": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), u32, u64, vp, vp, u32, vp, vp]),
     "wfb_mg_flush": (C.c_int, [vp, vp, vp, u32, vp, vp]),
     "wfb_mg_launches": (u64, [vp]),

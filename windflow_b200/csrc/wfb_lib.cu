@@ -2063,6 +2063,15 @@ int wfb_mg_create(wfb_mg_t **hh, int prog, int nranks, int rank, const void *id1
     return 0;
 }
 
+int wfb_mg_set_params(wfb_mg_t *h, const void *params, size_t bytes)
+{
+    if (!h) return WFB_E_BADARG;
+    // the source engine (map / filter / key / lift when a step passes no `pre`) and the destination window operator (its key
+    // extractor on the lifted records, comb and make_result): LiftedOf<P> shares P's params_t, so one size fits both
+    int rc = wfb_engine_set_params(h->eng, params, bytes); if (rc) return rc;
+    return wfb_ffat_set_params(h->ffat, params, bytes);
+}
+
 // ---- copy-engine exchange: setup (collective, at the first step) ---------------------------------------------------------------
 struct CeLayout { size_t slots_off, bins_off, bytes; };
 static CeLayout ce_layout(uint64_t cap, int n, size_t rb, uint32_t bps)
@@ -2172,13 +2181,16 @@ static int mg_source(wfb_mg *h, MgSlot &sl, const wfb_functors_t *pre, const wfb
         uint64_t positions = 0;
         for (uint32_t i = 0; i < nbatches; i++) positions += static_cast<uint64_t>(tiles_of(batches_h[i].n)) * TILE;
         if (!h->ce_tried) { rc = mg_ce_setup(h, std::max<uint64_t>(positions, 1)); if (rc) return rc; } // (collective: every rank is in its first step)
-        CK(sl.vslots.ensure(positions, waits, positions));
-        CK(sl.regions.ensure(positions * h->rb, waits, positions * h->rb));
+        // (at least one tile: a step without tuples on a slot that never held any still hands the partition buffers it accepts)
+        const uint64_t room = std::max<uint64_t>(positions, TILE);
+        CK(sl.vslots.ensure(room, waits, room));
+        CK(sl.regions.ensure(room * h->rb, waits, room * h->rb));
         rc = shard_lift_impl(h->eng, pre, batches_h, nbatches, static_cast<uint32_t>(h->nranks), sl.regions, static_cast<uint32_t>(sl.vslots.capacity()), sl.counts, s,
                              h->shard_slots, h->shard_keys, h->shift, sl.vslots, sl.bins, n ? sl.send_meta : nullptr, watermark);
     } else {
         const size_t region_bytes = static_cast<size_t>(h->nranks) * h->rb; // worst case: every item of the segment survives and goes to one shard
-        CK(sl.regions.ensure(n * region_bytes, waits, n * region_bytes));
+        const uint64_t room = std::max<uint64_t>(n, 1); // (a step without tuples: regions of one record, not none)
+        CK(sl.regions.ensure(room * region_bytes, waits, room * region_bytes));
         sl.region_cap = static_cast<uint32_t>(sl.regions.capacity() / region_bytes);
         rc = wfb_shard_lift(h->eng, pre, batches_h, nbatches, static_cast<uint32_t>(h->nranks), sl.regions, sl.region_cap, sl.counts, s);
     }

@@ -211,9 +211,12 @@ class KeyShardedPipelineC:
     are issued by ONE library call per step (NCCL send/recv groups from C on a communication stream; nothing of torch on the per-step
     path). Only the communicator's unique id travels through torch.distributed, once. Same interface as KeyShardedPipeline (always
     pipelined: results arrive THREE steps late, flush() delivers the rest, in step order). With at most 65536 slots over all ranks the
-    exchange is the bucketed one (include/wfb200.h): the destination side runs no partition."""
+    exchange is the bucketed one (include/wfb200.h): the destination side runs no partition.
 
-    def __init__(self, ops, functors, win, slide, nb, max_keys, rank, world, device, prog=None):
+    params: the program's params_t as a ctypes object (wfb_mg_set_params), for a program whose combine, make_result or result_key
+    reads it; `functors` is what every step passes as `pre` (None: the source side uses `params` too)."""
+
+    def __init__(self, ops, functors, win, slide, nb, max_keys, rank, world, device, prog=None, params=None):
         import ctypes as C
         from . import _lib
         self.ops, self.f, self.rank, self.world, self.dev = ops, functors, rank, world, device
@@ -230,6 +233,8 @@ class KeyShardedPipelineC:
         self._id = (C.c_char * 128).from_buffer_copy(bytes(ident.numpy().tobytes()))
         self.h = C.c_void_p()
         _lib.check(self.L.wfb_mg_create(C.byref(self.h), ops.PROG_TUPLE64 if prog is None else prog, world, rank, self._id, win, slide, nb, max_keys), "wfb_mg_create")
+        if params is not None:
+            _lib.check(self.L.wfb_mg_set_params(self.h, C.byref(params), C.sizeof(params)), "wfb_mg_set_params")
         self.res_dtype = ops.RESULT_DTYPE[ops.PROG_TUPLE64 if prog is None else prog]
         self.max_keys, self.slide, self.nb = max_keys, slide, nb
         self.ff = self  # (bench.py talks to `pipe.ff` for launches / stats / results)
