@@ -46,6 +46,7 @@
 #include <vector>
 #include <cuda_runtime.h>
 #include "../ff/ff.hpp"
+#include "deferred_counts.hpp"
 #include "../wfb200.h"
 #include "../../windflow_b200/csrc/wfb_launch.cuh"
 
@@ -213,7 +214,8 @@ template <class T, class S> struct StatefulKeepAll { __host__ __device__ bool op
 
 // ---- Batch_GPU_t (wf/batch_gpu_t.hpp:50-243) as structure of arrays ---------------------------------------------------
 // `size` may be DEFERRED: the producing kernel leaves the count on the device, an asynchronous copy brings it to the pinned
-// word `count_h`, and it is valid once `valid_after` has fired -- getSize() waits for it, nothing else does.
+// word `count_h`, and it is valid once `valid_after` has fired -- getSize() waits for it, nothing else does. The word belongs to a
+// block of the producing replica (wf/deferred_counts.hpp) that is not rewritten while this batch still points into it.
 struct Batch_Base {
     ff::MPMC_Ptr_Queue *home = nullptr; // the producer's recycling queue (the reference's batch->queue, wf/recycling_gpu.hpp:88-141)
     virtual ~Batch_Base() {}
@@ -227,7 +229,7 @@ struct Batch_GPU_t: Batch_Base {
     bool owns_device = true;            // false: the arrays belong to the application (device-side source)
     size_t size = 0, original_size = 0; // items (upper bound while deferred) | capacity
     bool deferred = false;              // size = *count_h once valid_after has fired
-    uint32_t *count_d = nullptr; uint32_t *count_h = nullptr; // deferred count: device word / pinned word (owned by the producing replica)
+    uint32_t *count_h = nullptr; CountBlock *count_blk = nullptr; // deferred count: the pinned word and the producing replica's block it lies in
     std::vector<uint64_t> watermarks{std::numeric_limits<uint64_t>::max()};
     bool isPunctuation = false;
     cudaStream_t cudaStream = nullptr;  // per-batch stream of the host->device copy (wf/batch_gpu_t.hpp:83-101)
@@ -246,6 +248,7 @@ struct Batch_GPU_t: Batch_Base {
     }
     ~Batch_GPU_t() override
     {
+        release_count();
         if (own_ev) { cudaEventSynchronize(own_ev); cudaEventDestroy(own_ev); }
         if (owns_device) { cudaFree(tuples_gpu); cudaFree(ts_gpu); }
         if (pinned_tuples_cpu) cudaFreeHost(pinned_tuples_cpu);
@@ -257,9 +260,12 @@ struct Batch_GPU_t: Batch_Base {
     bool isPunct() const { return isPunctuation; }
     size_t getSize() // resolves a deferred size (waits for the producing work)
     {
-        if (deferred) { gpuErrChk(cudaEventSynchronize(valid_after)); size = *count_h; deferred = false; }
+        if (deferred) { gpuErrChk(cudaEventSynchronize(valid_after)); size = *count_h; deferred = false; release_count(); }
         return size;
     }
+    // the size is word i of `blk`, at most `bound`, valid after `e`
+    void defer(size_t bound, CountBlock *blk, size_t i, cudaEvent_t e) { size = bound; deferred = true; count_blk = blk; count_h = blk->h + i; valid_after = e; }
+    void release_count() { if (count_blk) { count_blk->release(); count_blk = nullptr; } }
     uint64_t getWatermark(size_t id = 0) const { return id < watermarks.size() ? watermarks[id] : watermarks[0]; }
     void setWatermark(uint64_t wm, size_t id = 0) { if (id < watermarks.size()) watermarks[id] = wm; else watermarks[0] = wm; }
     void updateWatermark(uint64_t wm) { if (watermarks[0] > wm) watermarks[0] = wm; }
@@ -283,7 +289,7 @@ struct Batch_GPU_t: Batch_Base {
     }
     tuple_t &getTupleAtPos(size_t pos) { return pinned_tuples_cpu[pos]; }
     uint64_t getTimestampAtPos(size_t pos) { return pinned_ts_cpu[pos]; }
-    void reset(size_t n) { size = n; deferred = false; isPunctuation = false; valid_after = nullptr; watermarks.assign(1, std::numeric_limits<uint64_t>::max()); }
+    void reset(size_t n) { release_count(); size = n; deferred = false; isPunctuation = false; valid_after = nullptr; watermarks.assign(1, std::numeric_limits<uint64_t>::max()); }
 };
 
 // returns a batch to its producer (deleteBatch_t, wf/recycling.hpp:66-85); batches that do not fit the queue are freed
@@ -560,9 +566,8 @@ class ChainReplica: public Basic_Replica {
     using prog_t = ChainProgram<tuple_t>;
     using batch_t = Batch_GPU_t<tuple_t>;
     wfb_engine_t *eng = nullptr; typename prog_t::params_t prm{};
+    DeferredCounts counts; // (before the pool: its batches point into it)
     BatchPool<tuple_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-    uint32_t *counts_d = nullptr, *counts_h = nullptr; size_t ring = 0; // deferred sizes: a ring of device / pinned words
-    static constexpr size_t RING = 16 * WF_MAX_BATCHES_PER_CALL;
     size_t maxk;
     std::vector<batch_t *> in;
     std::vector<wfb_batch_t> bi, bo;
@@ -571,12 +576,12 @@ public:
     {
         if (c.has_filter) prm.filt.c = c; else prm.map.c = c; // (the filter slot runs maps and predicates in order)
     }
-    ~ChainReplica() override { if (eng) wfb_engine_destroy(eng); cudaFree(counts_d); cudaFreeHost(counts_h); }
+    ~ChainReplica() override { if (eng) wfb_engine_destroy(eng); }
     int svc_init() override
     {
         Basic_Replica::svc_init();
         wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
-        if (prm.filt.c.n) { gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING)); }
+        if (prm.filt.c.n) gpuErrChk(counts.init(maxk));
         return 0;
     }
     void *svc(void *msg) override
@@ -600,7 +605,6 @@ private:
             for (auto *b : work) { b->valid_after = e; this->ff_send_out(b); }
         } else {
             const size_t k = work.size();
-            if (ring + k > RING) ring = 0;
             bi.resize(k); bo.resize(k);
             std::vector<batch_t *> outs(k);
             for (size_t i = 0; i < k; i++) {
@@ -613,17 +617,18 @@ private:
                 bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
                 outs[i] = o;
             }
-            wfbErrChk(wfb_map_filter_batches(eng, f, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d + ring, stream));
-            gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
+            CountBlock *blk; uint32_t *counts_d;
+            gpuErrChk(counts.acquire(static_cast<uint32_t>(k), blk, counts_d));
+            wfbErrChk(wfb_map_filter_batches(eng, f, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream));
+            gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
             cudaEvent_t e = next_event();
             gpuErrChk(cudaEventRecord(e, stream));
             for (size_t i = 0; i < k; i++) {
                 batch_t *o = outs[i];
-                o->size = work[i]->size; o->deferred = true; o->count_h = counts_h + ring + i; o->valid_after = e;
+                o->defer(work[i]->size, blk, i, e);
                 work[i]->reuse_after = e; recycleBatch(work[i]); // (the reference drops empty batches here, wf/filter_gpu.hpp:572-581: the
                 this->ff_send_out(o);                             // size is not known on the host yet, the consumer skips an empty one)
             }
-            ring += k;
         }
         work.clear();
     }
@@ -674,10 +679,9 @@ class FlatMapReplica: public Basic_Replica {
     using batch_t = Batch_GPU_t<tuple_t>;
     wfb_engine_t *eng = nullptr; typename prog_t::params_t prm{};
     uint32_t max_out; size_t maxk;
+    DeferredCounts counts; // deferred sizes + the drop count of every call, which this replica reads itself (it holds the block until then)
     BatchPool<result_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-    uint32_t *counts_d = nullptr, *counts_h = nullptr; size_t ring = 0; // deferred sizes + the drop count of every call
-    static constexpr size_t RING = 16 * (WF_MAX_BATCHES_PER_CALL + 1);
-    struct Pending { size_t word; cudaEvent_t ev; };
+    struct Pending { CountBlock *blk; size_t word; cudaEvent_t ev; };
     std::vector<Pending> pending; uint64_t dropped = 0; // drop counts of calls the host has not read yet / the sum of those it read
     std::vector<batch_t *> in;
     std::vector<wfb_batch_t> bi, bo;
@@ -686,12 +690,12 @@ public:
     {
         prm.filt.c = pre; prm.fm = f;
     }
-    ~FlatMapReplica() override { if (eng) wfb_engine_destroy(eng); cudaFree(counts_d); cudaFreeHost(counts_h); }
+    ~FlatMapReplica() override { if (eng) wfb_engine_destroy(eng); }
     int svc_init() override
     {
         Basic_Replica::svc_init();
         wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
-        gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING));
+        gpuErrChk(counts.init(maxk + 1));
         return 0;
     }
     void *svc(void *msg) override
@@ -717,14 +721,15 @@ public:
         Basic_Replica::eosnotify(id);
     }
 private:
-    // adds the drop counts of finished calls (all of them with `wait`); the words of a call are reused only after it was read
+    // adds the drop counts of finished calls (all of them with `wait`)
     void read_drops(bool wait)
     {
         size_t i = 0;
         for (; i < pending.size(); i++) {
             if (wait || pending.size() - i > 8) { gpuErrChk(cudaEventSynchronize(pending[i].ev)); } // (events of the ring are re-recorded after 16 calls)
             else if (cudaEventQuery(pending[i].ev) != cudaSuccess) { cudaGetLastError(); break; }
-            dropped += counts_h[pending[i].word];
+            dropped += pending[i].blk->h[pending[i].word];
+            pending[i].blk->release();
         }
         pending.erase(pending.begin(), pending.begin() + static_cast<std::ptrdiff_t>(i));
     }
@@ -734,7 +739,6 @@ private:
         wait_inputs(work);
         read_drops(false);
         const size_t k = work.size();
-        if (ring + k + 1 > RING) { read_drops(true); ring = 0; }
         bi.resize(k); bo.resize(k);
         std::vector<Batch_GPU_t<result_t> *> outs(k);
         for (size_t i = 0; i < k; i++) {
@@ -747,19 +751,20 @@ private:
             bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(o->original_size), 0};
             outs[i] = o;
         }
+        CountBlock *blk; uint32_t *counts_d;
+        gpuErrChk(counts.acquire(static_cast<uint32_t>(k + 1), blk, counts_d));
         wfbErrChk(wfb_flatmap_batches(eng, reinterpret_cast<const wfb_functors_t *>(&prm), bi.data(), bo.data(), static_cast<uint32_t>(k), max_out,
-                                      counts_d + ring, stream));
-        gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
+                                      counts_d, stream));
+        gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
         cudaEvent_t e = next_event();
         gpuErrChk(cudaEventRecord(e, stream));
-        pending.push_back(Pending{ring + k, e});
+        pending.push_back(Pending{blk, k, e});
         for (size_t i = 0; i < k; i++) {
             Batch_GPU_t<result_t> *o = outs[i];
-            o->size = work[i]->size * max_out; o->deferred = true; o->count_h = counts_h + ring + i; o->valid_after = e;
+            o->defer(work[i]->size * max_out, blk, i, e);
             work[i]->reuse_after = e; recycleBatch(work[i]);
             this->ff_send_out(o);
         }
-        ring += k + 1;
         work.clear();
     }
 };
@@ -805,9 +810,8 @@ public:
     class Replica: public Basic_Replica {
         using batch_t = Batch_GPU_t<tuple_t>;
         std::shared_ptr<SharedKState> ks; typename prog_t::params_t prm; size_t maxk;
+        DeferredCounts counts;
         BatchPool<tuple_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-        uint32_t *counts_d = nullptr, *counts_h = nullptr; size_t ring = 0;
-        static constexpr size_t RING = 16 * WF_MAX_BATCHES_PER_CALL;
         std::vector<batch_t *> in;
         std::vector<wfb_batch_t> bi, bo;
     public:
@@ -816,11 +820,10 @@ public:
             if constexpr (IS_FILTER) return typename prog_t::params_t{{}, f, k}; else return typename prog_t::params_t{f, {}, k};
         }
         Replica(std::string n, std::shared_ptr<SharedKState> h, func_t f, keyextr_func_gpu_t k, size_t mk): Basic_Replica(std::move(n)), ks(std::move(h)), prm(make_params(f, k)), maxk(mk ? mk : 1) {}
-        ~Replica() override { cudaFree(counts_d); cudaFreeHost(counts_h); }
         int svc_init() override
         {
             Basic_Replica::svc_init();
-            if (IS_FILTER) { gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING)); }
+            if (IS_FILTER) gpuErrChk(counts.init(maxk));
             return 0;
         }
         void *svc(void *msg) override
@@ -841,8 +844,9 @@ public:
             bi.resize(k);
             for (size_t i = 0; i < k; i++) bi[i] = wfb_batch_t{work[i]->tuples_gpu, work[i]->ts_gpu, work[i]->getWatermark(), static_cast<uint32_t>(work[i]->size), 0};
             std::vector<batch_t *> outs;
+            CountBlock *blk = nullptr; uint32_t *counts_d = nullptr;
             if constexpr (IS_FILTER) {
-                if (ring + k > RING) ring = 0;
+                gpuErrChk(counts.acquire(static_cast<uint32_t>(k), blk, counts_d));
                 bo.resize(k); outs.resize(k);
                 for (size_t i = 0; i < k; i++) {
                     batch_t *o = pool.get(work[i]->original_size);
@@ -854,20 +858,19 @@ public:
             }
             {   // the replicas of the operator share the state table: one launch sequence at a time (stream order carries the dependency on)
                 std::lock_guard<std::mutex> lock(ks->mu);
-                if constexpr (IS_FILTER) { wfbErrChk(wfb_filter_stateful(ks->h, f, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d + ring, stream)); }
+                if constexpr (IS_FILTER) { wfbErrChk(wfb_filter_stateful(ks->h, f, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream)); }
                 else { wfbErrChk(wfb_map_stateful(ks->h, f, bi.data(), static_cast<uint32_t>(k), stream)); }
                 gpuErrChk(cudaStreamSynchronize(stream)); // another replica's launches on its own stream must see this call's state
             }
             cudaEvent_t e = next_event();
             if constexpr (IS_FILTER) {
-                gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
+                gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
                 gpuErrChk(cudaEventRecord(e, stream));
                 for (size_t i = 0; i < k; i++) {
-                    outs[i]->size = work[i]->size; outs[i]->deferred = true; outs[i]->count_h = counts_h + ring + i; outs[i]->valid_after = e;
+                    outs[i]->defer(work[i]->size, blk, i, e);
                     work[i]->reuse_after = e; recycleBatch(work[i]);
                     this->ff_send_out(outs[i]);
                 }
-                ring += k;
             } else {
                 gpuErrChk(cudaEventRecord(e, stream));
                 for (auto *b : work) { b->valid_after = e; this->ff_send_out(b); }
@@ -900,21 +903,20 @@ public:
     class Replica: public Basic_Replica {
         using batch_t = Batch_GPU_t<tuple_t>;
         wfb_engine_t *eng = nullptr; typename prog_t::params_t prm; uint32_t key_bits; size_t maxk;
+        DeferredCounts counts;
         BatchPool<tuple_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-        uint32_t *counts_d = nullptr, *counts_h = nullptr; size_t ring = 0;
-        static constexpr size_t RING = 16 * WF_MAX_BATCHES_PER_CALL;
         std::vector<batch_t *> in;
         std::vector<wfb_batch_t> bi, bo;
     public:
         Replica(std::string n, reduce_func_gpu_t f, keyextr_func_gpu_t k, uint32_t kb, size_t mk): Basic_Replica(std::move(n)), prm{{}, {}, k, {}, {}, f}, key_bits(kb), maxk(mk ? mk : 1) {}
-        ~Replica() override { if (eng) wfb_engine_destroy(eng); cudaFree(counts_d); cudaFreeHost(counts_h); }
+        ~Replica() override { if (eng) wfb_engine_destroy(eng); }
         int svc_init() override
         {
             Basic_Replica::svc_init();
             wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
             wfbErrChk(wfb_engine_set_params(eng, &prm, sizeof(prm)));
             if (key_bits != 64) wfbErrChk(wfb_engine_set_key_bits(eng, key_bits)); // (integral keys: ReduceGPU_Builder::build checks)
-            gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING));
+            if (isKeyed) gpuErrChk(counts.init(maxk));
             return 0;
         }
         void *svc(void *msg) override
@@ -931,9 +933,10 @@ public:
             if (work.empty()) return;
             wait_inputs(work);
             const size_t k = work.size();
-            if (ring + k > RING) ring = 0;
             bi.resize(k); bo.resize(k);
             std::vector<batch_t *> outs(k);
+            CountBlock *blk = nullptr; uint32_t *counts_d = nullptr;
+            if (isKeyed) gpuErrChk(counts.acquire(static_cast<uint32_t>(k), blk, counts_d));
             uint32_t kbits = 0; while ((1ull << kbits) < k) kbits++;
             for (size_t i = 0; i < k; i++) {
                 batch_t *o = pool.get(isKeyed ? work[i]->original_size : 1);
@@ -945,23 +948,21 @@ public:
             }
             if constexpr (isKeyed) {
                 const uint32_t sort_bits = integral_key_v<keyextr_func_gpu_t> ? key_bits : 32u; // other keys are sorted by their 32-bit rank
-                if (k > 1 && sort_bits + kbits <= 64) { wfbErrChk(wfb_reduce_by_key_batches(eng, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d + ring, stream)); }
+                if (k > 1 && sort_bits + kbits <= 64) { wfbErrChk(wfb_reduce_by_key_batches(eng, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream)); }
                 else for (size_t i = 0; i < k; i++)
-                    wfbErrChk(wfb_reduce_by_key(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), counts_d + ring + i, stream));
-                gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
+                    wfbErrChk(wfb_reduce_by_key(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), counts_d + i, stream));
+                gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
             } else {
                 for (size_t i = 0; i < k; i++) wfbErrChk(wfb_reduce_all(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), stream));
             }
             cudaEvent_t e = next_event();
             gpuErrChk(cudaEventRecord(e, stream));
             for (size_t i = 0; i < k; i++) {
-                if (isKeyed) { outs[i]->size = work[i]->size; outs[i]->deferred = true; outs[i]->count_h = counts_h + ring + i; }
-                else outs[i]->size = 1;
-                outs[i]->valid_after = e;
+                if (isKeyed) outs[i]->defer(work[i]->size, blk, i, e);
+                else { outs[i]->size = 1; outs[i]->valid_after = e; }
                 work[i]->reuse_after = e; recycleBatch(work[i]);
                 this->ff_send_out(outs[i]);
             }
-            ring += k;
             work.clear();
         }
     };
@@ -1005,22 +1006,21 @@ public:
         using batch_t = Batch_GPU_t<tuple_t>;
         Ffat_Windows_GPU op;
         wfb_ffat_t *ffat = nullptr; typename prog_t::params_t prm;
+        DeferredCounts counts; // (one word per call)
         BatchPool<result_t> pool{64};
-        uint32_t *counts_d = nullptr, *counts_h = nullptr; size_t ring = 0;
-        static constexpr size_t RING = 256;
         const bool tb; uint64_t last_wm = 0; size_t cap_hint = 0;
         std::vector<batch_t *> in;
         std::vector<wfb_batch_t> bi;
     public:
         explicit Replica(const Ffat_Windows_GPU &o): Basic_Replica(o.name), op(o), prm{{}, o.pre, o.key_extr, o.lift, o.comb, {}}, tb(o.winType == Win_Type_t::TB) {}
-        ~Replica() override { if (ffat) wfb_ffat_destroy(ffat); cudaFree(counts_d); cudaFreeHost(counts_h); }
+        ~Replica() override { if (ffat) wfb_ffat_destroy(ffat); }
         int svc_init() override
         {
             Basic_Replica::svc_init();
             wfbErrChk(wfb_ffat_create(&ffat, wfb::register_program<prog_t>(), op.win_len, op.slide_len, static_cast<uint32_t>(op.numWinPerBatch),
                                       op.max_keys, tb ? 1 : 0, op.lateness, (op.dense_keys ? WFB_FFAT_DENSE_KEYS : 0u) | (op.grow_keys ? WFB_KEYS_GROW : 0u)));
             wfbErrChk(wfb_ffat_set_params(ffat, &prm, sizeof(prm)));
-            gpuErrChk(cudaMalloc(&counts_d, sizeof(uint32_t) * RING)); gpuErrChk(cudaMallocHost(&counts_h, sizeof(uint32_t) * RING));
+            gpuErrChk(counts.init(1));
             return 0;
         }
         void *svc(void *msg) override
@@ -1049,16 +1049,16 @@ public:
             if (tb) last_wm = wm;
             Batch_GPU_t<result_t> *out = pool.get(cap);
             if (out->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, out->reuse_after, 0));
-            if (ring == RING) ring = 0;
+            CountBlock *blk; uint32_t *count_d;
+            gpuErrChk(counts.acquire(1, blk, count_d));
             const wfb_functors_t *pre = op.has_pre() ? reinterpret_cast<const wfb_functors_t *>(&prm) : nullptr;
-            if (tb) { wfbErrChk(wfb_ffat_process_tb(ffat, pre, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), counts_d + ring, stream)); }
-            else { wfbErrChk(wfb_ffat_process_cb(ffat, pre, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), counts_d + ring, stream)); }
+            if (tb) { wfbErrChk(wfb_ffat_process_tb(ffat, pre, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), count_d, stream)); }
+            else { wfbErrChk(wfb_ffat_process_cb(ffat, pre, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), count_d, stream)); }
             if (tb) check_errors(); // (the time-based path synchronises per batch anyway: a result that did not fit is reported, not lost silently)
-            gpuErrChk(cudaMemcpyAsync(counts_h + ring, counts_d + ring, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+            gpuErrChk(cudaMemcpyAsync(blk->h, count_d, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
             cudaEvent_t e = next_event();
             gpuErrChk(cudaEventRecord(e, stream));
-            out->size = cap; out->deferred = true; out->count_h = counts_h + ring; out->valid_after = e; out->setWatermark(wm);
-            ring++;
+            out->defer(cap, blk, 0, e); out->setWatermark(wm);
             for (auto *b : work) { b->reuse_after = e; recycleBatch(b); }
             this->ff_send_out(out);
             return this->GO_ON;

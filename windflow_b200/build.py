@@ -34,7 +34,7 @@ def build(force=False, verbose=False):
 
 APPS = os.path.join(HERE, "apps")
 INCLUDE = os.path.join(HERE, "..", "include")
-FACADE_HEADERS = [os.path.join(INCLUDE, "wf", "windflow_gpu.hpp"), os.path.join(INCLUDE, "ff", "ff.hpp"), os.path.join(INCLUDE, "wfb200.h")]
+FACADE_HEADERS = [os.path.join(INCLUDE, "wf", "windflow_gpu.hpp"), os.path.join(INCLUDE, "wf", "deferred_counts.hpp"), os.path.join(INCLUDE, "ff", "ff.hpp"), os.path.join(INCLUDE, "wfb200.h")]
 
 
 def build_apps(force=False):
