@@ -19,7 +19,11 @@
  *    without touching the operator API;
  *  - record schemas and functors are compiled in ("programs"): the library pre-instantiates the programs
  *    below; user code instantiates its own with WFB_DEFINE_PROGRAM from windflow_b200/csrc/wfb_kernels.cuh
- *    and gets the same entry points for its functors (see INTEGRATION.md).
+ *    and gets the same entry points for its functors (see INTEGRATION.md);
+ *  - a program's tuple_t and result_t are multiples of 8 bytes of up to about 430 bytes (two tile-pass stages of 256 records must
+ *    fit 227 KB of shared memory: larger records fail to compile in wfb::register_program); sizes up to 256 bytes are tested.
+ *    Results above 160 bytes have no bucket window update: their count-based handles take the full-sort path at every key count
+ *    (INTEGRATION.md section 3).
  */
 #ifndef WFB200_H
 #define WFB200_H

@@ -440,6 +440,10 @@ struct StageMeta {
     uint32_t wide, pad;                             // wide: ticket (= wide tile when tiles_per_ticket = 16)
 };
 
+constexpr uint32_t TP_SMEM_MAX = 232448; // opt-in dynamic shared memory of one block on sm_90 (227 KB)
+
+// Shared memory of k_tile_pass<P, MODE>. The ring keeps STAGES stages while they fit TP_SMEM_MAX; larger records get 3, then 2
+// (records of up to about 430 bytes); a record that does not fit twice fails to compile (launch_tile_pass).
 template <class P, int MODE>
 struct TilePassSmem {
     using T = typename P::tuple_t;
@@ -449,7 +453,9 @@ struct TilePassSmem {
     static constexpr uint32_t aux_bytes = (MODE == MODE_INGEST) ? TILE * 4u : (MODE == MODE_FILTER ? TILE * 16u : (MODE == MODE_FLATMAP ? TILE * 8u : 0u)); // slots | ts in + ts out | ts in
     static constexpr uint32_t stage_bytes = tile_bytes + aux_bytes;
     static constexpr uint32_t hist_bytes = (MODE == MODE_INGEST) ? 4u * 256u * 4u : 0u; // up to 4 sort passes of 8 bits or one of 10 | two buffers of 1024 packed 16-bit per-wide-tile counts
-    static constexpr uint32_t total = STAGES * stage_bytes + 1024 /*alignment slack*/ + 1024 /*barriers, meta, scan*/ + hist_bytes;
+    static constexpr uint32_t total_at(uint32_t st) { return st * stage_bytes + 1024 /*alignment slack*/ + 1024 /*barriers, meta, scan*/ + hist_bytes; }
+    static constexpr int stages = (STAGES <= 2 || total_at(STAGES) <= TP_SMEM_MAX) ? STAGES : ((STAGES > 3 && total_at(3) <= TP_SMEM_MAX) ? 3 : 2);
+    static constexpr uint32_t total = total_at(stages);
 };
 
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar)
@@ -515,12 +521,12 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
 
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    unsigned char *ctl = smem + STAGES * SM::stage_bytes;
-    uint64_t *full = reinterpret_cast<uint64_t *>(ctl);          // STAGES  producer -> consumers (tx)
-    uint64_t *staged = full + STAGES;                            // STAGES  consumers -> epilogue
-    uint64_t *empty = staged + STAGES;                           // STAGES  epilogue -> producer
-    StageMeta *meta = reinterpret_cast<StageMeta *>(empty + STAGES);  // STAGES
-    uint32_t *warp_tot = reinterpret_cast<uint32_t *>(meta + STAGES); // 2 x 8 warp totals (double-buffered by iteration parity)
+    unsigned char *ctl = smem + SM::stages * SM::stage_bytes;        // (SM::stages: the ring depth of this record size)
+    uint64_t *full = reinterpret_cast<uint64_t *>(ctl);              // stages  producer -> consumers (tx)
+    uint64_t *staged = full + SM::stages;                            // stages  consumers -> epilogue
+    uint64_t *empty = staged + SM::stages;                           // stages  epilogue -> producer
+    StageMeta *meta = reinterpret_cast<StageMeta *>(empty + SM::stages);  // stages
+    uint32_t *warp_tot = reinterpret_cast<uint32_t *>(meta + SM::stages); // 2 x 8 warp totals (double-buffered by iteration parity)
     uint32_t *fm_words = warp_tot + 2 * (TILE / 32);                  // MODE_FLATMAP: 2 x 8 warp drop counts, then 2 tile bases
     uint32_t *s_hist = reinterpret_cast<uint32_t *>(ctl + 1024);      // MODE_INGEST: [pass][1 << sort_dbits] digit counts of this CTA (1024 words)
 
@@ -529,7 +535,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
     auto stage_aux = [&](uint32_t s) { return smem + s * SM::stage_bytes + SM::tile_bytes; };
 
     if (tid == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&staged[s], TILE / 32); mbar_init(&empty[s], 1); }
+        for (int s = 0; s < SM::stages; s++) { mbar_init(&full[s], 1); mbar_init(&staged[s], TILE / 32); mbar_init(&empty[s], 1); }
         mbar_fence_init();
     }
     if constexpr (MODE == MODE_INGEST) { for (uint32_t i = tid; i < 4u * 256u; i += TP_THREADS) s_hist[i] = 0; }
@@ -544,7 +550,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
             const uint32_t tpt = a.tiles_per_ticket ? a.tiles_per_ticket : 1u;
             uint32_t t_next = 0, t_end = 0, claim = 0; // tiles [t_next, t_end) of the current claim are still to load
             for (uint32_t it = 0;; it++) {
-                const uint32_t s = it % STAGES, par = (it / STAGES) & 1u;
+                const uint32_t s = it % SM::stages, par = (it / SM::stages) & 1u;
                 mbar_wait(&empty[s], par ^ 1u); // a fresh barrier passes the wait on parity 1
                 // claim only now: a claimed tile is loaded at once, so the look-backs of its successors never wait on a stalled ring
                 StageMeta &m = meta[s];
@@ -588,7 +594,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
         const uint32_t ctid = tid - 32, cwarp = warp - 1;
         uint32_t wpar = 0; // which of the two digit-count buffers the current wide tile uses
         for (uint32_t it = 0;; it++) {
-            const uint32_t s = it % STAGES, par = (it / STAGES) & 1u;
+            const uint32_t s = it % SM::stages, par = (it / SM::stages) & 1u;
             unsigned char *buf = stage_buf(s);
             mbar_wait(&full[s], par);
             const StageMeta m = meta[s];
@@ -761,7 +767,7 @@ __global__ void __launch_bounds__(TP_THREADS) k_tile_pass(const __grid_constant_
     } else {
         // ================================= EPILOGUE =================================
         for (uint32_t it = 0;; it++) {
-            const uint32_t s = it % STAGES, par = (it / STAGES) & 1u;
+            const uint32_t s = it % SM::stages, par = (it / SM::stages) & 1u;
             unsigned char *buf = stage_buf(s);
             mbar_wait(&staged[s], par);
             const StageMeta m = meta[s];
@@ -1980,6 +1986,20 @@ constexpr uint32_t BK_CNT_U = 16;     // bucket-list loads in flight per thread 
 __device__ __forceinline__ uint32_t bk_opaque(uint32_t v) { asm volatile("" : "+r"(v)); return v; }
 template <uint32_t RB>                // items per thread and chunk: BK_REC_BYTES of records, 1..8
 constexpr uint32_t bk_items_per_thread() { return BK_REC_BYTES / (BK_THREADS * RB) < 1 ? 1 : (BK_REC_BYTES / (BK_THREADS * RB) > 8 ? 8 : BK_REC_BYTES / (BK_THREADS * RB)); }
+template <uint32_t RB>                // FlatFAT levels whose siblings k_ffat_update_buckets stages in shared memory
+constexpr uint32_t bk_sibl_levels() { return RB <= 32 ? 8 : (RB <= 48 ? 4 : (RB <= 128 ? 2 : 1)); }
+// static shared memory of k_ffat_update_buckets<P, LAZY> for results of RB bytes: its arrays below, plus 64 bytes for alignment
+template <uint32_t RB, bool LAZY>
+constexpr uint32_t bk_smem_bytes()
+{
+    constexpr uint32_t IT = bk_items_per_thread<RB>(), CAP = BK_THREADS * IT, CS = IT * (BK_THREADS / 32) + 2;
+    return CAP * RB + 3 * CAP * 4 + BK_KEYS * CS * 2 + 5 * BK_KEYS * 4 + 3 * BK_KEYS * 8 + BK_KEYS * RB
+         + (LAZY ? 16 : BK_KEYS * bk_sibl_levels<RB>() * RB) + 2 * BK_KEYS * 4 + BK_THREADS * 4 + (BK_THREADS / 32 + 5) * 4 + 64;
+}
+// The bucket update exists for results whose layout fits the 48 KB of static shared memory (RB <= 160 bytes): a program with larger
+// results has no bucket kernel (ProgramOps::ffat_buckets is null) and its count-based handles take the full-sort path at every capacity
+template <uint32_t RB>
+constexpr bool bk_fits() { return bk_smem_bytes<RB, false>() <= (48u << 10) && bk_smem_bytes<RB, true>() <= (48u << 10); }
 #ifndef WFB_BK_MINBLOCKS
 #define WFB_BK_MINBLOCKS 4        // eager FlatFAT levels (16 KB of staged siblings on top of the lazy footprint)
 #endif
@@ -2005,8 +2025,9 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
     constexpr uint32_t NCOL = IT * NW;                                 // (round, warp) columns of the split counts
     constexpr uint32_t CS = NCOL + 2;                                  // row stride of the split counts (odd in words: no bank conflicts)
     constexpr uint32_t CPB = (RB % 16 == 0) ? 16 : 8;                  // cp.async granule of a record
-    constexpr uint32_t BK_SIBL = RB <= 32 ? 8 : (RB <= 48 ? 4 : (RB <= 128 ? 2 : 1)); // FlatFAT levels whose siblings are staged in shared memory
+    constexpr uint32_t BK_SIBL = bk_sibl_levels<RB>();                 // FlatFAT levels whose siblings are staged in shared memory
     static_assert(DPT % 4 == 0 && BK_KEYS == 64 && BK_THREADS == 128 && RB % 8 == 0, "layout");
+    static_assert(bk_fits<RB>(), "the arrays below exceed 48 KB of static shared memory (bk_smem_bytes)");
     __shared__ __align__(16) unsigned char s_rec[CAP * RB]; // the chunk's records, key-major; a segment's fold replaces its first record
     __shared__ uint32_t s_idx[CAP];                    // record index of the items (into `lifted`), key-major
     __shared__ uint32_t s_lslot[CAP], s_lpos[CAP];     // the bucket list of the next chunk (slots, arrival positions), prefetched

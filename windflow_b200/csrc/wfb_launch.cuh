@@ -138,6 +138,8 @@ template <class P, int MODE>
 int launch_tile_pass(TileArgs &a, const void *params, uint32_t want_grid, cudaStream_t s, uint32_t *grid_used,
                      uint64_t span_begin, uint64_t span_end)
 {
+    static_assert(TilePassSmem<P, MODE>::total <= TP_SMEM_MAX, "tuple_t / result_t too large for the tile pass: two stages of 256 records "
+                  "must fit TP_SMEM_MAX (232448 bytes) of shared memory (records of up to about 430 bytes)");
     static int max_grid = -1;
     constexpr uint32_t smem = TilePassSmem<P, MODE>::total;
     if (max_grid < 0) {
@@ -198,6 +200,13 @@ int ffat_buckets_dispatch(const FfatDev &ff, const unsigned char *lifted, const 
                                                                           nbatches, out_res, out_ts, out_cap, n_out, load_params<P>(params));
     WFB_CK(cudaGetLastError());
     return 0;
+}
+// the bucket update of P, or null when its results are too large for it (the handles then take the full-sort path): the kernel is
+// instantiated only for results that fit (bk_fits)
+template <class P>
+constexpr decltype(ProgramOps::ffat_buckets) ffat_buckets_of()
+{
+    if constexpr (bk_fits<sizeof(typename P::result_t)>()) return &ffat_buckets_dispatch<P>; else return nullptr;
 }
 
 template <class P>
@@ -417,7 +426,7 @@ const void *lifted_ops_of()
         t.tuple_bytes = sizeof(typename L::tuple_t); t.result_bytes = sizeof(typename L::result_t);
         t.params_bytes = sizeof(typename L::params_t); t.reserved = 1u; // pass-through
         t.tile_pass = &tile_pass_ingest_dispatch<L>; t.slots_inplace = &slots_inplace_dispatch<L>;
-        t.ffat_update = &ffat_update_dispatch<L>; t.ffat_buckets = &ffat_buckets_dispatch<L>; t.ffat_windows = &ffat_windows_dispatch<L>;
+        t.ffat_update = &ffat_update_dispatch<L>; t.ffat_buckets = ffat_buckets_of<L>(); t.ffat_windows = &ffat_windows_dispatch<L>;
         t.key_bytes = 8u * key_codec<L>::words; t.key_kind = key_codec<L>::kind; t.key_size = sizeof(typename L::key_t);
         t.reserved2 = program_has_result_key<P>::value ? 1u : 0u; // bit 0: the lifted records carry their key (usable behind an exchange)
         return t;
@@ -434,7 +443,7 @@ ProgramOps make_ops()
     o.params_bytes = sizeof(typename P::params_t); o.reserved = program_passthrough<P>::value ? 1u : 0u; // bit 0: records pass through unchanged
     o.tile_pass = &tile_pass_dispatch<P>;
     o.ffat_update = &ffat_update_dispatch<P>;
-    o.ffat_buckets = &ffat_buckets_dispatch<P>;
+    o.ffat_buckets = ffat_buckets_of<P>();
     o.ffat_windows = &ffat_windows_dispatch<P>;
     o.extract_keys = &extract_keys_dispatch<P>;
     o.reduce_segments = &reduce_segments_dispatch<P>;

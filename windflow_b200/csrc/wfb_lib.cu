@@ -1164,8 +1164,9 @@ static void ffat_derive_paths(wfb_ffat *h)
     uint32_t bits = 0; while ((1ull << bits) < h->ff.max_keys) bits++;
     h->sort_passes = bits / 8 + 1;
     h->bucket_shift = bits > OSW_BITS ? bits - OSW_BITS : 0;
-    // bucket path: every bucket holds at most BK_KEYS keys and the pane length fits 32 bits
-    h->buckets = (1u << h->bucket_shift) <= BK_KEYS && h->ff.pane < (1ull << 32);
+    // bucket path: every bucket holds at most BK_KEYS keys, the pane length fits 32 bits and the program has a bucket kernel (a
+    // result_t above 160 bytes has none: bk_fits)
+    h->buckets = (1u << h->bucket_shift) <= BK_KEYS && h->ff.pane < (1ull << 32) && h->ops->ffat_buckets != nullptr;
 }
 
 // deferred window groups a segment of seg_cap records can fire: one per slide * Nb records, and one more per key
