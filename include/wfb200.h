@@ -283,7 +283,8 @@ int wfb_ffat_stats(wfb_ffat_t *h, uint32_t *n_keys_h, uint32_t *err_flags_h, voi
 uint32_t wfb_ffat_key_capacity(const wfb_ffat_t *h);
 /* Window results delivered by the handle since it was created (summed on the device by the last kernel of every call; synchronises
  * the stream). Lets a caller account for results without reading *n_out_dev back after every call (the role of the
- * outputs_sent counter of wf/stats_record.hpp:80-82). */
+ * outputs_sent counter of wf/stats_record.hpp:80-82). A WFB_FFAT_PIPELINED handle counts a segment's results when its window update
+ * runs, one call before it delivers them: after wfb_ffat_flush the total is what was delivered. */
 int wfb_ffat_results_total(wfb_ffat_t *h, uint64_t *total_h, void *stream);
 
 /* ---- the pipeline sharded by key across the GPUs of one box (no counterpart in the reference: it drives one device) ----------------
