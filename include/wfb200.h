@@ -14,6 +14,10 @@
  *  - a call that cannot allocate the scratch memory it grows on demand returns the CUDA error and leaves the handle usable: a later
  *    call allocates again;
  *  - pointers are DEVICE pointers unless the name ends in _h; `stream` is a cudaStream_t passed as void*;
+ *  - successive calls on one handle may pass different streams (a replica may bind every call to its batch's own stream): each call
+ *    is ordered on the device behind everything the handle issued before, and a query that takes a stream sees every earlier call.
+ *    The caller still orders its own input and output buffers with the stream it passes. Calls on a keyed-stateful handle
+ *    (wfb_kstate_t) may come from several threads at once;
  *  - a batch is structure-of-arrays: `tuples` (n * tuple_bytes, 16-byte aligned) and `ts` (n * uint64_t);
  *    user functors only ever see `tuple_t &`, so this replaces wf/basic_gpu.hpp:132-140's 72-byte AoS item
  *    without touching the operator API;

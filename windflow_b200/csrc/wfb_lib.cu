@@ -75,36 +75,44 @@ struct PinnedStage {
     void destroy() { for (int i = 0; i < SLOTS; i++) { if (ev[i]) cudaEventDestroy(ev[i]); ev[i] = nullptr; } }
 };
 
-// ---- scratch shared by the tile passes: ticket counter, epoch-tagged tile states, batch descriptors -----------
-struct TileScratch {
-    PinnedStage stage;
-    Scratch<uint64_t> tile_state;
-    Scratch<uint32_t> ticket; uint32_t ticket_base = 0; uint32_t epoch = 0;
-    Scratch<DevBatch> d_batches;
+// ---- stream order of one handle: a call on a new stream waits for everything the handle issued on the previous one ----------
+// A handle's scratch and state are shared by its consecutive calls, and the reference launches on each batch's own stream
+// (wf/map_gpu.hpp:399-405), so a caller may hop between streams from one call to the next.
+struct StreamOrder {
     cudaStream_t last_stream = nullptr; bool used = false; cudaEvent_t ev = nullptr;
 
-    int init()
-    {
-        CK(ticket.ensure(1));
-        CK(cudaMemset(ticket, 0, sizeof(uint32_t)));
-        CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        return 0;
-    }
-    void destroy()
-    {
-        stage.destroy();
-        if (ev) cudaEventDestroy(ev);
-    }
-    // scratch is shared by consecutive launches: order them when the caller hops between streams
-    // (the reference launches on each batch's own stream, wf/map_gpu.hpp:399-405)
+    int init() { CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); return 0; }
+    void destroy() { if (ev) cudaEventDestroy(ev); ev = nullptr; }
     int enter(cudaStream_t s)
     {
         if (used && s != last_stream) { CK(cudaEventRecord(ev, last_stream)); CK(cudaStreamWaitEvent(s, ev, 0)); }
         last_stream = s; used = true;
         return 0;
     }
-    int ensure_tiles(uint32_t num_tiles) { return tile_state.ensure_zeroed(num_tiles, last_stream, last_stream); } // epoch 0 is never used by a launch
-    int ensure_batches(uint32_t nb) { return d_batches.ensure(nb, last_stream); }
+};
+
+// ---- scratch shared by the tile passes: ticket counter, epoch-tagged tile states, batch descriptors -----------
+struct TileScratch {
+    PinnedStage stage;
+    Scratch<uint64_t> tile_state;
+    Scratch<uint32_t> ticket; uint32_t ticket_base = 0; uint32_t epoch = 0;
+    Scratch<DevBatch> d_batches;
+    StreamOrder order;
+
+    int init()
+    {
+        CK(ticket.ensure(1));
+        CK(cudaMemset(ticket, 0, sizeof(uint32_t)));
+        return order.init();
+    }
+    void destroy()
+    {
+        stage.destroy();
+        order.destroy();
+    }
+    int enter(cudaStream_t s) { return order.enter(s); }
+    int ensure_tiles(uint32_t num_tiles) { return tile_state.ensure_zeroed(num_tiles, order.last_stream, order.last_stream); } // epoch 0 is never used by a launch
+    int ensure_batches(uint32_t nb) { return d_batches.ensure(nb, order.last_stream); }
     void next_launch(TileArgs &a) { epoch = (epoch + 1) & 0x3fffffffu; if (epoch == 0) epoch = 1; a.epoch = epoch; a.ticket = ticket; a.ticket_base = ticket_base; a.tile_state = tile_state; }
     void launched(uint32_t num_claims, uint32_t grid) { ticket_base += num_claims + grid; } // one failing claim per CTA
 };
@@ -989,6 +997,8 @@ struct wfb_kstate {
     uint64_t launches = 0;
     PinnedStage stage;
     GrowCheck growc;              // WFB_KEYS_GROW (ff.grow)
+    StreamOrder order;            // a call on another stream waits for the previous call: the scratch and the states are shared
+    std::mutex mu;                // the replicas of an operator share the handle: one call at a time (the reference's spinlock)
 };
 extern "C" {
 
@@ -1018,6 +1028,7 @@ int wfb_kstate_create(wfb_kstate_t **hh, int prog, uint32_t max_keys, uint32_t f
     kstate_derive_paths(h, max_keys);
     FfatDev &ff = h->ff;
     ff.max_keys = max_keys; ff.dense = (flags & WFB_FFAT_DENSE_KEYS) ? 1u : 0u;
+    rc = h->order.init(); if (rc) { wfb_kstate_destroy(h); return rc; }
     if (flags & WFB_KEYS_GROW) { ff.grow = 1; rc = h->growc.init(); if (rc) { wfb_kstate_destroy(h); return rc; } }
     uint32_t cap = 1; while (cap < 2ull * max_keys) cap <<= 1;
     ff.ht_mask = cap - 1;
@@ -1041,7 +1052,7 @@ int wfb_kstate_destroy(wfb_kstate_t *h)
     if (!h) return 0;
     cudaDeviceSynchronize();
     cudaFree(h->ff.ht_keys); cudaFree(h->ff.ht_slots); cudaFree(h->ff.n_slots); cudaFree(h->ff.slot_key); cudaFree(h->states);
-    h->stage.destroy(); h->growc.destroy();
+    h->stage.destroy(); h->growc.destroy(); h->order.destroy();
     delete h;
     cudaGetLastError();
     return 0;
@@ -1054,6 +1065,8 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
 {
     if (!h || !f || (nbatches && !in_h) || (filter && (!out_h || !n_out_dev))) return WFB_E_BADARG;
     if (nbatches == 0) return 0;
+    std::lock_guard<std::mutex> lock(h->mu);
+    int rc = h->order.enter(s); if (rc) return rc;
     if (filter) CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t) * nbatches, s));
     std::vector<DevBatch> hb(nbatches);
     std::vector<uint32_t> boff(nbatches + 1);
@@ -1085,7 +1098,7 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
     { int rc_ = h->stage.h2d(h->d_boff, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
     // 1. slots; 2. one wide partition pass into 1024 buckets of consecutive slots; 3. per-bucket CTAs, one thread per key
     // (more than 65536 keys: 2. a stable sort by slot; 3. one thread per run of a slot)
-    int rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc;
+    rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc;
     for (bool grew = h->ff.grow != 0; grew; ) { // (a growing handle stops at 65536 keys, the last capacity of the bucket path, on its way up)
         rc = grow_keys(h->ff, h->ops->key_bytes, h->growc, 1u << (OSW_BITS + 6), 1u << 30, s, &grew,
                        [h](GrowPlan &plan, uint32_t cap) {
@@ -1854,19 +1867,22 @@ int wfb_ffat_stats(wfb_ffat_t *h, uint32_t *n_keys_h, uint32_t *err_flags_h, voi
 {
     if (!h) return WFB_E_BADARG;
     uint32_t v[2] = {0, 0};
+    int rc = h->ts.enter(static_cast<cudaStream_t>(stream)); if (rc) return rc; // (the counters of a call issued on another stream)
     if (h->s2) CK(cudaStreamSynchronize(h->s2));
     CK(cudaMemcpyAsync(v, h->ff.n_slots, sizeof(v), cudaMemcpyDeviceToHost, static_cast<cudaStream_t>(stream)));
     CK(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
     if (n_keys_h) *n_keys_h = v[0];
     if (err_flags_h) *err_flags_h = v[1];
-    if (h->cb && err_flags_h) { uint32_t e2 = 0; int rc = wfb_ffat_stats(h->cb, nullptr, &e2, stream); if (rc) return rc; *err_flags_h |= e2; }
+    if (h->cb && err_flags_h) { uint32_t e2 = 0; rc = wfb_ffat_stats(h->cb, nullptr, &e2, stream); if (rc) return rc; *err_flags_h |= e2; }
     return 0;
 }
 
 int wfb_ffat_results_total(wfb_ffat_t *h, uint64_t *total_h, void *stream)
 {
     if (!h || !total_h) return WFB_E_BADARG;
-    const wfb_ffat *src = h->cb ? h->cb : h; // time-based handles: the count-based back end emits the results
+    wfb_ffat *src = h->cb ? h->cb : h; // time-based handles: the count-based back end emits the results
+    int rc = h->ts.enter(static_cast<cudaStream_t>(stream)); if (rc) return rc;
+    if (src != h) { rc = src->ts.enter(static_cast<cudaStream_t>(stream)); if (rc) return rc; }
     unsigned long long v = 0;
     if (src->s2) CK(cudaStreamSynchronize(src->s2));
     if (src->ff.results_total == nullptr) { *total_h = 0; return 0; }
