@@ -1136,6 +1136,19 @@ constexpr uint32_t OSW_THREADS = 256, OSW_ITEMS = 16, OSW_TILE = OSW_THREADS * O
 static_assert(OSW_TILE == OSW_TILE_POS, "the tile pass files its digit counts per wide tile");
 // wide tiles per CTA of k_wide_scatter_ranked (and per offset row T of k_wide_tile_bases): a chunk is a whole number of groups
 constexpr uint32_t OSR_GROUP = 4, OSR_GROUP_POS = OSR_GROUP * OSW_TILE;
+// The bucket list the partition leaves for k_ffat_update_buckets: ONE word per item, pos << BKL_KEY_BITS | local key. local key = slot -
+// first slot of the item's bucket (a bucket holds at most 2^BKL_KEY_BITS consecutive slots; the bucket is the update's CTA), pos = the
+// item's record index relative to the first position of its position range (moved records: the arrival position of the item whose
+// record sits at that list index). The word holds positions below BKL_RANGE_POS, so a window phase over more positions runs in ranges
+// of BKL_RANGE_POS positions: partition, update and window queries of one range, then the next (ffat_window_phase,
+// ffat_process_prebucketed). A test build may lower WFB_BKL_RANGE_POS to cut small calls into many ranges.
+#ifndef WFB_BKL_RANGE_POS
+#define WFB_BKL_RANGE_POS (1u << 26)
+#endif
+constexpr uint32_t BKL_KEY_BITS = 6, BKL_RANGE_POS = WFB_BKL_RANGE_POS;
+static_assert(BKL_RANGE_POS <= (1u << (32 - BKL_KEY_BITS)) && BKL_RANGE_POS >= OSR_GROUP_POS && BKL_RANGE_POS % OSR_GROUP_POS == 0,
+              "a range is whole groups of wide tiles, and its positions fit the list word");
+__device__ __forceinline__ uint32_t bkl_word(uint32_t pos, uint32_t local_key) { return pos << BKL_KEY_BITS | local_key; }
 
 template <class K>
 __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_hist(const K *__restrict__ keys, const uint32_t *__restrict__ n_ptr, uint32_t n_host,
@@ -1260,18 +1273,21 @@ static __global__ void __launch_bounds__(OSW_THREADS) k_wide_tile_bases(const ui
 //   3. a sweep over the laid-out cells, consecutive threads on consecutive entries of a cell: ARRIVAL order inside each part (the count
 //      windows need every key's items in stream order, and two items of one key may share a part; every entry of an earlier part is
 //      earlier, every entry of a later part later) -- an entry's place in its part is the number of the part's entries with a smaller
-//      position, two 16-bit compares per 4-byte load as in k_wide_scatter_ranked_tile -- and one write of (slot, position) to the final
-//      place: first output position of the group's cell (C[chunk] + T[group] of k_wide_tile_bases) + the earlier parts + that number.
+//      position, two 16-bit compares per 4-byte load as in k_wide_scatter_ranked_tile -- and one write of the item's list word to the
+//      final place: first output position of the group's cell (C[chunk] + T[group] of k_wide_tile_bases) + the earlier parts + that number.
 // Why groups: a (wide tile, digit) cell holds about 2 items at the bench step (4096 positions, half of them survivors, 1024 digits), so
-// with one wide tile per CTA a warp's store touched about 16 separate 32-byte sectors per array; a group cell of 4 tiles is about 8
-// items, whole sectors (tools/micro/bucket_store.cu replays both patterns). Used when there are enough groups to give every SM one
-// (osr_group in wfb_lib.cu) and no records travel; otherwise k_wide_scatter_ranked_tile below (one wide tile per CTA) runs.
-// Output: keys_out[i] = slot, vals_out[i] = arrival position, stable by (digit, position) -- what k_wide_scatter produces.
+// with one wide tile per CTA a warp's store touched about 16 separate 32-byte sectors; a group cell of 4 tiles is about 8 items, whole
+// sectors (tools/micro/bucket_store.cu replays both patterns). Used when there are enough groups to give every SM one (osr_group in
+// wfb_lib.cu) and no records travel; otherwise k_wide_scatter_ranked_tile below (one wide tile per CTA) runs.
+// Output: list_out[i] = bkl_word(position, slot - first slot of its bucket), stable by (digit, position). `packed` starts at the
+// position range's first position (the positions in the words are relative to it), n < BKL_RANGE_POS. The tile pass wrote no word for
+// an item without a slot (INVALID_SLOT is never counted in a row), and every slot is below the key capacity, 1024 << shift: every item
+// lies inside its bucket's keys.
 // OSR_SMEM = 74 KB of dynamic shared memory: 3 resident CTAs per SM. Positions within a group are < 2^14, slots < 2^16.
 constexpr uint32_t OSR_SMEM = OSR_GROUP_POS * 2u * 2u + OSW_DIGITS * 8u + OSW_DIGITS * 2u;
 static_assert(OSR_GROUP == 4 && OSR_GROUP_POS <= 0x8000u, "one ushort4 of part sizes per digit; 16-bit packed position compare");
-static __global__ void __launch_bounds__(OSW_THREADS, 3) k_wide_scatter_ranked(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
-                                                                            uint32_t *__restrict__ vals_out, uint32_t n, uint32_t shift, uint32_t chunk_shift,
+static __global__ void __launch_bounds__(OSW_THREADS, 3) k_wide_scatter_ranked(const uint32_t *__restrict__ packed, uint32_t *__restrict__ list_out,
+                                                                            uint32_t n, uint32_t shift, uint32_t chunk_shift,
                                                                             uint32_t tiles, const uint16_t *__restrict__ H, const uint32_t *__restrict__ Cx,
                                                                             const uint32_t *__restrict__ T)
 {
@@ -1355,8 +1371,7 @@ static __global__ void __launch_bounds__(OSW_THREADS, 3) k_wide_scatter_ranked(c
         for (; j + 1 < end; j += 2) less += __popc((mm - *reinterpret_cast<const uint32_t *>(lpos + j)) & 0x80008000u);
         if (j < end) less += lpos[j] < mine ? 1u : 0u;
         const uint32_t dst = __ldg(cbase + d) + __ldg(tbase + d) + before + less;
-        keys_out[dst] = slot;
-        vals_out[dst] = start + mine;
+        list_out[dst] = bkl_word(start + mine, slot - (d << shift));
     }
 }
 
@@ -1367,12 +1382,13 @@ static __global__ void __launch_bounds__(OSW_THREADS, 3) k_wide_scatter_ranked(c
 //   2. every item files its position within the tile at cell start + rank -- no ranking rounds, no per-warp counters,
 //   3. a sweep over the laid-out cells, consecutive threads on consecutive entries of a cell: ARRIVAL order inside the cell (the count
 //      windows need every key's items in stream order, and two items of one key may share a cell) -- an entry's place is the number of
-//      the cell's entries with a smaller position -- and one write of (slot, position) to the final place. The stores of a warp land in
-//      the few cells it sweeps, and no per-thread array outlives a loop (nothing is indexed at run time: no local memory).
-// Output: keys_out[i] = slot, vals_out[i] = arrival position, stable by (digit, position) -- what k_wide_scatter produces.
-// RBYTES != 0: the records travel as well (payload_in at the arrival positions -> payload_out at the final places; vals_out may be
-// null): the source side of the bucketed multi-GPU exchange, and WFB_BUCKET_MOVE=1, whose update reads the arrival position of a
-// group's triggering item from vals_out.
+//      the cell's entries with a smaller position -- and one write to the final place. The stores of a warp land in the few cells it
+//      sweeps, and no per-thread array outlives a loop (nothing is indexed at run time: no local memory).
+// Output, stable by (digit, position): list != 0, keys_out[i] = the item's bucket-list word (bkl_word, as k_wide_scatter_ranked); list
+// = 0 (RBYTES != 0 only), keys_out[i] = slot.
+// RBYTES != 0: the records travel as well (payload_in at the arrival positions -> payload_out at the final places): the source side of
+// the bucketed multi-GPU exchange (list = 0: the destination splits its coarse buckets by slot), and WFB_BUCKET_MOVE=1 (list = 1: the
+// record index is the list index, and the word's position is the arrival position the update needs for a group's triggering item).
 // 34 KB of shared memory and at most 40 registers: 6 resident CTAs per SM, so the 2048 wide tiles of the bench step take 2.6 waves
 // on 132 SMs.
 #ifndef WFB_OSR_MINBLOCKS
@@ -1380,7 +1396,7 @@ static __global__ void __launch_bounds__(OSW_THREADS, 3) k_wide_scatter_ranked(c
 #endif
 template <int RBYTES>
 static __global__ void __launch_bounds__(OSW_THREADS, WFB_OSR_MINBLOCKS) k_wide_scatter_ranked_tile(const uint32_t *__restrict__ packed, uint32_t *__restrict__ keys_out,
-                                                                            uint32_t *__restrict__ vals_out, uint32_t n, uint32_t shift, uint32_t chunk_shift,
+                                                                            uint32_t list, uint32_t n, uint32_t shift, uint32_t chunk_shift,
                                                                             const uint16_t *__restrict__ H, const uint32_t *__restrict__ Cx, const uint32_t *__restrict__ T,
                                                                             const unsigned char *__restrict__ payload_in, unsigned char *__restrict__ payload_out)
 {
@@ -1447,8 +1463,7 @@ static __global__ void __launch_bounds__(OSW_THREADS, WFB_OSR_MINBLOCKS) k_wide_
         uint32_t less = 0;
         for (uint32_t j = 0; j < cnt; j += 2) less += __popc((mm - cell[j >> 1]) & 0x80008000u);
         const uint32_t dst = bin_base[d] + less;
-        keys_out[dst] = slot;
-        if (RBYTES == 0 || vals_out != nullptr) vals_out[dst] = start + mine;
+        keys_out[dst] = (RBYTES == 0 || list) ? bkl_word(start + mine, slot - (d << shift)) : slot;
         if constexpr (RBYTES != 0) {
             static_assert(RBYTES % 8 == 0, "record size");
             using W = typename std::conditional<RBYTES % 16 == 0, uint4, uint2>::type;
@@ -1481,9 +1496,18 @@ static __global__ void k_shard_bin_counts(const uint32_t *__restrict__ bin_count
 // source's 1024 bins are shared by all destinations), a run of cnt[s][b] records in arrival order -- the runs of one source back to
 // back from recv position off[s]. The update kernel wants all 1024 CTAs busy, so every coarse bucket is split into nsub = 1024 / bps
 // sub-buckets by slot: the items of sub-bucket (b, j) are, source after source (= global stream order), the items of run (s, b) whose
-// slot falls into j, in arrival order. Three small kernels write them as the (slot, position) lists + sizes k_ffat_update_buckets
-// consumes: count per (b, j, s) | exclusive scan in that order | stable split of every run.
+// slot falls into j, in arrival order. Three small kernels write them as the bucket list + sizes k_ffat_update_buckets consumes:
+// count per (b, j, s) | exclusive scan in that order | stable split of every run. A record's index is its receive position, and the
+// kernels see only the items of one range of receive positions [lo, hi) (hi - lo <= BKL_RANGE_POS; the list words hold positions
+// relative to lo). Sources' regions lie in source order and a key's run inside a region is in arrival order, so every key's items
+// are in increasing receive position: consecutive ranges are consecutive parts of every key's stream.
 struct MgRuns { uint32_t off[MAX_SHARDS + 1]; };
+// the items [*i0, *i1) of a run of m items from receive position p0 that lie in [lo, hi)
+__device__ __forceinline__ void mg_clip(uint32_t p0, uint32_t m, uint32_t lo, uint32_t hi, uint32_t *i0, uint32_t *i1)
+{
+    *i0 = min(m, max(p0, lo) - p0);
+    *i1 = min(m, max(p0, hi) - p0);
+}
 constexpr uint32_t MG_THREADS = 256;
 __device__ __forceinline__ uint32_t mg_run_start(const uint32_t *__restrict__ cnt, uint32_t s, uint32_t bps, uint32_t b, uint32_t *sh)
 {   // records of source s in the coarse buckets before b (block-wide sum; sh: 8 words of shared memory)
@@ -1502,7 +1526,7 @@ __device__ __forceinline__ uint32_t mg_run_start(const uint32_t *__restrict__ cn
 static __global__ void __launch_bounds__(MG_THREADS) k_mg_count(const uint32_t *__restrict__ cnt, uint32_t nsrc, uint32_t bps, const MgRuns runs,
                                                                 const uint32_t *__restrict__ recv_slots, uint32_t slot_mask, uint32_t shift2, uint32_t nsub,
                                                                 uint32_t *__restrict__ cnt3, uint32_t *__restrict__ run_starts,
-                                                                uint32_t *__restrict__ n_trig, uint32_t *__restrict__ n_heavy)
+                                                                uint32_t *__restrict__ n_trig, uint32_t *__restrict__ n_heavy, uint32_t lo, uint32_t hi)
 {
     __shared__ uint32_t sh[8], c[MAX_SHARDS];
     const uint32_t b = blockIdx.x, s = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
@@ -1511,9 +1535,11 @@ static __global__ void __launch_bounds__(MG_THREADS) k_mg_count(const uint32_t *
     const uint32_t rs = mg_run_start(cnt, s, bps, b, sh), m = cnt[s * bps + b];
     if (tid == 0) run_starts[s * bps + b] = rs;
     const uint32_t *sl = recv_slots + runs.off[s] + rs;
-    for (uint32_t i0 = 0; i0 < m; i0 += MG_THREADS) {
+    uint32_t ib, ie;
+    mg_clip(runs.off[s] + rs, m, lo, hi, &ib, &ie);
+    for (uint32_t i0 = ib; i0 < ie; i0 += MG_THREADS) {
         const uint32_t i = i0 + tid;
-        const uint32_t j = i < m ? ((sl[i] & slot_mask) >> shift2) & (nsub - 1u) : nsub;
+        const uint32_t j = i < ie ? ((sl[i] & slot_mask) >> shift2) & (nsub - 1u) : nsub;
         for (uint32_t jj = 0; jj < nsub; jj++) { const uint32_t bal = __ballot_sync(FULL, j == jj); if (lane == 0 && bal) atomicAdd(&c[jj], __popc(bal)); }
     }
     __syncthreads();
@@ -1549,27 +1575,29 @@ static __global__ void __launch_bounds__(1024) k_mg_scan(const uint32_t *__restr
 static __global__ void __launch_bounds__(MG_THREADS) k_mg_split(const uint32_t *__restrict__ cnt, uint32_t nsrc, uint32_t bps, const MgRuns runs,
                                                                 const uint32_t *__restrict__ recv_slots, uint32_t slot_mask, uint32_t shift2, uint32_t nsub,
                                                                 const uint32_t *__restrict__ off3, const uint32_t *__restrict__ run_starts,
-                                                                uint32_t *__restrict__ out_slots, uint32_t *__restrict__ out_pos)
+                                                                uint32_t *__restrict__ out_list, uint32_t lo, uint32_t hi)
 {
     __shared__ uint32_t wc[MG_THREADS / 32][MAX_SHARDS], fill[MAX_SHARDS];
     const uint32_t b = blockIdx.x, s = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t m = cnt[s * bps + b], src0 = runs.off[s] + run_starts[s * bps + b];
+    uint32_t ib, ie;
+    mg_clip(src0, m, lo, hi, &ib, &ie);
     if (tid < nsub) fill[tid] = off3[(b * nsub + tid) * nsrc + s];
     __syncthreads();
-    for (uint32_t i0 = 0; i0 < m; i0 += MG_THREADS) {
+    for (uint32_t i0 = ib; i0 < ie; i0 += MG_THREADS) {
         const uint32_t i = i0 + tid;
         uint32_t slot = 0, j = nsub, before = 0;
-        if (i < m) { slot = recv_slots[src0 + i] & slot_mask; j = (slot >> shift2) & (nsub - 1u); }
+        if (i < ie) { slot = recv_slots[src0 + i] & slot_mask; j = (slot >> shift2) & (nsub - 1u); }
         for (uint32_t jj = 0; jj < nsub; jj++) {
             const uint32_t bal = __ballot_sync(FULL, j == jj);
             if (lane == 0) wc[warp][jj] = __popc(bal);
             if (j == jj) before = __popc(bal & lanemask_lt());
         }
         __syncthreads();
-        if (i < m) {
+        if (i < ie) { // (slot >> shift2 is the update's bucket: the local key is the slot's low shift2 bits)
             uint32_t dst = fill[j] + before;
             for (uint32_t w = 0; w < warp; w++) dst += wc[w][j];
-            out_slots[dst] = slot; out_pos[dst] = src0 + i;
+            out_list[dst] = bkl_word(src0 + i - lo, slot & ((1u << shift2) - 1u));
         }
         __syncthreads();
         if (tid < nsub) { uint32_t t = 0; for (uint32_t w = 0; w < MG_THREADS / 32; w++) t += wc[w][tid]; fill[tid] += t; }
@@ -1937,9 +1965,10 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
 }
 
 // ------------------------------------------------------------------------------------------------------
-// k_ffat_update_buckets: the window update after ONE wide partition pass (k_wide_scatter) on the top 10 bits of the
-// slot. The pass leaves the segment's (slot, arrival position) pairs in 1024 buckets of at most BK_KEYS consecutive
-// slots, arrival order inside a bucket. One CTA per bucket. The kernel's time is the random gather of the records and the
+// k_ffat_update_buckets: the window update after ONE wide partition pass (k_wide_scatter_ranked) on the top 10 bits of the
+// slot. The pass leaves the bucket list of a position range -- one word per item, its position in the range and its key within
+// the bucket (bkl_word) -- in 1024 buckets of at most BK_KEYS consecutive slots, arrival order inside a bucket. One CTA per
+// bucket. The kernel's time is the random gather of the records and the
 // dependent round trips in front of it, so every phase issues all of its global loads before it uses the first one:
 //   0. the bucket's range (scan of the pass histogram), the keys' state, and the items of every key in the whole bucket
 //      (BK_CNT_U independent loads of the bucket list per thread and round trip): the deferral of fired groups needs them,
@@ -1961,7 +1990,8 @@ __global__ void __launch_bounds__(128) k_ffat_update_lanes(const FfatDev ff, con
 // Per-key bookkeeping (count, position in the open pane, next leaf, next trigger, open-pane accumulator) is computed
 // once per CTA by one thread per key and lives in shared memory across the chunks.
 // `moved` = 1: the partition pass also moved the records (bucket b's records are lifted[boff[b] ..)); 0: records are
-// gathered through the arrival positions.
+// gathered through the positions, and `lifted` points at the range's first record. pos_base = the range's first position: a
+// triggering item's position in the call is pos_base + the position in its word.
 // ------------------------------------------------------------------------------------------------------
 #ifdef WFB_BK_TRACE
 // debug build only, per CTA: start time, time thread 0 spent in phases 1..6 (summed over the chunks), end time (globaltimer ns)
@@ -1993,6 +2023,8 @@ template <uint32_t RB, bool LAZY>
 constexpr uint32_t bk_smem_bytes()
 {
     constexpr uint32_t IT = bk_items_per_thread<RB>(), CAP = BK_THREADS * IT, CS = IT * (BK_THREADS / 32) + 2;
+    // (CAP * 4 bytes of the sum are not used since the bucket list is one word per item: kept, so that results above 160 bytes keep
+    // the full-sort path)
     return CAP * RB + 3 * CAP * 4 + BK_KEYS * CS * 2 + 5 * BK_KEYS * 4 + 3 * BK_KEYS * 8 + BK_KEYS * RB
          + (LAZY ? 16 : BK_KEYS * bk_sibl_levels<RB>() * RB) + 2 * BK_KEYS * 4 + BK_THREADS * 4 + (BK_THREADS / 32 + 5) * 4 + 64;
 }
@@ -2009,7 +2041,7 @@ constexpr bool bk_fits() { return bk_smem_bytes<RB, false>() <= (48u << 10) && b
 
 template <class P, bool LAZY>
 __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB_BK_MINBLOCKS) k_ffat_update_buckets(const FfatDev ff, const unsigned char *__restrict__ lifted,
-                                                                       const uint32_t *__restrict__ bk_slots, const uint32_t *__restrict__ bk_pos,
+                                                                       const uint32_t *__restrict__ bk_list, uint32_t pos_base,
                                                                        const uint32_t *__restrict__ digit_counts, uint32_t shift, uint32_t moved,
                                                                        const uint32_t *__restrict__ batch_off, const DevBatch *__restrict__ batches,
                                                                        uint32_t nbatches, unsigned char *__restrict__ out_res,
@@ -2026,11 +2058,11 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
     constexpr uint32_t CS = NCOL + 2;                                  // row stride of the split counts (odd in words: no bank conflicts)
     constexpr uint32_t CPB = (RB % 16 == 0) ? 16 : 8;                  // cp.async granule of a record
     constexpr uint32_t BK_SIBL = bk_sibl_levels<RB>();                 // FlatFAT levels whose siblings are staged in shared memory
-    static_assert(DPT % 4 == 0 && BK_KEYS == 64 && BK_THREADS == 128 && RB % 8 == 0, "layout");
+    static_assert(DPT % 4 == 0 && BK_KEYS == 64 && BK_KEYS == (1u << BKL_KEY_BITS) && BK_THREADS == 128 && RB % 8 == 0, "layout");
     static_assert(bk_fits<RB>(), "the arrays below exceed 48 KB of static shared memory (bk_smem_bytes)");
     __shared__ __align__(16) unsigned char s_rec[CAP * RB]; // the chunk's records, key-major; a segment's fold replaces its first record
     __shared__ uint32_t s_idx[CAP];                    // record index of the items (into `lifted`), key-major
-    __shared__ uint32_t s_lslot[CAP], s_lpos[CAP];     // the bucket list of the next chunk (slots, arrival positions), prefetched
+    __shared__ uint32_t s_list[CAP];                   // the bucket list of the next chunk, prefetched
     __shared__ __align__(16) uint16_t s_col[BK_KEYS][CS]; // items of key k in (round, warp) column c -> exclusive over the columns
     __shared__ uint32_t kcnt[BK_KEYS], koff[BK_KEYS];  // items / first index of key k in this chunk
     __shared__ uint32_t kleft[BK_KEYS];                // items of key k still to come in this segment
@@ -2090,16 +2122,13 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
         __syncthreads();
     }
     const uint32_t bbeg = s_boff[0], bend = s_boff[1];
-    // the bucket list of the chunk at `at` -> s_lslot / s_lpos, asynchronously. Item r * BK_THREADS + tid is copied and later read by
-    // thread tid alone: its own cp.async.wait_all makes it visible, no barrier is needed.
+    // the bucket list of the chunk at `at` -> s_list, asynchronously. Item r * BK_THREADS + tid is copied and later read by thread
+    // tid alone: its own cp.async.wait_all makes it visible, no barrier is needed.
     const auto fetch_list = [&](uint32_t at, uint32_t end) {
 #pragma unroll
         for (uint32_t r = 0; r < IT; r++) {
             const uint32_t i = r * BK_THREADS + tid;
-            if (at + i < end) {
-                cp_async<4>(s_lslot + i, bk_slots + at + i);
-                if (!moved) cp_async<4>(s_lpos + i, bk_pos + at + i);
-            }
+            if (at + i < end) cp_async<4>(s_list + i, bk_list + at + i);
         }
     };
     fetch_list(bbeg, bend); // the first chunk's list: in flight during the key counts
@@ -2111,10 +2140,10 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
 #pragma unroll
         for (uint32_t q = 0; q < BK_CNT_U; q++) {
             const uint32_t i = base + q * BK_THREADS + tid;
-            lk[q] = i < bend ? bk_slots[i] - key_lo : 0xffffffffu;
+            lk[q] = i < bend ? bk_list[i] & (BK_KEYS - 1u) : BK_KEYS;
         }
 #pragma unroll
-        for (uint32_t q = 0; q < BK_CNT_U; q++) if (lk[q] < kpc) atomicAdd(&kleft[lk[q]], 1u);
+        for (uint32_t q = 0; q < BK_CNT_U; q++) if (lk[q] < BK_KEYS) atomicAdd(&kleft[lk[q]], 1u);
     }
     __syncthreads();
     if (tid < BK_KEYS) {
@@ -2147,9 +2176,9 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
             const uint32_t i = r * BK_THREADS + tid;
             ek[r] = BK_KEYS; ep[r] = cursor + i;
             if (i < nsel) {
-                const uint32_t lk = s_lslot[i] - key_lo; // slots outside the bucket's keys (invalid slots) are dropped
-                if (!moved) ep[r] = s_lpos[i];           // records still in arrival order: the index is the position
-                if (lk < kpc) ek[r] = lk;
+                const uint32_t w = s_list[i];              // (every producer writes items of the bucket's keys only)
+                if (!moved) ep[r] = w >> BKL_KEY_BITS;     // records still in arrival order: the index is the position
+                ek[r] = w & (BK_KEYS - 1u);
             }
         }
         {
@@ -2312,7 +2341,7 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                         sib_staged = false; // the next pane of the same run reads the tree it has just written
                         if (consumed == tt) {
                             const uint32_t lp = s_idx[koff[k] + consumed - 1];
-                            const uint32_t last_pos = moved ? bk_pos[lp] : lp; // arrival position of the triggering item
+                            const uint32_t last_pos = pos_base + (moved ? bk_list[lp] >> BKL_KEY_BITS : lp); // arrival position of the triggering item
                             const uint32_t obase = atomicAdd(n_out, ff.nb);
                             bool deferred = (kleft[k] - consumed) < ff.defer_items; // the panes this key still completes in this segment fit the spare ring leaves
                             if (deferred) {
@@ -2394,7 +2423,8 @@ __global__ void __launch_bounds__(BK_THREADS, LAZY ? WFB_BK_MINBLOCKS_LAZY : WFB
                             }
                             __syncwarp();
                             if (tt == 0) {
-                                const uint32_t last_pos = moved ? bk_pos[s_idx[off + j + hi - 1]] : s_idx[off + j + hi - 1]; // arrival position of the triggering item
+                                const uint32_t lp = s_idx[off + j + hi - 1];
+                                const uint32_t last_pos = pos_base + (moved ? bk_list[lp] >> BKL_KEY_BITS : lp); // arrival position of the triggering item
                                 uint32_t obase = 0;
                                 if (lane == 0) obase = atomicAdd(n_out, ff.nb);
                                 obase = __shfl_sync(FULL, obase, 0);

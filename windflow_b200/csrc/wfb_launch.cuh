@@ -66,7 +66,7 @@ struct ProgramOps {
     int (*ffat_update)(const FfatDev &ff, const unsigned char *lifted, const uint32_t *sorted_pos, const uint32_t *batch_off,
                        const DevBatch *batches, uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts,
                        uint32_t out_cap, uint32_t *n_out, uint32_t grid, cudaStream_t s, const void *params, uint32_t lanes_grid);
-    int (*ffat_buckets)(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_slots, const uint32_t *bk_pos,
+    int (*ffat_buckets)(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_list, uint32_t pos_base,
                         const uint32_t *digit_counts, uint32_t shift, uint32_t moved, const uint32_t *batch_off, const DevBatch *batches,
                         uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts, uint32_t out_cap, uint32_t *n_out, cudaStream_t s,
                         const void *params);
@@ -189,14 +189,14 @@ int ffat_update_dispatch(const FfatDev &ff, const unsigned char *lifted, const u
 }
 
 template <class P>
-int ffat_buckets_dispatch(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_slots, const uint32_t *bk_pos,
+int ffat_buckets_dispatch(const FfatDev &ff, const unsigned char *lifted, const uint32_t *bk_list, uint32_t pos_base,
                           const uint32_t *digit_counts, uint32_t shift, uint32_t moved, const uint32_t *batch_off, const DevBatch *batches,
                           uint32_t nbatches, unsigned char *out_res, uint64_t *out_ts, uint32_t out_cap, uint32_t *n_out, cudaStream_t s,
                           const void *params)
 {
-    if (ff.lazy) k_ffat_update_buckets<P, true><<<OSW_DIGITS, BK_THREADS, 0, s>>>(ff, lifted, bk_slots, bk_pos, digit_counts, shift, moved, batch_off, batches,
+    if (ff.lazy) k_ffat_update_buckets<P, true><<<OSW_DIGITS, BK_THREADS, 0, s>>>(ff, lifted, bk_list, pos_base, digit_counts, shift, moved, batch_off, batches,
                                                                                  nbatches, out_res, out_ts, out_cap, n_out, load_params<P>(params));
-    else k_ffat_update_buckets<P, false><<<OSW_DIGITS, BK_THREADS, 0, s>>>(ff, lifted, bk_slots, bk_pos, digit_counts, shift, moved, batch_off, batches,
+    else k_ffat_update_buckets<P, false><<<OSW_DIGITS, BK_THREADS, 0, s>>>(ff, lifted, bk_list, pos_base, digit_counts, shift, moved, batch_off, batches,
                                                                           nbatches, out_res, out_ts, out_cap, n_out, load_params<P>(params));
     WFB_CK(cudaGetLastError());
     return 0;

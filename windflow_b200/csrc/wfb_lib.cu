@@ -208,11 +208,14 @@ struct RadixSorter {
     // ready_ctl: the producer of the keys (the tile pass) cleared it and filed the 16-bit rows of the wide tiles (TileArgs::wide_h16) --
     // in h16_rows when they do not live in this sorter (a pipelined handle keeps one set per segment in flight) -- and, without few_bins,
     // packed a rank with every key (TileArgs::pack_rank), by which k_wide_scatter_ranked places them. Null: k_wide_tile_hist counts.
+    // list (ranked only): kout receives the bucket list of k_ffat_update_buckets (bkl_word; kin starts at the first position of a
+    // range of fewer than BKL_RANGE_POS positions) instead of the slots; vout is not written. Without records travelling the ranked
+    // pass writes the bucket list only.
     template <class K>
     int sort_wide(const K *kin, K *kout, uint32_t *vout, const uint32_t *n_ptr, uint32_t n_host, uint32_t cap, uint32_t shift,
                   cudaStream_t s, uint32_t *ready_ctl, const uint32_t **counts, const unsigned char *payload_in = nullptr,
                   unsigned char *payload_out = nullptr, uint32_t payload_bytes = 0, bool skip_invalid = false, uint32_t region_stride = 0, uint32_t few_bins = 0,
-                  const uint16_t *h16_rows = nullptr)
+                  const uint16_t *h16_rows = nullptr, bool list = false)
     {
         if (payload_in && (payload_bytes == 0 || (payload_bytes & 7u))) return WFB_E_BADARG;
         CK(ctl.ensure(CTL_WORDS));
@@ -251,14 +254,14 @@ struct RadixSorter {
             }
         }
         if (ranked) {
-            if (sizeof(K) != 4 || !kout || (payload_in ? !payload_out || region_stride : !vout)) return WFB_E_UNSUPPORTED;
+            if (sizeof(K) != 4 || !kout || (payload_in ? !payload_out || region_stride : !list) || (list && n_host > BKL_RANGE_POS)) return WFB_E_UNSUPPORTED;
             if (!payload_in && osr_group(tiles, false) == OSR_GROUP) {
                 CK(osr_smem_attr());
                 k_wide_scatter_ranked<<<(tiles + OSR_GROUP - 1) / OSR_GROUP, OSW_THREADS, OSR_SMEM, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout),
-                                                                                                       vout, n_host, shift, chunk_shift, tiles, rows, wideC, wideT);
+                                                                                                       n_host, shift, chunk_shift, tiles, rows, wideC, wideT);
             }
-#define WFB_WSRT(RB_) k_wide_scatter_ranked_tile<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), vout, n_host, shift, \
-                                                                                  chunk_shift, rows, wideC, wideT, payload_in, payload_out)
+#define WFB_WSRT(RB_) k_wide_scatter_ranked_tile<RB_><<<tiles, OSW_THREADS, 0, s>>>(reinterpret_cast<const uint32_t *>(kin), reinterpret_cast<uint32_t *>(kout), list ? 1u : 0u, \
+                                                                                  n_host, shift, chunk_shift, rows, wideC, wideT, payload_in, payload_out)
             else if (!payload_in) WFB_WSRT(0);
             else switch (payload_bytes) { // the records travel with their slots (bucketed exchange)
                 case 16: WFB_WSRT(16); break; case 24: WFB_WSRT(24); break; case 32: WFB_WSRT(32); break; case 48: WFB_WSRT(48); break; case 64: WFB_WSRT(64); break;
@@ -482,7 +485,8 @@ struct wfb_engine {
 // per-segment scratch of one Ffat_Windows_GPU; two sets when the handle is pipelined (the ingest pass of segment k+1
 // overlaps sort + update of segment k)
 struct SegScratch {
-    Scratch<uint32_t> slotsA, slotsB, posA, posB; // the segment's capacity in records: slotsA's
+    Scratch<uint32_t> slotsA, slotsB, posA, posB; // the segment's capacity in records: slotsA's. Bucket path: slotsB holds the bucket
+                                                  // list (posA / posB are the full sort's and stay unallocated)
     Scratch<unsigned char> lifted, lifted_sorted;
     Scratch<uint32_t> batch_off; Scratch<DevBatch> d_batches;
     uint32_t *n_total = nullptr;
@@ -1551,7 +1555,8 @@ static int ffat_ensure_segment(wfb_ffat *h, SegScratch &g, uint32_t total, uint3
     const ScratchWaits w = h->s2 ? ScratchWaits(s, h->s2) : ScratchWaits(s);
     CK(g.slotsA.ensure(total, w));
     const size_t cap = g.slotsA.capacity(), RB = h->ops->result_bytes;
-    CK(g.slotsB.ensure(total, w, cap)); CK(g.posA.ensure(total, w, cap)); CK(g.posB.ensure(total, w, cap));
+    CK(g.slotsB.ensure(total, w, cap));
+    if (!h->buckets) { CK(g.posA.ensure(total, w, cap)); CK(g.posB.ensure(total, w, cap)); }
     CK(g.lifted.ensure(RB * total, w, RB * cap));
     if (h->bucket_move) CK(g.lifted_sorted.ensure(RB * total, w, RB * cap));
     // the window groups the segment can fire, for the current key capacity (key growth raises it before the pass runs again)
@@ -1566,6 +1571,10 @@ static int ffat_ensure_segment(wfb_ffat *h, SegScratch &g, uint32_t total, uint3
     return 0;
 }
 
+// the last kernel of a call adds *n_out to results_total: a call (or position range) whose results follow the ones already in the
+// output buffer takes those out of the total first
+__global__ void k_results_pre_append(unsigned long long *results_total, const uint32_t *n_out) { if (results_total) *results_total -= *n_out; }
+
 // sort + update + deferred window queries of the segment held in `g`, results to (out, out_ts, n_out)
 static int ffat_window_phase(wfb_ffat *h, SegScratch &g, const FfatDev &ff, unsigned char *out, uint64_t *out_ts, uint32_t out_cap,
                              uint32_t *n_out, cudaStream_t s)
@@ -1574,20 +1583,40 @@ static int ffat_window_phase(wfb_ffat *h, SegScratch &g, const FfatDev &ff, unsi
     const uint64_t before = h->sorter.launches;
     int rc;
     if (h->buckets) {
-        // ONE wide radix pass on the top 10 slot bits: 1024 buckets of consecutive keys, arrival order inside a bucket ...
-        const uint32_t *counts = nullptr;
-        rc = h->sorter.sort_wide<uint32_t>(g.slotsA, g.slotsB, g.posB, nullptr, g.total, g.total, h->bucket_shift, s, g.sort_ctl, &counts,
-                                           h->bucket_move ? static_cast<unsigned char *>(g.lifted) : nullptr,
-                                           h->bucket_move ? static_cast<unsigned char *>(g.lifted_sorted) : nullptr,
-                                           static_cast<uint32_t>(h->ops->result_bytes), true, 0, 0, h->pipelined ? static_cast<uint16_t *>(g.h16) : nullptr);
-        if (rc) return rc;
-        h->launches += h->sorter.launches - before;
-        h->mark(2, s);
-        // ... then one CTA per bucket finishes the job (local split by key, per-key ordered fold, FlatFAT update)
-        rc = h->ops->ffat_buckets(ff, h->bucket_move ? g.lifted_sorted : g.lifted_src, g.slotsB, g.posB, counts, h->bucket_shift, h->bucket_move ? 1u : 0u, g.batch_off, g.d_batches, g.nbatches, out, out_ts,
-                                  out_cap, n_out, s, h->pp());
-        if (rc) return rc;
-        h->launches += 1;
+        // The bucket list holds positions below BKL_RANGE_POS: a segment of more positions is partitioned, updated and queried one range
+        // of BKL_RANGE_POS positions (whole wide tiles) at a time. The ranges are consecutive in arrival order, so every key's state
+        // carries over from one range to the next as it does from call to call, and the windows a range fires are evaluated before
+        // the next range writes leaves. Results of all ranges are appended to `out`.
+        const size_t RB = h->ops->result_bytes;
+        const uint16_t *rows = h->pipelined ? static_cast<const uint16_t *>(g.h16) : static_cast<const uint16_t *>(h->sorter.wideH);
+        for (uint32_t base = 0; base < g.total; base += BKL_RANGE_POS) {
+            const uint32_t n = std::min(BKL_RANGE_POS, g.total - base);
+            if (base != 0) { // (the first range's trigger list: cleared by the tile pass)
+                CK(cudaMemsetAsync(g.n_trig, 0, sizeof(uint32_t), s));
+                k_results_pre_append<<<1, 1, 0, s>>>(ff.results_total, n_out);
+                CK(cudaGetLastError());
+                h->launches++;
+            }
+            // ONE wide radix pass on the top 10 slot bits: 1024 buckets of consecutive keys, arrival order inside a bucket ...
+            const uint32_t *counts = nullptr;
+            const uint64_t before_r = h->sorter.launches;
+            rc = h->sorter.sort_wide<uint32_t>(g.slotsA + base, g.slotsB, nullptr, nullptr, n, n, h->bucket_shift, s, g.sort_ctl, &counts,
+                                               h->bucket_move ? static_cast<unsigned char *>(g.lifted) + base * RB : nullptr,
+                                               h->bucket_move ? static_cast<unsigned char *>(g.lifted_sorted) : nullptr,
+                                               static_cast<uint32_t>(RB), true, 0, 0, rows + static_cast<size_t>(base / OSW_TILE) * OSW_DIGITS, true);
+            if (rc) return rc;
+            h->launches += h->sorter.launches - before_r;
+            h->mark(2, s);
+            // ... then one CTA per bucket finishes the job (local split by key, per-key ordered fold, FlatFAT update)
+            rc = h->ops->ffat_buckets(ff, h->bucket_move ? static_cast<const unsigned char *>(g.lifted_sorted) : g.lifted_src + base * RB, g.slotsB, base, counts,
+                                      h->bucket_shift, h->bucket_move ? 1u : 0u, g.batch_off, g.d_batches, g.nbatches, out, out_ts, out_cap, n_out, s, h->pp());
+            if (rc) return rc;
+            // deferred window groups: one thread per window
+            rc = h->ops->ffat_windows(ff, g.batch_off, g.d_batches, g.nbatches, out, out_ts, out_cap, static_cast<uint32_t>(g_num_sms) * 4u, s, h->pp(), n_out);
+            if (rc) return rc;
+            h->launches += 2;
+        }
+        return 0;
     } else {
         // stable sort of (slot, arrival position) by slot: onesweep radix, 8 bits per pass
         rc = h->sorter.sort<uint32_t>(g.slotsA, g.slotsB, g.posA, g.posB, g.n_total, 0, g.total, h->sort_passes, s, &sorted_slots,
@@ -1807,19 +1836,26 @@ static int ffat_process_prebucketed(wfb_ffat *h, const unsigned char *records, c
     CK(h->mg_scratch.ensure(3 * OSW_DIGITS * MAX_SHARDS));
     uint32_t *cnt3 = h->mg_scratch, *off3 = cnt3 + OSW_DIGITS * MAX_SHARDS, *run_starts = off3 + OSW_DIGITS * MAX_SHARDS;
     const dim3 grid(bps, nsrc);
-    k_mg_count<<<grid, MG_THREADS, 0, s>>>(bins, nsrc, bps, runs, recv_slots, slot_mask, shift2, nsub, cnt3, run_starts, g.n_trig, g.n_heavy);
-    k_mg_scan<<<1, 1024, 0, s>>>(cnt3, bps * nsub * nsrc, nsrc, off3, g.sort_ctl);
-    k_mg_split<<<grid, MG_THREADS, 0, s>>>(bins, nsrc, bps, runs, recv_slots, slot_mask, shift2, nsub, off3, run_starts, g.slotsB, g.posB);
-    CK(cudaGetLastError());
-    h->mark(2, s);
-    rc = h->ops->ffat_buckets(ff, records, g.slotsB, g.posB, g.sort_ctl, shift2, 0u, g.batch_off, g.d_batches, nsrc, static_cast<unsigned char *>(out_results), out_ts,
-                              out_capacity, n_out_dev, s, h->pp());
-    if (rc) return rc;
-    rc = h->ops->ffat_windows(ff, g.batch_off, g.d_batches, nsrc, static_cast<unsigned char *>(out_results), out_ts, out_capacity, static_cast<uint32_t>(g_num_sms) * 4u, s,
-                              h->pp(), n_out_dev);
-    if (rc) return rc;
+    // a record's index is its receive position, and the bucket list holds positions below BKL_RANGE_POS: ranges of receive positions,
+    // each split, updated and queried before the next (every key's items are in increasing receive position: k_mg_split)
+    const uint64_t npos = offs_h[nsrc];
+    for (uint64_t lo = 0; lo < npos; lo += BKL_RANGE_POS) {
+        const uint32_t lo32 = static_cast<uint32_t>(lo), hi32 = static_cast<uint32_t>(std::min<uint64_t>(npos, lo + BKL_RANGE_POS));
+        if (lo != 0) { k_results_pre_append<<<1, 1, 0, s>>>(ff.results_total, n_out_dev); h->launches++; }
+        k_mg_count<<<grid, MG_THREADS, 0, s>>>(bins, nsrc, bps, runs, recv_slots, slot_mask, shift2, nsub, cnt3, run_starts, g.n_trig, g.n_heavy, lo32, hi32);
+        k_mg_scan<<<1, 1024, 0, s>>>(cnt3, bps * nsub * nsrc, nsrc, off3, g.sort_ctl);
+        k_mg_split<<<grid, MG_THREADS, 0, s>>>(bins, nsrc, bps, runs, recv_slots, slot_mask, shift2, nsub, off3, run_starts, g.slotsB, lo32, hi32);
+        CK(cudaGetLastError());
+        h->mark(2, s);
+        rc = h->ops->ffat_buckets(ff, records + lo * h->ops->result_bytes, g.slotsB, lo32, g.sort_ctl, shift2, 0u, g.batch_off, g.d_batches, nsrc,
+                                  static_cast<unsigned char *>(out_results), out_ts, out_capacity, n_out_dev, s, h->pp());
+        if (rc) return rc;
+        rc = h->ops->ffat_windows(ff, g.batch_off, g.d_batches, nsrc, static_cast<unsigned char *>(out_results), out_ts, out_capacity, static_cast<uint32_t>(g_num_sms) * 4u, s,
+                                  h->pp(), n_out_dev);
+        if (rc) return rc;
+        h->launches += 5;
+    }
     h->mark(3, s);
-    h->launches += 5;
     if (h->timing && h->tev_used < wfb_ffat::TEV_MAX) h->tev_used++;
     h->call_no++;
     return 0;
@@ -1933,7 +1969,6 @@ __global__ void k_mg_meta(const uint32_t *__restrict__ counts, uint64_t watermar
 }
 
 // appended results (wfb_mg_flush): the call about to run adds the WHOLE count of the output buffer to the handle's total
-__global__ void k_mg_pre_append(unsigned long long *results_total, const uint32_t *n_out) { if (results_total) *results_total -= *n_out; }
 
 struct MgSlot { // buffers of one step in flight (three: the exchange of step i-2 overlaps the source pass of step i)
     Scratch<unsigned char> regions;            // records by destination (bucketed: bin after bin, as many as the segment's positions)
@@ -2404,7 +2439,7 @@ static int mg_update(wfb_mg *h, MgSlot &sl, void *out, uint64_t *out_ts, uint32_
     if (h->trace) CK(cudaEventRecord(sl.tr[2], s));
     uint64_t items = 0;
     for (int p = 0; p < n; p++) items += sl.h_recv[2 * p];
-    if (append && items != 0) { k_mg_pre_append<<<1, 1, 0, s>>>(h->ffat->ff.results_total, n_out_dev); CK(cudaGetLastError()); }
+    if (append && items != 0) { k_results_pre_append<<<1, 1, 0, s>>>(h->ffat->ff.results_total, n_out_dev); CK(cudaGetLastError()); }
     int rc;
     if (h->bucketed) {
         rc = ffat_process_prebucketed(h->ffat, sl.recv, sl.recv_slots, sl.recv_bins, static_cast<uint32_t>(n), h->bps, sl.offs, sl.wms, h->shard_slots - 1u, h->shift,
