@@ -209,6 +209,29 @@ struct FacadeFlatMapProgram {
     __host__ __device__ static result_t make_result(key_t, uint64_t, const params_t &) { return result_t(); }
     __host__ __device__ static tuple_t reduce(const tuple_t &a, const tuple_t &, const params_t &) { return a; }
 };
+// The program of a keyed-stateful FlatMap_GPU: func(const tuple_t &, Shipper_GPU<result_t> &, state_t &) in per-key arrival order
+// (nothing runs in front of it: a stateless run before it is materialised, as before the keyed Map / Filter)
+template <class T, class R, class S, class FlatF, class KeyF>
+struct FacadeStatefulFlatMapProgram {
+    using tuple_t = T; using result_t = R; using key_t = key_of_t<KeyF>; using state_t = S;
+    struct params_t { FlatF fm; KeyF key; };
+    static_assert(std::is_trivially_copyable<T>::value && std::is_trivially_copyable<R>::value && std::is_trivially_copyable<S>::value,
+                  "tuple_t / result_t / state_t must be trivially copyable");
+    static_assert(sizeof(T) % 8 == 0 && sizeof(R) % 8 == 0, "tuple_t / result_t sizes must be multiples of 8 bytes");
+    __host__ __device__ static void map(tuple_t &, const params_t &) {}
+    __host__ __device__ static bool filter(tuple_t &, const params_t &) { return true; }
+    __host__ __device__ static key_t key(const tuple_t &t, const params_t &p) { KeyF f = p.key; return f(t); }
+    __host__ __device__ static void lift(const tuple_t &, result_t &, const params_t &) {}
+    __host__ __device__ static void comb(const result_t &, const result_t &, result_t &, const params_t &) {}
+    __host__ __device__ static result_t make_result(key_t, uint64_t, const params_t &) { return result_t(); }
+    __host__ __device__ static tuple_t reduce(const tuple_t &a, const tuple_t &, const params_t &) { return a; }
+    __host__ __device__ static void map_stateful(tuple_t &, state_t &, const params_t &) {}
+    __host__ __device__ static bool filter_stateful(tuple_t &, state_t &, const params_t &) { return true; }
+    __host__ __device__ static void flatmap_stateful(const tuple_t &t, Shipper_GPU<result_t> &sh, state_t &st, const params_t &p)
+    {
+        FlatF f = p.fm; f(t, sh, st);
+    }
+};
 template <class T, class S> struct StatefulIdMap { __host__ __device__ void operator()(T &, S &) const {} };
 template <class T, class S> struct StatefulKeepAll { __host__ __device__ bool operator()(T &, S &) const { return true; } };
 
@@ -673,6 +696,34 @@ template <class F> using Filter_GPU = Stateless_GPU<F, true>;
 template <class shipper_t> struct shipper_result;
 template <class R> struct shipper_result<wfb::Shipper<R>> { using type = R; };
 
+// The drop counts of a FlatMap_GPU replica's calls: every call leaves its count in the word after its batches' sizes, in a block the
+// replica holds until the host has read that word.
+class FlatMapDrops {
+    struct Pending { CountBlock *blk; size_t word; cudaEvent_t ev; };
+    std::vector<Pending> pending; uint64_t dropped = 0; // drop counts of calls the host has not read yet / the sum of those it read
+public:
+    void add(CountBlock *blk, size_t word, cudaEvent_t ev) { pending.push_back(Pending{blk, word, ev}); }
+    // adds the drop counts of finished calls (all of them with `wait`)
+    void read(bool wait)
+    {
+        size_t i = 0;
+        for (; i < pending.size(); i++) {
+            if (wait || pending.size() - i > 8) { gpuErrChk(cudaEventSynchronize(pending[i].ev)); } // (events of the ring are re-recorded after 16 calls)
+            else if (cudaEventQuery(pending[i].ev) != cudaSuccess) { cudaGetLastError(); break; }
+            dropped += pending[i].blk->h[pending[i].word];
+            pending[i].blk->release();
+        }
+        pending.erase(pending.begin(), pending.begin() + static_cast<std::ptrdiff_t>(i));
+    }
+    // end of stream: stops the program when a push was dropped
+    void check(const std::string &op_name, uint32_t max_out)
+    {
+        read(true);
+        if (dropped) wf_fatal("FlatMap_GPU [" + op_name + "]: " + std::to_string(dropped) + " records pushed beyond withMaxOutputsPerTuple(" +
+                              std::to_string(max_out) + ") were dropped");
+    }
+};
+
 template <class tuple_t, class result_t, class func_t>
 class FlatMapReplica: public Basic_Replica {
     using prog_t = FacadeFlatMapProgram<tuple_t, result_t, func_t>;
@@ -681,8 +732,7 @@ class FlatMapReplica: public Basic_Replica {
     uint32_t max_out; size_t maxk;
     DeferredCounts counts; // deferred sizes + the drop count of every call, which this replica reads itself (it holds the block until then)
     BatchPool<result_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-    struct Pending { CountBlock *blk; size_t word; cudaEvent_t ev; };
-    std::vector<Pending> pending; uint64_t dropped = 0; // drop counts of calls the host has not read yet / the sum of those it read
+    FlatMapDrops drops;
     std::vector<batch_t *> in;
     std::vector<wfb_batch_t> bi, bo;
 public:
@@ -715,29 +765,15 @@ public:
     }
     void eosnotify(ssize_t id) override
     {
-        read_drops(true);
-        if (dropped) wf_fatal("FlatMap_GPU [" + opName + "]: " + std::to_string(dropped) + " records pushed beyond withMaxOutputsPerTuple(" +
-                              std::to_string(max_out) + ") were dropped");
+        drops.check(opName, max_out);
         Basic_Replica::eosnotify(id);
     }
 private:
-    // adds the drop counts of finished calls (all of them with `wait`)
-    void read_drops(bool wait)
-    {
-        size_t i = 0;
-        for (; i < pending.size(); i++) {
-            if (wait || pending.size() - i > 8) { gpuErrChk(cudaEventSynchronize(pending[i].ev)); } // (events of the ring are re-recorded after 16 calls)
-            else if (cudaEventQuery(pending[i].ev) != cudaSuccess) { cudaGetLastError(); break; }
-            dropped += pending[i].blk->h[pending[i].word];
-            pending[i].blk->release();
-        }
-        pending.erase(pending.begin(), pending.begin() + static_cast<std::ptrdiff_t>(i));
-    }
     void flush_work(std::vector<batch_t *> &work)
     {
         if (work.empty()) return;
         wait_inputs(work);
-        read_drops(false);
+        drops.read(false);
         const size_t k = work.size();
         bi.resize(k); bo.resize(k);
         std::vector<Batch_GPU_t<result_t> *> outs(k);
@@ -758,7 +794,7 @@ private:
         gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
         cudaEvent_t e = next_event();
         gpuErrChk(cudaEventRecord(e, stream));
-        pending.push_back(Pending{blk, k, e});
+        drops.add(blk, k, e);
         for (size_t i = 0; i < k; i++) {
             Batch_GPU_t<result_t> *o = outs[i];
             o->defer(work[i]->size * max_out, blk, i, e);
@@ -887,6 +923,111 @@ public:
 };
 template <class F, class K> using Map_GPU_KB = Stateful_GPU<F, K, false>;
 template <class F, class K> using Filter_GPU_KB = Stateful_GPU<F, K, true>;
+
+// FlatMap_GPU, keyed-stateful (FlatMap_Builder(f).withKeyBy(k) of wf/flatmap.hpp on the GPU): func(const tuple_t &, Shipper_GPU<result_t> &,
+// state_t &) in per-key arrival order. The key -> state table is shared by the replicas as for the keyed Map / Filter (SharedKState);
+// the outputs and the drop count are those of FlatMap_GPU: input batch i becomes output batch i of capacity original_size * m whose size
+// stays on the device, and a push beyond the m-th of a tuple stops the program at the end of the stream.
+template <class func_t, class keyextr_func_gpu_t>
+class FlatMap_GPU_KB: public Basic_Operator {
+public:
+    using tuple_t = fn_arg_t<func_t, 0>;
+    using result_t = typename shipper_result<fn_arg_t<func_t, 1>>::type;
+    using state_t = fn_arg_t<func_t, 2>;
+    using prog_t = FacadeStatefulFlatMapProgram<tuple_t, result_t, state_t, func_t, keyextr_func_gpu_t>;
+    static constexpr op_type_t op_type = op_type_t::BASIC_GPU;
+    func_t func; keyextr_func_gpu_t key_extr; uint32_t max_keys, max_outputs; size_t maxk = WF_MAX_BATCHES_PER_CALL;
+    bool grow_keys = false; // withKeyGrowth(): max_keys is the initial capacity of the table (WFB_KEYS_GROW)
+    FlatMap_GPU_KB(func_t f, keyextr_func_gpu_t k, size_t p, std::string n, uint32_t mk, uint32_t m)
+        : Basic_Operator(std::move(n), p, Routing_Mode_t::KEYBY, 1), func(f), key_extr(k), max_keys(mk), max_outputs(m)
+    {
+        static_assert(std::is_trivially_copyable<func_t>::value, "GPU functors must be trivially copyable");
+    }
+    std::string getType() const override { return "FlatMap_GPU"; }
+    keyextr_func_gpu_t getKeyExtractor() const { return key_extr; }
+    class Replica: public Basic_Replica {
+        using batch_t = Batch_GPU_t<tuple_t>;
+        std::shared_ptr<SharedKState> ks; typename prog_t::params_t prm; uint32_t max_out; size_t maxk;
+        DeferredCounts counts; // deferred sizes + the drop count of every call
+        BatchPool<result_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
+        FlatMapDrops drops;
+        std::vector<batch_t *> in;
+        std::vector<wfb_batch_t> bi, bo;
+    public:
+        Replica(std::string n, std::shared_ptr<SharedKState> h, func_t f, keyextr_func_gpu_t k, uint32_t m, size_t mk)
+            : Basic_Replica(std::move(n)), ks(std::move(h)), prm{f, k}, max_out(m), maxk(mk ? mk : 1) {}
+        int svc_init() override
+        {
+            Basic_Replica::svc_init();
+            gpuErrChk(counts.init(maxk + 1));
+            return 0;
+        }
+        void *svc(void *msg) override
+        {
+            drain(msg, maxk, in);
+            std::vector<batch_t *> work;
+            for (auto *b : in) {
+                if (!b->isPunct()) { work.push_back(b); continue; }
+                run(work);
+                Batch_GPU_t<result_t> *p = pool.get(1); // (a punctuation of the output type)
+                p->isPunctuation = true; p->size = 0; p->watermarks = b->watermarks;
+                recycleBatch(b);
+                this->ff_send_out(p);
+            }
+            run(work);
+            return this->GO_ON;
+        }
+        void eosnotify(ssize_t id) override
+        {
+            drops.check(opName, max_out);
+            Basic_Replica::eosnotify(id);
+        }
+    private:
+        void run(std::vector<batch_t *> &work)
+        {
+            if (work.empty()) return;
+            wait_inputs(work);
+            drops.read(false);
+            const size_t k = work.size();
+            bi.resize(k); bo.resize(k);
+            std::vector<Batch_GPU_t<result_t> *> outs(k);
+            for (size_t i = 0; i < k; i++) {
+                batch_t *b = work[i];
+                b->getSize();
+                Batch_GPU_t<result_t> *o = pool.get(b->original_size * max_out);
+                o->watermarks = b->watermarks;
+                if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
+                bi[i] = wfb_batch_t{b->tuples_gpu, b->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
+                bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(o->original_size), 0};
+                outs[i] = o;
+            }
+            CountBlock *blk; uint32_t *counts_d;
+            gpuErrChk(counts.acquire(static_cast<uint32_t>(k + 1), blk, counts_d));
+            {   // the replicas of the operator share the state table: one launch sequence at a time
+                std::lock_guard<std::mutex> lock(ks->mu);
+                wfbErrChk(wfb_flatmap_stateful(ks->h, reinterpret_cast<const wfb_functors_t *>(&prm), bi.data(), bo.data(), static_cast<uint32_t>(k),
+                                               max_out, counts_d, stream));
+                gpuErrChk(cudaStreamSynchronize(stream)); // another replica's launches on its own stream must see this call's state
+            }
+            gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
+            cudaEvent_t e = next_event();
+            gpuErrChk(cudaEventRecord(e, stream));
+            drops.add(blk, k, e);
+            for (size_t i = 0; i < k; i++) {
+                outs[i]->defer(work[i]->size * max_out, blk, i, e);
+                work[i]->reuse_after = e; recycleBatch(work[i]);
+                this->ff_send_out(outs[i]);
+            }
+            work.clear();
+        }
+    };
+    std::shared_ptr<SharedKState> kstate;
+    Replica *make_replica()
+    {
+        if (!kstate) { kstate = std::make_shared<SharedKState>(); wfbErrChk(wfb_kstate_create(&kstate->h, wfb::register_program<prog_t>(), max_keys, grow_keys ? WFB_KEYS_GROW : 0u)); }
+        return new Replica(name, kstate, func, key_extr, max_outputs, parallelism > 1 ? 1 : maxk);
+    }
+};
 
 // Reduce_GPU (wf/reduce_gpu.hpp:109-289): per batch, one item per distinct key (ascending) or one item for the batch.
 template <class reduce_func_gpu_t, class keyextr_func_gpu_t>
@@ -1154,25 +1295,60 @@ public:
     }
 };
 
+template <class flatmap_func_gpu_t, class keyextr_func_gpu_t>
+class FlatMapGPU_KB_Builder { // FlatMapGPU_Builder(func).withKeyBy(key_extr): the keyed-stateful operator
+    flatmap_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
+    uint32_t max_outputs;
+public:
+    FlatMapGPU_KB_Builder(flatmap_func_gpu_t f, keyextr_func_gpu_t k, std::string n, size_t p, uint32_t m)
+        : func(f), key(k), name(std::move(n)), parallelism(p), max_outputs(m) {}
+    auto &withName(std::string n) { name = std::move(n); return *this; }
+    auto &withParallelism(size_t p) { parallelism = p; return *this; }
+    auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; } // capacity of the device key -> state table (the initial one withKeyGrowth())
+    auto &withKeyGrowth() { grow = true; return *this; } // extension: the table grows with the keys
+    auto &withMaxOutputsPerTuple(uint32_t m) { max_outputs = m; return *this; } // required: the output batches hold original_size * m records
+    auto build()
+    {
+        if (max_outputs == 0) wf_fatal("FlatMapGPU_Builder [" + name + "]: withMaxOutputsPerTuple(m >= 1) is required");
+        FlatMap_GPU_KB<flatmap_func_gpu_t, keyextr_func_gpu_t> op(func, key, parallelism, name, max_keys, max_outputs);
+        op.grow_keys = grow;
+        return op;
+    }
+};
+
 template <class flatmap_func_gpu_t>
 class FlatMapGPU_Builder {
     flatmap_func_gpu_t func; std::string name = "flatmap_gpu"; size_t parallelism = 1; Routing_Mode_t mode = Routing_Mode_t::FORWARD;
     uint32_t max_outputs = 0;
+    using args_t = typename fn_sig<flatmap_func_gpu_t>::args;
+    static constexpr size_t arity = std::tuple_size<args_t>::value;
 public:
     explicit FlatMapGPU_Builder(flatmap_func_gpu_t f): func(f)
     {
-        static_assert(std::tuple_size<typename fn_sig<flatmap_func_gpu_t>::args>::value == 2 &&
+        static_assert(arity == 3 || (arity == 2 &&
                       std::is_same<fn_ret_t<flatmap_func_gpu_t>, void>::value &&
-                      std::is_same<std::tuple_element_t<1, typename fn_sig<flatmap_func_gpu_t>::args>,
-                                   Shipper_GPU<typename shipper_result<fn_arg_t<flatmap_func_gpu_t, 1>>::type> &>::value,
+                      std::is_same<std::tuple_element_t<1, args_t>,
+                                   Shipper_GPU<typename shipper_result<fn_arg_t<flatmap_func_gpu_t, 1>>::type> &>::value),
                       "WindFlow Compilation Error - FlatMapGPU_Builder: __host__ __device__ void(const tuple_t &, Shipper_GPU<result_t> &)");
+        if constexpr (arity == 3)
+            static_assert(std::is_same<fn_ret_t<flatmap_func_gpu_t>, void>::value &&
+                          std::is_same<std::tuple_element_t<1, args_t>, Shipper_GPU<typename shipper_result<fn_arg_t<flatmap_func_gpu_t, 1>>::type> &>::value &&
+                          std::is_same<std::tuple_element_t<2, args_t>, fn_arg_t<flatmap_func_gpu_t, 2> &>::value,
+                          "WindFlow Compilation Error - FlatMapGPU_Builder: __host__ __device__ void(const tuple_t &, Shipper_GPU<result_t> &, state_t &)");
     }
     auto &withName(std::string n) { name = std::move(n); return *this; }
     auto &withParallelism(size_t p) { parallelism = p; return *this; }
     auto &withRebalancing() { mode = Routing_Mode_t::REBALANCING; return *this; }
     auto &withMaxOutputsPerTuple(uint32_t m) { max_outputs = m; return *this; } // required: the output batches hold original_size * m records
+    template <class keyextr_t> auto withKeyBy(keyextr_t k)
+    {
+        static_assert(arity == 3, "WindFlow Compilation Error - FlatMapGPU_Builder: withKeyBy() needs the stateful signature "
+                                  "void(const tuple_t &, Shipper_GPU<result_t> &, state_t &)");
+        return FlatMapGPU_KB_Builder<flatmap_func_gpu_t, keyextr_t>(func, k, name, parallelism, max_outputs);
+    }
     auto build()
     {
+        static_assert(arity == 2, "WindFlow Compilation Error - FlatMapGPU_Builder: a stateful functor needs withKeyBy()");
         if (max_outputs == 0) wf_fatal("FlatMapGPU_Builder [" + name + "]: withMaxOutputsPerTuple(m >= 1) is required");
         return FlatMap_GPU<flatmap_func_gpu_t>(func, parallelism, name, mode, max_outputs);
     }
@@ -1303,6 +1479,7 @@ public:
     template <class F, bool IS> FusedPipe<Stateless_GPU<F, IS>> chain(Stateless_GPU<F, IS> op);
     template <class F, class K> MultiPipe &chain(Map_GPU_KB<F, K> op) { return add_replicated(op); }
     template <class F, class K> MultiPipe &chain(Filter_GPU_KB<F, K> op) { return add_replicated(op); }
+    template <class F, class K> MultiPipe &chain(FlatMap_GPU_KB<F, K> op) { return add_replicated(op); }
     template <class F, class K> MultiPipe &chain(Reduce_GPU<F, K> op) { return add_replicated(op); }
     template <class F> MultiPipe &chain(FlatMap_GPU<F> op)
     {

@@ -172,6 +172,16 @@ int wfb_map_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t
  * n_out_dev[i] of them. out[i] must not alias in[i]. */
 int wfb_filter_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
                         uint32_t *n_out_dev, void *stream);
+/* FlatMap_GPU, keyed-stateful: flatmap(tuple, shipper, state_of_key) in per-key arrival order. out[i] holds >= in[i].n * m
+ * records; n_out_dev holds nbatches + 1 words (n_out[i], then the pushes dropped beyond m). Records of batch i are placed as by
+ * wfb_flatmap_batches: in input order, per tuple in push order, each with the timestamp of its tuple (out[i].ts written when in[i].ts
+ * and out[i].ts are both non-null); K batches give the bytes of K single-batch calls. The first m pushes of a tuple are kept, later
+ * ones dropped and counted (their state changes stand). A tuple whose key finds no slot pushes nothing and touches no state. The
+ * input is not modified; the functor may run more than once per tuple and must push the same records from the same (tuple, state).
+ * m >= 1, in[i].n * m < 2^31 and the call's sum of in[i].n * m < 2^32; out[i] must not overlap in[i] (WFB_E_BADARG otherwise).
+ * Programs without flatmap_stateful: WFB_E_UNSUPPORTED. */
+int wfb_flatmap_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h,
+                         uint32_t nbatches, uint32_t max_per_tuple, uint32_t *n_out_dev, void *stream);
 
 /* ---- Reduce_GPU, per batch -------------------------------------------------------------------------
  * keyed: one output item per distinct key, ascending key order (floating-point keys: numeric, NaN last; other keys that are not

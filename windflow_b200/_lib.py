@@ -52,6 +52,7 @@ SYMBOLS = {
     "wfb_kstate_key_capacity": (u32, [vp]),
     "wfb_map_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), u32, vp]),
     "wfb_filter_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
+    "wfb_flatmap_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, u32, vp, vp]),
     "wfb_reduce_by_key_batches": (C.c_int, [vp, C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_map_filter_batches": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_flatmap_batches": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, u32, vp, vp]),

@@ -3269,8 +3269,53 @@ __global__ void k_tb_pop_write(const FfatDev ff, const TbDev tb, uint64_t first_
 // shape as the window update -- slots of the segment's tuples, ONE wide partition pass into 1024 buckets of consecutive
 // slots, one CTA per bucket splits its items by key (stable) and ONE THREAD per key walks its run in arrival order with
 // the key's state in registers (above 65536 keys: a full sort by slot and k_ks_apply_runs). Stateful filter: keep flags,
-// then a stable per-batch compaction.
+// then a stable per-batch compaction. Keyed-stateful FlatMap_GPU: two walks over the same partition -- KS_FM_COUNT runs the
+// functor with a counting Shipper and keeps neither records nor state, a per-batch scan of the counts gives every tuple its
+// first record's index (k_fm_offsets), and KS_FM_EMIT runs it again from the same states, writing the records in place.
 // ------------------------------------------------------------------------------------------------------
+enum { KS_MAP = 0, KS_FILTER = 1, KS_FM_COUNT = 2, KS_FM_EMIT = 3 };
+// the flatmap walks' arrays: records kept per position (min(pushes, m); written by KS_FM_COUNT), the record index of every
+// position's first record within its batch (read by KS_FM_EMIT), and the word that sums the pushes dropped beyond m
+struct KsFlatMap { uint32_t *cnt; const uint32_t *off; uint32_t m; uint32_t *drop; };
+
+// one tuple of a key's run (global position gi) with the key's state `st`
+template <class P, int KM>
+__device__ __forceinline__ void ks_visit(uint32_t gi, const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff, uint32_t nb,
+                                         typename P::state_t &st, unsigned char *__restrict__ keep, const KsFlatMap fm, uint32_t &excess,
+                                         const typename P::params_t &prm)
+{
+    using T = typename P::tuple_t;
+    const uint32_t b = batch_of(boff, nb, gi);
+    unsigned char *tp = const_cast<unsigned char *>(batches[b].tuples) + static_cast<size_t>(gi - boff[b]) * sizeof(T);
+    if constexpr (KM == KS_MAP || KM == KS_FILTER) {
+        alignas(16) T t;
+        ld_rec<T>(tp, t);
+        if constexpr (KM == KS_FILTER) keep[gi] = P::filter_stateful(t, st, prm) ? 1 : 0;
+        else P::map_stateful(t, st, prm);
+        st_rec<T>(tp, t);
+    } else {
+        using R = typename P::result_t;
+        if constexpr (KM == KS_FM_COUNT) {
+            alignas(16) T t;
+            ld_rec<T>(tp, t);
+            Shipper<R> sh(nullptr, nullptr, 0, fm.m);
+            P::flatmap_stateful(t, sh, st, prm);
+            const uint32_t c = sh.pushes();
+            fm.cnt[gi] = min(c, fm.m);
+            excess += c > fm.m ? c - fm.m : 0u;
+        } else {
+            const uint32_t o = fm.off[gi]; // (issued with the tuple's load: no longer chain of dependent loads)
+            const uint32_t li = gi - boff[b];
+            unsigned char *out = batches[b].out;
+            uint64_t *ts_out = batches[b].ts_out;
+            alignas(16) T t;
+            ld_rec<T>(tp, t);
+            const uint64_t ts = ts_out != nullptr ? batches[b].ts[li] : 0;
+            Shipper<R> sh(out + static_cast<size_t>(o) * sizeof(R), ts_out != nullptr ? ts_out + o : nullptr, ts, fm.m);
+            P::flatmap_stateful(t, sh, st, prm);
+        }
+    }
+}
 template <class P>
 __global__ void k_ks_slots(const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff, uint32_t nb, uint32_t total, const FfatDev ff,
                            uint32_t *__restrict__ slots, const typename P::params_t prm)
@@ -3285,13 +3330,12 @@ __global__ void k_ks_slots(const DevBatch *__restrict__ batches, const uint32_t 
 
 constexpr uint32_t KS_KEYS = 64, KS_THREADS = 128, KS_IT = 18, KS_CAP = KS_THREADS * KS_IT;
 
-template <class P, bool FILTER>
+template <class P, int KM>
 __global__ void __launch_bounds__(KS_THREADS) k_ks_apply(const FfatDev ff, const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff,
                                                          uint32_t nb, const uint32_t *__restrict__ bk_slots, const uint32_t *__restrict__ bk_pos,
                                                          const uint32_t *__restrict__ digit_counts, uint32_t shift, unsigned char *__restrict__ states,
-                                                         unsigned char *__restrict__ keep, const typename P::params_t prm)
+                                                         unsigned char *__restrict__ keep, const typename P::params_t prm, const KsFlatMap fm)
 {
-    using T = typename P::tuple_t;
     using S = typename P::state_t;
     constexpr uint32_t NW = KS_THREADS / 32, DPT = OSW_DIGITS / KS_THREADS, HS = KS_THREADS + 2;
     __shared__ uint32_t s_idx[KS_CAP];                 // positions (global tuple index in the segment), key-major
@@ -3332,6 +3376,7 @@ __global__ void __launch_bounds__(KS_THREADS) k_ks_apply(const FfatDev ff, const
     alignas(8) S st;
     const bool has_key = tid < kpc && key_lo + tid < ff.max_keys;
     bool touched = false;
+    uint32_t excess = 0; // KS_FM_COUNT: pushes of this thread's key dropped beyond m
     if (has_key) st = *reinterpret_cast<const S *>(states + static_cast<size_t>(key_lo + tid) * sizeof(S));
     while (cursor < bend) {
         const uint32_t nsel = min(KS_CAP, bend - cursor);
@@ -3391,63 +3436,60 @@ __global__ void __launch_bounds__(KS_THREADS) k_ks_apply(const FfatDev ff, const
         __syncthreads();
         if (has_key) { // one thread per key: the run in arrival order
             const uint32_t m = kcnt[tid], off = koff[tid];
-            for (uint32_t j = 0; j < m; j++) {
-                const uint32_t gi = s_idx[off + j];
-                const uint32_t b = batch_of(boff, nb, gi);
-                unsigned char *tp = const_cast<unsigned char *>(batches[b].tuples) + static_cast<size_t>(gi - boff[b]) * sizeof(T);
-                alignas(16) T t;
-                ld_rec<T>(tp, t);
-                if constexpr (FILTER) keep[gi] = P::filter_stateful(t, st, prm) ? 1 : 0;
-                else P::map_stateful(t, st, prm);
-                st_rec<T>(tp, t);
-            }
+            for (uint32_t j = 0; j < m; j++) ks_visit<P, KM>(s_idx[off + j], batches, boff, nb, st, keep, fm, excess, prm);
             touched |= m != 0;
         }
         cursor += nsel;
         __syncthreads();
     }
-    if (has_key && touched) *reinterpret_cast<S *>(states + static_cast<size_t>(key_lo + tid) * sizeof(S)) = st;
+    if constexpr (KM == KS_FM_COUNT) { // the count walk keeps no state; one atomic per warp for the drops
+        const uint32_t w = __reduce_add_sync(FULL, excess);
+        if (lane == 0 && w != 0) atomicAdd(fm.drop, w);
+    } else if (has_key && touched) *reinterpret_cast<S *>(states + static_cast<size_t>(key_lo + tid) * sizeof(S)) = st;
 }
 
 // More than 65536 keys: the (slot, arrival position) pairs come fully sorted by slot (stable onesweep passes with 8·passes > log2
 // capacity, so INVALID_SLOT sorts behind every real slot). The thread whose item starts a run -- its slot differs from its
 // predecessor's -- walks that run in arrival order with the key's state in registers: work follows the call's items, not the capacity.
-template <class P, bool FILTER>
+template <class P, int KM>
 __global__ void __launch_bounds__(256) k_ks_apply_runs(const FfatDev ff, const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff,
                                                        uint32_t nb, uint32_t n, const uint32_t *__restrict__ sorted_slots,
                                                        const uint32_t *__restrict__ sorted_pos, unsigned char *__restrict__ states,
-                                                       unsigned char *__restrict__ keep, const typename P::params_t prm)
+                                                       unsigned char *__restrict__ keep, const typename P::params_t prm, const KsFlatMap fm)
 {
-    using T = typename P::tuple_t;
     using S = typename P::state_t;
+    uint32_t excess = 0; // KS_FM_COUNT: pushes of this thread's runs dropped beyond m
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t slot = sorted_slots[i];
         if (slot >= ff.max_keys || (i > 0 && sorted_slots[i - 1] == slot)) continue; // (no slot: the item is not applied)
         S *sp = reinterpret_cast<S *>(states + static_cast<size_t>(slot) * sizeof(S));
         alignas(8) S st = *sp;
         uint32_t j = i;
-        do {
-            const uint32_t gi = sorted_pos[j];
-            const uint32_t b = batch_of(boff, nb, gi);
-            unsigned char *tp = const_cast<unsigned char *>(batches[b].tuples) + static_cast<size_t>(gi - boff[b]) * sizeof(T);
-            alignas(16) T t;
-            ld_rec<T>(tp, t);
-            if constexpr (FILTER) keep[gi] = P::filter_stateful(t, st, prm) ? 1 : 0;
-            else P::map_stateful(t, st, prm);
-            st_rec<T>(tp, t);
-        } while (++j < n && sorted_slots[j] == slot);
-        *sp = st;
+        do ks_visit<P, KM>(sorted_pos[j], batches, boff, nb, st, keep, fm, excess, prm);
+        while (++j < n && sorted_slots[j] == slot);
+        if constexpr (KM != KS_FM_COUNT) *sp = st; // (the count walk keeps no state)
+    }
+    if constexpr (KM == KS_FM_COUNT) {
+        const uint32_t w = __reduce_add_sync(FULL, excess);
+        if ((threadIdx.x & 31u) == 0 && w != 0) atomicAdd(fm.drop, w);
     }
 }
 
-// stable per-batch compaction by the keep flags of a stateful filter: tile counts, scan, scatter
-static __global__ void __launch_bounds__(256) k_flag_tile_counts(const unsigned char *__restrict__ keep, uint32_t n, uint32_t *__restrict__ counts)
+// stable per-batch compaction by the keep flags of a stateful filter (E = unsigned char): tile counts, scan, scatter. The same
+// tile counts and batch starts over the kept record counts of a stateful flatmap (E = uint32_t) give its per-batch offsets.
+template <class E> __device__ __forceinline__ uint32_t flag_count(E v) { if constexpr (sizeof(E) == 1) return v ? 1u : 0u; else return v; }
+
+template <class E>
+static __global__ void __launch_bounds__(256) k_flag_tile_counts(const E *__restrict__ keep, uint32_t n, uint32_t *__restrict__ counts)
 {
     __shared__ uint32_t wsum[8];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, base = blockIdx.x * SEGT;
     uint32_t c = 0;
 #pragma unroll
-    for (uint32_t r = 0; r < SEGT / 256; r++) { const uint32_t i = base + r * 256 + tid; if (i < n && keep[i]) c++; }
+    for (uint32_t r = 0; r < SEGT / 256; r++) {
+        const uint32_t i = base + r * 256 + tid;
+        if constexpr (sizeof(E) == 1) { if (i < n && keep[i]) c++; } else { if (i < n) c += keep[i]; }
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL, c, o);
     if (lane == 0) wsum[warp] = c;
@@ -3456,7 +3498,8 @@ static __global__ void __launch_bounds__(256) k_flag_tile_counts(const unsigned 
 }
 
 // rank_start[b] = survivors before batch b (global rank of its first tuple); n_out of every batch
-static __global__ void k_flag_batch_starts(const unsigned char *__restrict__ keep, const uint32_t *__restrict__ tile_base, const uint32_t *__restrict__ boff,
+template <class E>
+static __global__ void k_flag_batch_starts(const E *__restrict__ keep, const uint32_t *__restrict__ tile_base, const uint32_t *__restrict__ boff,
                                            uint32_t nb, uint32_t n, uint32_t *__restrict__ rank_start, const DevBatch *__restrict__ batches)
 {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -3466,11 +3509,11 @@ static __global__ void k_flag_batch_starts(const unsigned char *__restrict__ kee
     if (gi >= n) { // total survivors
         const uint32_t lt = (n - 1) / SEGT;
         r = tile_base[lt];
-        for (uint32_t i = lt * SEGT; i < n; i++) r += keep[i] ? 1u : 0u;
+        for (uint32_t i = lt * SEGT; i < n; i++) r += flag_count(keep[i]);
     } else {
         const uint32_t t = gi / SEGT;
         r = tile_base[t];
-        for (uint32_t i = t * SEGT; i < gi; i++) r += keep[i] ? 1u : 0u;
+        for (uint32_t i = t * SEGT; i < gi; i++) r += flag_count(keep[i]);
     }
     rank_start[b] = r;
 }
@@ -3512,6 +3555,34 @@ __global__ void __launch_bounds__(256) k_flag_scatter(const unsigned char *__res
             if (bt.ts_out) bt.ts_out[o] = bt.ts[li];
             rank++;
         }
+    }
+}
+
+// keyed-stateful FlatMap_GPU: off[gi] = the records of the tuples before gi in its batch (the exclusive scan of the kept counts,
+// per batch), laid out as k_flag_scatter ranks its survivors
+static __global__ void __launch_bounds__(256) k_fm_offsets(const uint32_t *__restrict__ cnt, const uint32_t *__restrict__ tile_base,
+                                                           const uint32_t *__restrict__ boff, uint32_t nb, uint32_t n,
+                                                           const uint32_t *__restrict__ rank_start, uint32_t *__restrict__ off)
+{
+    __shared__ uint32_t wsum[8];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t first = blockIdx.x * SEGT + tid * (SEGT / 256);
+    uint32_t c[SEGT / 256];
+    uint32_t mine = 0;
+#pragma unroll
+    for (uint32_t r = 0; r < SEGT / 256; r++) { const uint32_t i = first + r; c[r] = i < n ? cnt[i] : 0u; mine += c[r]; }
+    uint32_t incl = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if (lane >= static_cast<uint32_t>(o)) incl += v; }
+    if (lane == 31) wsum[warp] = incl;
+    __syncthreads();
+    uint32_t rank = tile_base[blockIdx.x] + incl - mine;
+    for (uint32_t w = 0; w < warp; w++) rank += wsum[w];
+#pragma unroll
+    for (uint32_t r = 0; r < SEGT / 256; r++) {
+        const uint32_t gi = first + r;
+        if (gi < n) off[gi] = rank - rank_start[batch_of(boff, nb, gi)];
+        rank += c[r];
     }
 }
 

@@ -97,13 +97,14 @@ struct ProgramOps {
     uint32_t state_bytes, reserved2;
     int (*ks_slots)(const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t total, const FfatDev &ff, uint32_t *slots, cudaStream_t s,
                     const void *params);
-    int (*ks_apply)(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, const uint32_t *bk_slots,
-                    const uint32_t *bk_pos, const uint32_t *digit_counts, uint32_t shift, unsigned char *states, unsigned char *keep, cudaStream_t s,
-                    const void *params);
+    // mode: KS_MAP, KS_FILTER (keep flags), KS_FM_COUNT / KS_FM_EMIT (the two walks of a keyed-stateful flatmap, over `fm`)
+    int (*ks_apply)(int mode, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, const uint32_t *bk_slots,
+                    const uint32_t *bk_pos, const uint32_t *digit_counts, uint32_t shift, unsigned char *states, unsigned char *keep,
+                    const KsFlatMap &fm, cudaStream_t s, const void *params);
     // (more than 65536 keys) the same over the n (slot, position) pairs sorted by slot
-    int (*ks_apply_runs)(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n,
-                         const uint32_t *sorted_slots, const uint32_t *sorted_pos, unsigned char *states, unsigned char *keep, cudaStream_t s,
-                         const void *params);
+    int (*ks_apply_runs)(int mode, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n,
+                         const uint32_t *sorted_slots, const uint32_t *sorted_pos, unsigned char *states, unsigned char *keep,
+                         const KsFlatMap &fm, cudaStream_t s, const void *params);
     int (*flag_scatter)(const unsigned char *keep, const uint32_t *tile_base, const uint32_t *boff, uint32_t nb, uint32_t n,
                         const uint32_t *rank_start, const DevBatch *batches, cudaStream_t s);
     // Reduce_GPU over K queued batches
@@ -120,6 +121,8 @@ struct ProgramOps {
                            uint64_t *hi, cudaStream_t s, const void *params);
     // FlatMap_GPU: the tile pass in MODE_FLATMAP (null when the program has no flatmap)
     int (*flatmap)(TileArgs &a, const void *params, uint32_t want_grid, cudaStream_t s, uint32_t *grid_used, uint64_t span_begin, uint64_t span_end);
+    // 1: the program has flatmap_stateful (keyed-stateful FlatMap_GPU: ks_apply / ks_apply_runs take KS_FM_COUNT and KS_FM_EMIT)
+    uint32_t has_flatmap_stateful, reserved3;
 };
 
 // P::passthrough (optional): map is a no-op and lift the identity (tuple_t == result_t)
@@ -262,28 +265,52 @@ int ks_slots_dispatch(const DevBatch *batches, const uint32_t *boff, uint32_t nb
     WFB_CK(cudaGetLastError());
     return 0;
 }
+// P::flatmap_stateful(const tuple_t &, Shipper<result_t> &, state_t &, const params_t &) (optional: keyed-stateful FlatMap_GPU)
+template <class P, class = void> struct program_has_flatmap_stateful : std::false_type {};
+template <class P> struct program_has_flatmap_stateful<P, std::void_t<decltype(P::flatmap_stateful(std::declval<const typename P::tuple_t &>(),
+    std::declval<Shipper<typename P::result_t> &>(), std::declval<typename P::state_t &>(), std::declval<const typename P::params_t &>()))>>
+    : std::true_type {};
+
+// the walk of `mode` through `launch` (a generic lambda called with the mode as a constant); WFB_E_UNSUPPORTED for a flatmap walk of a
+// program without flatmap_stateful
+template <class P, class L>
+int ks_mode_launch(int mode, L &&launch)
+{
+    switch (mode) {
+    case KS_MAP: launch(std::integral_constant<int, KS_MAP>()); break;
+    case KS_FILTER: launch(std::integral_constant<int, KS_FILTER>()); break;
+    case KS_FM_COUNT: case KS_FM_EMIT:
+        if constexpr (program_has_flatmap_stateful<P>::value) {
+            if (mode == KS_FM_COUNT) launch(std::integral_constant<int, KS_FM_COUNT>()); else launch(std::integral_constant<int, KS_FM_EMIT>());
+            break;
+        } else return WFB_E_UNSUPPORTED;
+    default: return WFB_E_BADARG;
+    }
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
 template <class P>
-int ks_apply_dispatch(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, const uint32_t *bk_slots,
-                      const uint32_t *bk_pos, const uint32_t *digit_counts, uint32_t shift, unsigned char *states, unsigned char *keep, cudaStream_t s,
-                      const void *params)
+int ks_apply_dispatch(int mode, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, const uint32_t *bk_slots,
+                      const uint32_t *bk_pos, const uint32_t *digit_counts, uint32_t shift, unsigned char *states, unsigned char *keep,
+                      const KsFlatMap &fm, cudaStream_t s, const void *params)
 {
     if constexpr (program_has_state<P>::value) {
-        if (filter) k_ks_apply<P, true><<<OSW_DIGITS, KS_THREADS, 0, s>>>(ff, batches, boff, nb, bk_slots, bk_pos, digit_counts, shift, states, keep, load_params<P>(params));
-        else k_ks_apply<P, false><<<OSW_DIGITS, KS_THREADS, 0, s>>>(ff, batches, boff, nb, bk_slots, bk_pos, digit_counts, shift, states, keep, load_params<P>(params));
-        WFB_CK(cudaGetLastError());
-        return 0;
+        return ks_mode_launch<P>(mode, [&](auto km) {
+            k_ks_apply<P, decltype(km)::value><<<OSW_DIGITS, KS_THREADS, 0, s>>>(ff, batches, boff, nb, bk_slots, bk_pos, digit_counts, shift, states, keep,
+                                                                              load_params<P>(params), fm);
+        });
     } else return WFB_E_UNSUPPORTED;
 }
 template <class P>
-int ks_apply_runs_dispatch(int filter, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n,
-                           const uint32_t *sorted_slots, const uint32_t *sorted_pos, unsigned char *states, unsigned char *keep, cudaStream_t s,
-                           const void *params)
+int ks_apply_runs_dispatch(int mode, const FfatDev &ff, const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n,
+                           const uint32_t *sorted_slots, const uint32_t *sorted_pos, unsigned char *states, unsigned char *keep,
+                           const KsFlatMap &fm, cudaStream_t s, const void *params)
 {
     if constexpr (program_has_state<P>::value) {
-        if (filter) k_ks_apply_runs<P, true><<<grid_for(n, 256), 256, 0, s>>>(ff, batches, boff, nb, n, sorted_slots, sorted_pos, states, keep, load_params<P>(params));
-        else k_ks_apply_runs<P, false><<<grid_for(n, 256), 256, 0, s>>>(ff, batches, boff, nb, n, sorted_slots, sorted_pos, states, keep, load_params<P>(params));
-        WFB_CK(cudaGetLastError());
-        return 0;
+        return ks_mode_launch<P>(mode, [&](auto km) {
+            k_ks_apply_runs<P, decltype(km)::value><<<grid_for(n, 256), 256, 0, s>>>(ff, batches, boff, nb, n, sorted_slots, sorted_pos, states, keep,
+                                                                                  load_params<P>(params), fm);
+        });
     } else return WFB_E_UNSUPPORTED;
 }
 template <class P>
@@ -459,6 +486,7 @@ ProgramOps make_ops()
     o.key_order_words = &key_order_words_dispatch<P>;
     if constexpr (program_is_lifted<P>::value) o.lifted_ops = nullptr; else o.lifted_ops = &lifted_ops_of<P>;
     if constexpr (program_has_flatmap<P>::value) o.flatmap = &flatmap_dispatch<P>; else o.flatmap = nullptr;
+    o.has_flatmap_stateful = program_has_flatmap_stateful<P>::value ? 1u : 0u; o.reserved3 = 0;
     return o;
 }
 

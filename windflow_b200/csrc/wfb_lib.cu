@@ -998,6 +998,7 @@ struct wfb_kstate {
     Scratch<DevBatch> d_batches; Scratch<uint32_t> d_boff, rank_start; // capacity in batches: d_batches'
     Scratch<uint32_t> slotsA, slotsB, posA, posB, tile_cnt;           // capacity in tuples per call: slotsA's
     Scratch<unsigned char> keep;
+    Scratch<uint32_t> fm_cnt, fm_off; // keyed-stateful flatmap: records kept per position, first record's index in its batch (capacity: slotsA's)
     uint64_t launches = 0;
     PinnedStage stage;
     GrowCheck growc;              // WFB_KEYS_GROW (ff.grow)
@@ -1064,28 +1065,41 @@ int wfb_kstate_destroy(wfb_kstate_t *h)
 
 uint32_t wfb_kstate_key_capacity(const wfb_kstate_t *h) { return h ? h->ff.max_keys : 0; }
 
+// mode: KS_MAP (in place), KS_FILTER (survivors into out), KS_FM_COUNT (the flatmap: both of its walks, records into out, m per tuple)
 static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
-                      uint32_t *n_out_dev, bool filter, cudaStream_t s)
+                      uint32_t *n_out_dev, int mode, uint32_t m, cudaStream_t s)
 {
-    if (!h || !f || (nbatches && !in_h) || (filter && (!out_h || !n_out_dev))) return WFB_E_BADARG;
-    if (nbatches == 0) return 0;
+    const bool filter = mode == KS_FILTER, flatmap = mode == KS_FM_COUNT, has_out = filter || flatmap;
+    if (!h || !f || (nbatches && !in_h) || (filter && (!out_h || !n_out_dev)) || (flatmap && (!n_out_dev || (nbatches && !out_h)))) return WFB_E_BADARG;
+    if (flatmap && m == 0) return WFB_E_BADARG;
+    if (flatmap && !h->ops->has_flatmap_stateful) return WFB_E_UNSUPPORTED;
+    if (nbatches == 0 && !flatmap) return 0;
     std::lock_guard<std::mutex> lock(h->mu);
     int rc = h->order.enter(s); if (rc) return rc;
-    if (filter) CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t) * nbatches, s));
+    if (has_out) CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t) * (nbatches + (flatmap ? 1 : 0)), s)); // (flatmap: + the drop word)
     std::vector<DevBatch> hb(nbatches);
     std::vector<uint32_t> boff(nbatches + 1);
-    uint64_t total = 0;
+    uint64_t total = 0, records = 0;
     for (uint32_t i = 0; i < nbatches; i++) {
-        if (in_h[i].n && (!in_h[i].tuples || (filter && !out_h[i].tuples))) return WFB_E_BADARG;
+        if (in_h[i].n && (!in_h[i].tuples || (has_out && !out_h[i].tuples))) return WFB_E_BADARG;
         DevBatch b; std::memset(&b, 0, sizeof(b));
         b.tuples = static_cast<const unsigned char *>(in_h[i].tuples); b.ts = in_h[i].ts; b.n = in_h[i].n;
-        if (filter) {
+        if (has_out) {
             b.out = static_cast<unsigned char *>(const_cast<void *>(out_h[i].tuples));
             b.ts_out = in_h[i].ts ? const_cast<uint64_t *>(out_h[i].ts) : nullptr;
             b.n_out = n_out_dev + i;
         }
+        if (flatmap && b.n) { // (record indices of a batch and of the call are 32-bit; the walks read the input while they write the output)
+            const uint64_t nr = static_cast<uint64_t>(b.n) * m;
+            if (nr >= (1ull << 31)) return WFB_E_BADARG;
+            records += nr;
+            const uint64_t ib = reinterpret_cast<uint64_t>(b.tuples), ie = ib + static_cast<uint64_t>(b.n) * h->ops->tuple_bytes;
+            const uint64_t ob = reinterpret_cast<uint64_t>(b.out), oe = ob + nr * h->ops->result_bytes;
+            if (ib < oe && ob < ie) return WFB_E_BADARG;
+        }
         hb[i] = b; boff[i] = static_cast<uint32_t>(total); total += b.n;
     }
+    if (records >= (1ull << 32)) return WFB_E_BADARG;
     boff[nbatches] = static_cast<uint32_t>(total);
     if (total == 0) return 0;
     if (total > 0x7fffffffull) return WFB_E_BADARG;
@@ -1096,6 +1110,7 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
     CK(h->slotsA.ensure(n, s));
     const size_t cap = h->slotsA.capacity();
     CK(h->slotsB.ensure(n, s, cap)); CK(h->posA.ensure(n, s, cap)); CK(h->posB.ensure(n, s, cap)); CK(h->keep.ensure(n, s, cap));
+    if (flatmap) { CK(h->fm_cnt.ensure(n, s, cap)); CK(h->fm_off.ensure(n, s, cap)); }
     const size_t cnt_cap = (cap + SEGT - 1) / SEGT + 1;
     CK(h->tile_cnt.ensure(cnt_cap, s, cnt_cap));
     { int rc_ = h->stage.h2d(h->d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
@@ -1115,42 +1130,55 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
         if (grew) { rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc; h->launches += 2; }
     }
     const uint64_t before = h->sorter.launches;
-    if (h->buckets) {
-        const uint32_t *counts = nullptr;
-        rc = h->sorter.sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, &counts, nullptr, nullptr, 0, true);
-        if (rc) return rc;
-        rc = h->ops->ks_apply(filter ? 1 : 0, h->ff, h->d_batches, h->d_boff, nbatches, h->slotsB, h->posB, counts, h->bucket_shift, h->states,
-                              h->keep, s, f);
-    } else {
-        const uint32_t *sorted_slots, *sorted_pos;
-        rc = h->sorter.sort<uint32_t>(h->slotsA, h->slotsB, h->posA, h->posB, nullptr, n, n, h->sort_passes, s, &sorted_slots, &sorted_pos);
-        if (rc) return rc;
-        rc = h->ops->ks_apply_runs(filter ? 1 : 0, h->ff, h->d_batches, h->d_boff, nbatches, n, sorted_slots, sorted_pos, h->states, h->keep, s, f);
-    }
+    KsFlatMap fm{h->fm_cnt, h->fm_off, m, flatmap ? n_out_dev + nbatches : nullptr};
+    const uint32_t *counts = nullptr, *sorted_slots = nullptr, *sorted_pos = nullptr;
+    if (h->buckets) rc = h->sorter.sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, &counts, nullptr, nullptr, 0, true);
+    else rc = h->sorter.sort<uint32_t>(h->slotsA, h->slotsB, h->posA, h->posB, nullptr, n, n, h->sort_passes, s, &sorted_slots, &sorted_pos);
     if (rc) return rc;
-    h->launches += 2 + (h->sorter.launches - before);
-    if (filter) { // stable per-batch compaction by the keep flags
+    h->launches += 1 + (h->sorter.launches - before);
+    // the walk of `walk` over the partition (both walks of a flatmap visit every key's items in the same order from the same partition)
+    auto apply = [&](int walk) {
+        h->launches++;
+        if (h->buckets) return h->ops->ks_apply(walk, h->ff, h->d_batches, h->d_boff, nbatches, h->slotsB, h->posB, counts, h->bucket_shift, h->states,
+                                                h->keep, fm, s, f);
+        return h->ops->ks_apply_runs(walk, h->ff, h->d_batches, h->d_boff, nbatches, n, sorted_slots, sorted_pos, h->states, h->keep, fm, s, f);
+    };
+    if (flatmap) CK(cudaMemsetAsync(h->fm_cnt, 0, sizeof(uint32_t) * n, s)); // (positions whose key has no slot keep 0 records)
+    rc = apply(mode); if (rc) return rc;
+    if (has_out) { // filter: a stable per-batch compaction by the keep flags; flatmap: per-batch offsets of the kept counts, then the emit walk
         const uint32_t tiles = (n + SEGT - 1) / SEGT;
-        k_flag_tile_counts<<<tiles, 256, 0, s>>>(h->keep, n, h->tile_cnt);
+        const uint32_t sgrid = (nbatches + 1 + 127) / 128;
+        if (filter) k_flag_tile_counts<unsigned char><<<tiles, 256, 0, s>>>(h->keep, n, h->tile_cnt);
+        else k_flag_tile_counts<uint32_t><<<tiles, 256, 0, s>>>(h->fm_cnt, n, h->tile_cnt);
         k_scan_u32<<<1, 1024, 0, s>>>(h->tile_cnt, h->tile_cnt, tiles, nullptr);
-        k_flag_batch_starts<<<(nbatches + 1 + 127) / 128, 128, 0, s>>>(h->keep, h->tile_cnt, h->d_boff, nbatches, n, h->rank_start, h->d_batches);
+        if (filter) k_flag_batch_starts<unsigned char><<<sgrid, 128, 0, s>>>(h->keep, h->tile_cnt, h->d_boff, nbatches, n, h->rank_start, h->d_batches);
+        else k_flag_batch_starts<uint32_t><<<sgrid, 128, 0, s>>>(h->fm_cnt, h->tile_cnt, h->d_boff, nbatches, n, h->rank_start, h->d_batches);
         k_flag_batch_counts<<<(nbatches + 127) / 128, 128, 0, s>>>(h->rank_start, nbatches, h->d_batches);
+        if (flatmap) k_fm_offsets<<<tiles, 256, 0, s>>>(h->fm_cnt, h->tile_cnt, h->d_boff, nbatches, n, h->rank_start, h->fm_off);
         CK(cudaGetLastError());
-        rc = h->ops->flag_scatter(h->keep, h->tile_cnt, h->d_boff, nbatches, n, h->rank_start, h->d_batches, s); if (rc) return rc;
-        h->launches += 5;
+        h->launches += flatmap ? 5 : 4;
+        if (filter) { rc = h->ops->flag_scatter(h->keep, h->tile_cnt, h->d_boff, nbatches, n, h->rank_start, h->d_batches, s); h->launches++; }
+        else rc = apply(KS_FM_EMIT);
+        if (rc) return rc;
     }
     return 0;
 }
 
 int wfb_map_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *batches_h, uint32_t nbatches, void *stream)
 {
-    return kstate_run(h, f, batches_h, nullptr, nbatches, nullptr, false, static_cast<cudaStream_t>(stream));
+    return kstate_run(h, f, batches_h, nullptr, nbatches, nullptr, KS_MAP, 0, static_cast<cudaStream_t>(stream));
 }
 
 int wfb_filter_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
                         uint32_t *n_out_dev, void *stream)
 {
-    return kstate_run(h, f, in_h, out_h, nbatches, n_out_dev, true, static_cast<cudaStream_t>(stream));
+    return kstate_run(h, f, in_h, out_h, nbatches, n_out_dev, KS_FILTER, 0, static_cast<cudaStream_t>(stream));
+}
+
+int wfb_flatmap_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
+                         uint32_t max_per_tuple, uint32_t *n_out_dev, void *stream)
+{
+    return kstate_run(h, f, in_h, out_h, nbatches, n_out_dev, KS_FM_COUNT, max_per_tuple, static_cast<cudaStream_t>(stream));
 }
 
 static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_t *batches_h, uint32_t nbatches, void *out_results, uint64_t *out_ts,

@@ -240,6 +240,13 @@ class KeyedState:
               "wfb_filter_stateful")
         return outs, n_out
 
+    def flatmap(self, batches, f, outs, n_out, max_per_tuple, stream=None):
+        """flatmap(tuple, shipper, state_of_key); batch i expands into outs[i] (room for batches[i].n * max_per_tuple records),
+        n_out[i] records; n_out[K] = pushes dropped beyond max_per_tuple."""
+        check(self.L.wfb_flatmap_stateful(self.h, C.byref(f), _cbatches(batches), _cbatches(outs), len(batches), max_per_tuple, _ptr(n_out),
+                                          _stream_ptr(stream)), "wfb_flatmap_stateful")
+        return outs, n_out
+
 
 class Segment(list):
     """A list of DeviceBatch whose C descriptor array is built once: a replica that re-submits the same device buffers
