@@ -254,7 +254,6 @@ struct Batch_GPU_t: Batch_Base {
     bool deferred = false;              // size = *count_h once valid_after has fired
     uint32_t *count_h = nullptr; CountBlock *count_blk = nullptr; // deferred count: the pinned word and the producing replica's block it lies in
     std::vector<uint64_t> watermarks{std::numeric_limits<uint64_t>::max()};
-    bool isPunctuation = false;
     cudaStream_t cudaStream = nullptr;  // per-batch stream of the host->device copy (wf/batch_gpu_t.hpp:83-101)
     cudaEvent_t own_ev = nullptr;       // recorded by the producer behind the work that fills this batch ...
     cudaEvent_t valid_after = nullptr;  // ... or the event of the group this batch was produced with (consumers wait for this one)
@@ -280,7 +279,6 @@ struct Batch_GPU_t: Batch_Base {
     }
     Batch_GPU_t(const Batch_GPU_t &) = delete;
     Batch_GPU_t &operator=(const Batch_GPU_t &) = delete;
-    bool isPunct() const { return isPunctuation; }
     size_t getSize() // resolves a deferred size (waits for the producing work)
     {
         if (deferred) { gpuErrChk(cudaEventSynchronize(valid_after)); size = *count_h; deferred = false; release_count(); }
@@ -312,7 +310,7 @@ struct Batch_GPU_t: Batch_Base {
     }
     tuple_t &getTupleAtPos(size_t pos) { return pinned_tuples_cpu[pos]; }
     uint64_t getTimestampAtPos(size_t pos) { return pinned_ts_cpu[pos]; }
-    void reset(size_t n) { release_count(); size = n; deferred = false; isPunctuation = false; valid_after = nullptr; watermarks.assign(1, std::numeric_limits<uint64_t>::max()); }
+    void reset(size_t n) { release_count(); size = n; deferred = false; valid_after = nullptr; watermarks.assign(1, std::numeric_limits<uint64_t>::max()); }
 };
 
 // returns a batch to its producer (deleteBatch_t, wf/recycling.hpp:66-85); batches that do not fit the queue are freed
@@ -561,7 +559,7 @@ public:
     void *svc(void *msg) override
     {
         auto *b = reinterpret_cast<Batch_GPU_t<tuple_t> *>(msg);
-        if (!b->isPunct() && b->getSize() != 0) {
+        if (b->getSize() != 0) {
             b->transfer2CPU(stream);
             for (size_t i = 0; i < b->size; i++) { std::optional<tuple_t> o(b->getTupleAtPos(i)); func(o); }
         }
@@ -581,21 +579,121 @@ public:
 #define WF_MAX_BATCHES_PER_CALL 128
 #endif
 
+// The drop counts of a FlatMap_GPU replica's calls: every call leaves its count in the word after its batches' sizes, in a block the
+// replica holds until the host has read that word.
+class FlatMapDrops {
+    struct Pending { CountBlock *blk; size_t word; cudaEvent_t ev; };
+    std::vector<Pending> pending; uint64_t dropped = 0; // drop counts of calls the host has not read yet / the sum of those it read
+public:
+    void add(CountBlock *blk, size_t word, cudaEvent_t ev) { pending.push_back(Pending{blk, word, ev}); }
+    // adds the drop counts of finished calls (all of them with `wait`)
+    void read(bool wait)
+    {
+        size_t i = 0;
+        for (; i < pending.size(); i++) {
+            if (wait || pending.size() - i > 8) { gpuErrChk(cudaEventSynchronize(pending[i].ev)); } // (events of the ring are re-recorded after 16 calls)
+            else if (cudaEventQuery(pending[i].ev) != cudaSuccess) { cudaGetLastError(); break; }
+            dropped += pending[i].blk->h[pending[i].word];
+            pending[i].blk->release();
+        }
+        pending.erase(pending.begin(), pending.begin() + static_cast<std::ptrdiff_t>(i));
+    }
+    // end of stream: stops the program when a push was dropped
+    void check(const std::string &op_name, uint32_t max_out)
+    {
+        read(true);
+        if (dropped) wf_fatal("FlatMap_GPU [" + op_name + "]: " + std::to_string(dropped) + " records pushed beyond withMaxOutputsPerTuple(" +
+                              std::to_string(max_out) + ") were dropped");
+    }
+};
+
+// The call of every GPU replica: svc() takes the batches queued on its input (up to maxk) and hands them to ONE launch sequence.
+// take() is the input half. The operator then sends its results in one of two shapes: send_in_place() (the inputs, changed in place,
+// move on) or send_deferred() (input i becomes output batch i, whose size stays on the device).
+template <class in_t, class out_t = in_t>
+class Batch_Replica: public Basic_Replica {
+protected:
+    using in_batch_t = Batch_GPU_t<in_t>;
+    using out_batch_t = Batch_GPU_t<out_t>;
+    size_t maxk;
+    DeferredCounts counts; // (before the pool: its batches point into it)
+    BatchPool<out_t> pool;
+    std::vector<in_batch_t *> in;     // the batches of the call
+    std::vector<wfb_batch_t> bi, bo;  // their descriptors, and those of their output batches
+    std::vector<out_batch_t *> outs;
+    Batch_Replica(std::string n, size_t maxk_, size_t pool_size = 4 * WF_MAX_BATCHES_PER_CALL): Basic_Replica(std::move(n)), maxk(maxk_ ? maxk_ : 1), pool(pool_size) {}
+    // the batches queued on the input (those of size 0 recycled with `skip_empty`), the stream ordered behind their producers, their
+    // descriptors in bi; false: nothing to launch
+    bool take(void *msg, bool skip_empty)
+    {
+        drain(msg, maxk, in);
+        size_t k = 0;
+        for (auto *b : in) { if (b->getSize() == 0 && skip_empty) recycleBatch(b); else in[k++] = b; }
+        in.resize(k);
+        if (k == 0) return false;
+        wait_inputs(in);
+        bi.resize(k);
+        for (size_t i = 0; i < k; i++) bi[i] = wfb_batch_t{in[i]->tuples_gpu, in[i]->ts_gpu, in[i]->getWatermark(), static_cast<uint32_t>(in[i]->size), 0};
+        return true;
+    }
+    // a batch of capacity >= cap for the results of input b, which the stream may write
+    out_batch_t *output_for(const in_batch_t *b, size_t cap)
+    {
+        out_batch_t *o = pool.get(cap);
+        o->watermarks = b->watermarks;
+        if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
+        return o;
+    }
+    // the inputs, changed in place by the launches just issued, move on
+    void send_in_place()
+    {
+        cudaEvent_t e = next_event();
+        gpuErrChk(cudaEventRecord(e, stream));
+        for (auto *b : in) { b->valid_after = e; this->ff_send_out(b); }
+    }
+    // input i becomes output batch i, of capacity original_size * mult and at most size * mult results: call(counts_d) issues the
+    // launches, which leave the size of output i in counts_d[i] and `extra` words of the operator's after the k sizes. Those words are
+    // the replica's to read and release. Returns the call's block and the event behind the call.
+    template <class Call> std::pair<CountBlock *, cudaEvent_t> send_deferred(size_t mult, size_t extra, Call &&call)
+    {
+        const size_t k = in.size();
+        bo.resize(k); outs.resize(k);
+        for (size_t i = 0; i < k; i++) {
+            outs[i] = output_for(in[i], in[i]->original_size * mult);
+            bo[i] = wfb_batch_t{outs[i]->tuples_gpu, outs[i]->ts_gpu, in[i]->getWatermark(), static_cast<uint32_t>(outs[i]->original_size), 0};
+        }
+        CountBlock *blk; uint32_t *counts_d;
+        gpuErrChk(counts.acquire(static_cast<uint32_t>(k + extra), blk, counts_d));
+        call(counts_d);
+        gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * (k + extra), cudaMemcpyDeviceToHost, stream));
+        cudaEvent_t e = next_event();
+        gpuErrChk(cudaEventRecord(e, stream));
+        for (size_t i = 0; i < k; i++) {
+            outs[i]->defer(in[i]->size * mult, blk, i, e);
+            in[i]->reuse_after = e; recycleBatch(in[i]); // (the reference drops empty batches here, wf/filter_gpu.hpp:572-581: the
+            this->ff_send_out(outs[i]);                   // size is not known on the host yet, the consumer skips an empty one)
+        }
+        return {blk, e};
+    }
+    // send_deferred() of a FlatMap_GPU: outputs of original_size * m records, and the call's drop count in the word after the sizes
+    template <class Call> void send_expanded(FlatMapDrops &drops, uint32_t m, Call &&call)
+    {
+        drops.read(false);
+        const auto sent = send_deferred(m, 1, call);
+        drops.add(sent.first, in.size(), sent.second);
+    }
+};
+
 // A fused run of stateless Map_GPU / Filter_GPU operators over tuple_t (wf/map_gpu.hpp:313-420, wf/filter_gpu.hpp:401-600): ONE
 // streaming pass per svc() over the K batches found queued. A run of maps only works in place (wfb_map per batch: same batch
 // moves on); with a filter in the run the survivors are compacted, stable, into K spare batches whose sizes stay on the device.
 template <class tuple_t>
-class ChainReplica: public Basic_Replica {
+class ChainReplica: public Batch_Replica<tuple_t> {
+    using base_t = Batch_Replica<tuple_t>; using base_t::in; using base_t::bi; using base_t::bo; using base_t::stream;
     using prog_t = ChainProgram<tuple_t>;
-    using batch_t = Batch_GPU_t<tuple_t>;
     wfb_engine_t *eng = nullptr; typename prog_t::params_t prm{};
-    DeferredCounts counts; // (before the pool: its batches point into it)
-    BatchPool<tuple_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-    size_t maxk;
-    std::vector<batch_t *> in;
-    std::vector<wfb_batch_t> bi, bo;
 public:
-    ChainReplica(std::string n, const StageChain &c, size_t maxk_): Basic_Replica(std::move(n)), maxk(maxk_ ? maxk_ : 1)
+    ChainReplica(std::string n, const StageChain &c, size_t maxk): base_t(std::move(n), maxk)
     {
         if (c.has_filter) prm.filt.c = c; else prm.map.c = c; // (the filter slot runs maps and predicates in order)
     }
@@ -604,56 +702,22 @@ public:
     {
         Basic_Replica::svc_init();
         wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
-        if (prm.filt.c.n) gpuErrChk(counts.init(maxk));
+        if (prm.filt.c.n) gpuErrChk(this->counts.init(this->maxk));
         return 0;
     }
     void *svc(void *msg) override
     {
-        drain(msg, maxk, in);
-        std::vector<batch_t *> work;
-        for (auto *b : in) { if (b->isPunct()) { flush_work(work); this->ff_send_out(b); } else work.push_back(b); }
-        flush_work(work);
-        return this->GO_ON;
-    }
-private:
-    void flush_work(std::vector<batch_t *> &work)
-    {
-        if (work.empty()) return;
-        wait_inputs(work);
+        if (!this->take(msg, false)) return this->GO_ON;
         const wfb_functors_t *f = reinterpret_cast<const wfb_functors_t *>(&prm);
         if (prm.filt.c.n == 0) { // maps only: in place, the same batches move on
-            for (auto *b : work) { b->getSize(); if (b->size) wfbErrChk(wfb_map(eng, f, b->tuples_gpu, static_cast<uint32_t>(b->size), stream)); }
-            cudaEvent_t e = next_event();
-            gpuErrChk(cudaEventRecord(e, stream));
-            for (auto *b : work) { b->valid_after = e; this->ff_send_out(b); }
+            for (auto *b : in) if (b->size) wfbErrChk(wfb_map(eng, f, b->tuples_gpu, static_cast<uint32_t>(b->size), stream));
+            this->send_in_place();
         } else {
-            const size_t k = work.size();
-            bi.resize(k); bo.resize(k);
-            std::vector<batch_t *> outs(k);
-            for (size_t i = 0; i < k; i++) {
-                batch_t *b = work[i];
-                b->getSize();
-                batch_t *o = pool.get(b->original_size);
-                o->watermarks = b->watermarks;
-                if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
-                bi[i] = wfb_batch_t{b->tuples_gpu, b->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
-                bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
-                outs[i] = o;
-            }
-            CountBlock *blk; uint32_t *counts_d;
-            gpuErrChk(counts.acquire(static_cast<uint32_t>(k), blk, counts_d));
-            wfbErrChk(wfb_map_filter_batches(eng, f, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream));
-            gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
-            cudaEvent_t e = next_event();
-            gpuErrChk(cudaEventRecord(e, stream));
-            for (size_t i = 0; i < k; i++) {
-                batch_t *o = outs[i];
-                o->defer(work[i]->size, blk, i, e);
-                work[i]->reuse_after = e; recycleBatch(work[i]); // (the reference drops empty batches here, wf/filter_gpu.hpp:572-581: the
-                this->ff_send_out(o);                             // size is not known on the host yet, the consumer skips an empty one)
-            }
+            this->send_deferred(1, 0, [&](uint32_t *counts_d) {
+                wfbErrChk(wfb_map_filter_batches(eng, f, bi.data(), bo.data(), static_cast<uint32_t>(in.size()), counts_d, stream));
+            });
         }
-        work.clear();
+        return this->GO_ON;
     }
 };
 
@@ -696,47 +760,15 @@ template <class F> using Filter_GPU = Stateless_GPU<F, true>;
 template <class shipper_t> struct shipper_result;
 template <class R> struct shipper_result<wfb::Shipper<R>> { using type = R; };
 
-// The drop counts of a FlatMap_GPU replica's calls: every call leaves its count in the word after its batches' sizes, in a block the
-// replica holds until the host has read that word.
-class FlatMapDrops {
-    struct Pending { CountBlock *blk; size_t word; cudaEvent_t ev; };
-    std::vector<Pending> pending; uint64_t dropped = 0; // drop counts of calls the host has not read yet / the sum of those it read
-public:
-    void add(CountBlock *blk, size_t word, cudaEvent_t ev) { pending.push_back(Pending{blk, word, ev}); }
-    // adds the drop counts of finished calls (all of them with `wait`)
-    void read(bool wait)
-    {
-        size_t i = 0;
-        for (; i < pending.size(); i++) {
-            if (wait || pending.size() - i > 8) { gpuErrChk(cudaEventSynchronize(pending[i].ev)); } // (events of the ring are re-recorded after 16 calls)
-            else if (cudaEventQuery(pending[i].ev) != cudaSuccess) { cudaGetLastError(); break; }
-            dropped += pending[i].blk->h[pending[i].word];
-            pending[i].blk->release();
-        }
-        pending.erase(pending.begin(), pending.begin() + static_cast<std::ptrdiff_t>(i));
-    }
-    // end of stream: stops the program when a push was dropped
-    void check(const std::string &op_name, uint32_t max_out)
-    {
-        read(true);
-        if (dropped) wf_fatal("FlatMap_GPU [" + op_name + "]: " + std::to_string(dropped) + " records pushed beyond withMaxOutputsPerTuple(" +
-                              std::to_string(max_out) + ") were dropped");
-    }
-};
-
 template <class tuple_t, class result_t, class func_t>
-class FlatMapReplica: public Basic_Replica {
+class FlatMapReplica: public Batch_Replica<tuple_t, result_t> {
+    using base_t = Batch_Replica<tuple_t, result_t>; using base_t::in; using base_t::bi; using base_t::bo; using base_t::stream;
     using prog_t = FacadeFlatMapProgram<tuple_t, result_t, func_t>;
-    using batch_t = Batch_GPU_t<tuple_t>;
     wfb_engine_t *eng = nullptr; typename prog_t::params_t prm{};
-    uint32_t max_out; size_t maxk;
-    DeferredCounts counts; // deferred sizes + the drop count of every call, which this replica reads itself (it holds the block until then)
-    BatchPool<result_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-    FlatMapDrops drops;
-    std::vector<batch_t *> in;
-    std::vector<wfb_batch_t> bi, bo;
+    uint32_t max_out;
+    FlatMapDrops drops; // (the replica holds every call's block until it has read the drop count)
 public:
-    FlatMapReplica(std::string n, const StageChain &pre, func_t f, uint32_t m, size_t maxk_): Basic_Replica(std::move(n)), max_out(m), maxk(maxk_ ? maxk_ : 1)
+    FlatMapReplica(std::string n, const StageChain &pre, func_t f, uint32_t m, size_t maxk): base_t(std::move(n), maxk), max_out(m)
     {
         prm.filt.c = pre; prm.fm = f;
     }
@@ -745,63 +777,22 @@ public:
     {
         Basic_Replica::svc_init();
         wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
-        gpuErrChk(counts.init(maxk + 1));
+        gpuErrChk(this->counts.init(this->maxk + 1));
         return 0;
     }
     void *svc(void *msg) override
     {
-        drain(msg, maxk, in);
-        std::vector<batch_t *> work;
-        for (auto *b : in) {
-            if (!b->isPunct()) { work.push_back(b); continue; }
-            flush_work(work);
-            Batch_GPU_t<result_t> *p = pool.get(1); // (a punctuation of the output type)
-            p->isPunctuation = true; p->size = 0; p->watermarks = b->watermarks;
-            recycleBatch(b);
-            this->ff_send_out(p);
-        }
-        flush_work(work);
+        if (!this->take(msg, false)) return this->GO_ON;
+        this->send_expanded(drops, max_out, [&](uint32_t *counts_d) {
+            wfbErrChk(wfb_flatmap_batches(eng, reinterpret_cast<const wfb_functors_t *>(&prm), bi.data(), bo.data(), static_cast<uint32_t>(in.size()),
+                                          max_out, counts_d, stream));
+        });
         return this->GO_ON;
     }
     void eosnotify(ssize_t id) override
     {
-        drops.check(opName, max_out);
+        drops.check(this->opName, max_out);
         Basic_Replica::eosnotify(id);
-    }
-private:
-    void flush_work(std::vector<batch_t *> &work)
-    {
-        if (work.empty()) return;
-        wait_inputs(work);
-        drops.read(false);
-        const size_t k = work.size();
-        bi.resize(k); bo.resize(k);
-        std::vector<Batch_GPU_t<result_t> *> outs(k);
-        for (size_t i = 0; i < k; i++) {
-            batch_t *b = work[i];
-            b->getSize();
-            Batch_GPU_t<result_t> *o = pool.get(b->original_size * max_out);
-            o->watermarks = b->watermarks;
-            if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
-            bi[i] = wfb_batch_t{b->tuples_gpu, b->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
-            bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(o->original_size), 0};
-            outs[i] = o;
-        }
-        CountBlock *blk; uint32_t *counts_d;
-        gpuErrChk(counts.acquire(static_cast<uint32_t>(k + 1), blk, counts_d));
-        wfbErrChk(wfb_flatmap_batches(eng, reinterpret_cast<const wfb_functors_t *>(&prm), bi.data(), bo.data(), static_cast<uint32_t>(k), max_out,
-                                      counts_d, stream));
-        gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
-        cudaEvent_t e = next_event();
-        gpuErrChk(cudaEventRecord(e, stream));
-        drops.add(blk, k, e);
-        for (size_t i = 0; i < k; i++) {
-            Batch_GPU_t<result_t> *o = outs[i];
-            o->defer(work[i]->size * max_out, blk, i, e);
-            work[i]->reuse_after = e; recycleBatch(work[i]);
-            this->ff_send_out(o);
-        }
-        work.clear();
     }
 };
 
@@ -824,210 +815,101 @@ public:
     }
 };
 
-// Map_GPU / Filter_GPU, keyed-stateful (wf/map_gpu.hpp:104-310, wf/filter_gpu.hpp:120-399): func(tuple, state_of_key) in per-key arrival
-// order. The key -> state table is one wfb_kstate_t per operator, shared by its replicas behind a mutex (the reference's TBB map +
-// spinlock, wf/map_gpu.hpp:551-559); a replica hands the K batches it finds queued to one launch sequence.
+// Map_GPU / Filter_GPU / FlatMap_GPU, keyed-stateful (wf/map_gpu.hpp:104-310, wf/filter_gpu.hpp:120-399, FlatMap_Builder(f).withKeyBy(k)
+// of wf/flatmap.hpp): func(tuple_t &, state_t &), or func(const tuple_t &, Shipper_GPU<result_t> &, state_t &) for a FlatMap, in per-key
+// arrival order. The key -> state table is one wfb_kstate_t per operator, shared by its replicas behind a mutex (the reference's TBB
+// map + spinlock, wf/map_gpu.hpp:551-559); a replica hands the K batches it finds queued to one launch sequence. A Map works in place,
+// a Filter compacts the survivors into output batches whose sizes stay on the device, and a FlatMap has the outputs and the drop count
+// of FlatMap_GPU: input batch i becomes output batch i of capacity original_size * m whose size stays on the device, and a push beyond
+// the m-th of a tuple stops the program at the end of the stream.
 struct SharedKState { wfb_kstate_t *h = nullptr; std::mutex mu; ~SharedKState() { if (h) wfb_kstate_destroy(h); } };
+enum class Stateful_Kind_t { MAP, FILTER, FLATMAP };
+template <class F, Stateful_Kind_t KIND> struct stateful_result { using type = fn_arg_t<F, 0>; };
+template <class F> struct stateful_result<F, Stateful_Kind_t::FLATMAP> { using type = typename shipper_result<fn_arg_t<F, 1>>::type; };
 
-template <class func_t, class keyextr_func_gpu_t, bool IS_FILTER>
+template <class func_t, class keyextr_func_gpu_t, Stateful_Kind_t KIND>
 class Stateful_GPU: public Basic_Operator {
 public:
+    static constexpr bool is_flatmap = KIND == Stateful_Kind_t::FLATMAP;
     using tuple_t = fn_arg_t<func_t, 0>;
-    using state_t = fn_arg_t<func_t, 1>;
-    using result_t = tuple_t;
-    using prog_t = std::conditional_t<IS_FILTER, FacadeStatefulProgram<tuple_t, state_t, StatefulIdMap<tuple_t, state_t>, func_t, keyextr_func_gpu_t>,
-                                      FacadeStatefulProgram<tuple_t, state_t, func_t, StatefulKeepAll<tuple_t, state_t>, keyextr_func_gpu_t>>;
-    static constexpr op_type_t op_type = op_type_t::BASIC_GPU;
-    func_t func; keyextr_func_gpu_t key_extr; uint32_t max_keys; size_t maxk = WF_MAX_BATCHES_PER_CALL;
-    bool grow_keys = false; // withKeyGrowth(): max_keys is the initial capacity of the table (WFB_KEYS_GROW), which grows under the replicas' mutex
-    Stateful_GPU(func_t f, keyextr_func_gpu_t k, size_t p, std::string n, uint32_t mk): Basic_Operator(std::move(n), p, Routing_Mode_t::KEYBY, 1), func(f), key_extr(k), max_keys(mk) {}
-    std::string getType() const override { return IS_FILTER ? "Filter_GPU" : "Map_GPU"; }
-    keyextr_func_gpu_t getKeyExtractor() const { return key_extr; }
-    class Replica: public Basic_Replica {
-        using batch_t = Batch_GPU_t<tuple_t>;
-        std::shared_ptr<SharedKState> ks; typename prog_t::params_t prm; size_t maxk;
-        DeferredCounts counts;
-        BatchPool<tuple_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-        std::vector<batch_t *> in;
-        std::vector<wfb_batch_t> bi, bo;
-    public:
-        static typename prog_t::params_t make_params(func_t f, keyextr_func_gpu_t k)
-        {
-            if constexpr (IS_FILTER) return typename prog_t::params_t{{}, f, k}; else return typename prog_t::params_t{f, {}, k};
-        }
-        Replica(std::string n, std::shared_ptr<SharedKState> h, func_t f, keyextr_func_gpu_t k, size_t mk): Basic_Replica(std::move(n)), ks(std::move(h)), prm(make_params(f, k)), maxk(mk ? mk : 1) {}
-        int svc_init() override
-        {
-            Basic_Replica::svc_init();
-            if (IS_FILTER) gpuErrChk(counts.init(maxk));
-            return 0;
-        }
-        void *svc(void *msg) override
-        {
-            drain(msg, maxk, in);
-            std::vector<batch_t *> work;
-            for (auto *b : in) { if (b->isPunct()) { run(work); this->ff_send_out(b); } else if (b->getSize() == 0) recycleBatch(b); else work.push_back(b); }
-            run(work);
-            return this->GO_ON;
-        }
-    private:
-        void run(std::vector<batch_t *> &work)
-        {
-            if (work.empty()) return;
-            wait_inputs(work);
-            const size_t k = work.size();
-            const wfb_functors_t *f = reinterpret_cast<const wfb_functors_t *>(&prm);
-            bi.resize(k);
-            for (size_t i = 0; i < k; i++) bi[i] = wfb_batch_t{work[i]->tuples_gpu, work[i]->ts_gpu, work[i]->getWatermark(), static_cast<uint32_t>(work[i]->size), 0};
-            std::vector<batch_t *> outs;
-            CountBlock *blk = nullptr; uint32_t *counts_d = nullptr;
-            if constexpr (IS_FILTER) {
-                gpuErrChk(counts.acquire(static_cast<uint32_t>(k), blk, counts_d));
-                bo.resize(k); outs.resize(k);
-                for (size_t i = 0; i < k; i++) {
-                    batch_t *o = pool.get(work[i]->original_size);
-                    o->watermarks = work[i]->watermarks;
-                    if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
-                    bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, work[i]->getWatermark(), bi[i].n, 0};
-                    outs[i] = o;
-                }
-            }
-            {   // the replicas of the operator share the state table: one launch sequence at a time (stream order carries the dependency on)
-                std::lock_guard<std::mutex> lock(ks->mu);
-                if constexpr (IS_FILTER) { wfbErrChk(wfb_filter_stateful(ks->h, f, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream)); }
-                else { wfbErrChk(wfb_map_stateful(ks->h, f, bi.data(), static_cast<uint32_t>(k), stream)); }
-                gpuErrChk(cudaStreamSynchronize(stream)); // another replica's launches on its own stream must see this call's state
-            }
-            cudaEvent_t e = next_event();
-            if constexpr (IS_FILTER) {
-                gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
-                gpuErrChk(cudaEventRecord(e, stream));
-                for (size_t i = 0; i < k; i++) {
-                    outs[i]->defer(work[i]->size, blk, i, e);
-                    work[i]->reuse_after = e; recycleBatch(work[i]);
-                    this->ff_send_out(outs[i]);
-                }
-            } else {
-                gpuErrChk(cudaEventRecord(e, stream));
-                for (auto *b : work) { b->valid_after = e; this->ff_send_out(b); }
-            }
-            work.clear();
-        }
-    };
-    std::shared_ptr<SharedKState> kstate;
-    Replica *make_replica()
-    {
-        if (!kstate) { kstate = std::make_shared<SharedKState>(); wfbErrChk(wfb_kstate_create(&kstate->h, wfb::register_program<prog_t>(), max_keys, grow_keys ? WFB_KEYS_GROW : 0u)); }
-        return new Replica(name, kstate, func, key_extr, parallelism > 1 ? 1 : maxk);
-    }
-};
-template <class F, class K> using Map_GPU_KB = Stateful_GPU<F, K, false>;
-template <class F, class K> using Filter_GPU_KB = Stateful_GPU<F, K, true>;
-
-// FlatMap_GPU, keyed-stateful (FlatMap_Builder(f).withKeyBy(k) of wf/flatmap.hpp on the GPU): func(const tuple_t &, Shipper_GPU<result_t> &,
-// state_t &) in per-key arrival order. The key -> state table is shared by the replicas as for the keyed Map / Filter (SharedKState);
-// the outputs and the drop count are those of FlatMap_GPU: input batch i becomes output batch i of capacity original_size * m whose size
-// stays on the device, and a push beyond the m-th of a tuple stops the program at the end of the stream.
-template <class func_t, class keyextr_func_gpu_t>
-class FlatMap_GPU_KB: public Basic_Operator {
-public:
-    using tuple_t = fn_arg_t<func_t, 0>;
-    using result_t = typename shipper_result<fn_arg_t<func_t, 1>>::type;
-    using state_t = fn_arg_t<func_t, 2>;
-    using prog_t = FacadeStatefulFlatMapProgram<tuple_t, result_t, state_t, func_t, keyextr_func_gpu_t>;
+    using result_t = typename stateful_result<func_t, KIND>::type;
+    using state_t = fn_arg_t<func_t, is_flatmap ? 2 : 1>;
+    using prog_t = std::conditional_t<is_flatmap, FacadeStatefulFlatMapProgram<tuple_t, result_t, state_t, func_t, keyextr_func_gpu_t>,
+                   std::conditional_t<KIND == Stateful_Kind_t::FILTER,
+                                      FacadeStatefulProgram<tuple_t, state_t, StatefulIdMap<tuple_t, state_t>, func_t, keyextr_func_gpu_t>,
+                                      FacadeStatefulProgram<tuple_t, state_t, func_t, StatefulKeepAll<tuple_t, state_t>, keyextr_func_gpu_t>>>;
     static constexpr op_type_t op_type = op_type_t::BASIC_GPU;
     func_t func; keyextr_func_gpu_t key_extr; uint32_t max_keys, max_outputs; size_t maxk = WF_MAX_BATCHES_PER_CALL;
-    bool grow_keys = false; // withKeyGrowth(): max_keys is the initial capacity of the table (WFB_KEYS_GROW)
-    FlatMap_GPU_KB(func_t f, keyextr_func_gpu_t k, size_t p, std::string n, uint32_t mk, uint32_t m)
+    bool grow_keys = false; // withKeyGrowth(): max_keys is the initial capacity of the table (WFB_KEYS_GROW), which grows under the replicas' mutex
+    Stateful_GPU(func_t f, keyextr_func_gpu_t k, size_t p, std::string n, uint32_t mk, uint32_t m)
         : Basic_Operator(std::move(n), p, Routing_Mode_t::KEYBY, 1), func(f), key_extr(k), max_keys(mk), max_outputs(m)
     {
-        static_assert(std::is_trivially_copyable<func_t>::value, "GPU functors must be trivially copyable");
+        static_assert(!is_flatmap || std::is_trivially_copyable<func_t>::value, "GPU functors must be trivially copyable");
     }
-    std::string getType() const override { return "FlatMap_GPU"; }
+    std::string getType() const override { return KIND == Stateful_Kind_t::MAP ? "Map_GPU" : KIND == Stateful_Kind_t::FILTER ? "Filter_GPU" : "FlatMap_GPU"; }
     keyextr_func_gpu_t getKeyExtractor() const { return key_extr; }
-    class Replica: public Basic_Replica {
-        using batch_t = Batch_GPU_t<tuple_t>;
-        std::shared_ptr<SharedKState> ks; typename prog_t::params_t prm; uint32_t max_out; size_t maxk;
-        DeferredCounts counts; // deferred sizes + the drop count of every call
-        BatchPool<result_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-        FlatMapDrops drops;
-        std::vector<batch_t *> in;
-        std::vector<wfb_batch_t> bi, bo;
+    class Replica: public Batch_Replica<tuple_t, result_t> {
+        using base_t = Batch_Replica<tuple_t, result_t>; using base_t::in; using base_t::bi; using base_t::bo; using base_t::stream;
+        std::shared_ptr<SharedKState> ks; typename prog_t::params_t prm; uint32_t max_out;
+        FlatMapDrops drops; // (FlatMap)
+        // the replicas of the operator share the state table: one launch sequence at a time
+        template <class Launch> void locked(Launch &&launch)
+        {
+            std::lock_guard<std::mutex> lock(ks->mu);
+            wfbErrChk(launch());
+            gpuErrChk(cudaStreamSynchronize(stream)); // another replica's launches on its own stream must see this call's state
+        }
     public:
-        Replica(std::string n, std::shared_ptr<SharedKState> h, func_t f, keyextr_func_gpu_t k, uint32_t m, size_t mk)
-            : Basic_Replica(std::move(n)), ks(std::move(h)), prm{f, k}, max_out(m), maxk(mk ? mk : 1) {}
+        Replica(std::string n, std::shared_ptr<SharedKState> h, typename prog_t::params_t p, uint32_t m, size_t maxk)
+            : base_t(std::move(n), maxk), ks(std::move(h)), prm(p), max_out(m) {}
         int svc_init() override
         {
             Basic_Replica::svc_init();
-            gpuErrChk(counts.init(maxk + 1));
+            if constexpr (KIND == Stateful_Kind_t::FILTER) gpuErrChk(this->counts.init(this->maxk));
+            if constexpr (is_flatmap) gpuErrChk(this->counts.init(this->maxk + 1));
             return 0;
         }
         void *svc(void *msg) override
         {
-            drain(msg, maxk, in);
-            std::vector<batch_t *> work;
-            for (auto *b : in) {
-                if (!b->isPunct()) { work.push_back(b); continue; }
-                run(work);
-                Batch_GPU_t<result_t> *p = pool.get(1); // (a punctuation of the output type)
-                p->isPunctuation = true; p->size = 0; p->watermarks = b->watermarks;
-                recycleBatch(b);
-                this->ff_send_out(p);
+            if (!this->take(msg, !is_flatmap)) return this->GO_ON;
+            const wfb_functors_t *f = reinterpret_cast<const wfb_functors_t *>(&prm);
+            const uint32_t k = static_cast<uint32_t>(in.size());
+            if constexpr (KIND == Stateful_Kind_t::MAP) {
+                locked([&] { return wfb_map_stateful(ks->h, f, bi.data(), k, stream); });
+                this->send_in_place();
+            } else if constexpr (KIND == Stateful_Kind_t::FILTER) {
+                this->send_deferred(1, 0, [&](uint32_t *counts_d) {
+                    locked([&] { return wfb_filter_stateful(ks->h, f, bi.data(), bo.data(), k, counts_d, stream); });
+                });
+            } else {
+                this->send_expanded(drops, max_out, [&](uint32_t *counts_d) {
+                    locked([&] { return wfb_flatmap_stateful(ks->h, f, bi.data(), bo.data(), k, max_out, counts_d, stream); });
+                });
             }
-            run(work);
             return this->GO_ON;
         }
         void eosnotify(ssize_t id) override
         {
-            drops.check(opName, max_out);
+            if constexpr (is_flatmap) drops.check(this->opName, max_out);
             Basic_Replica::eosnotify(id);
         }
-    private:
-        void run(std::vector<batch_t *> &work)
-        {
-            if (work.empty()) return;
-            wait_inputs(work);
-            drops.read(false);
-            const size_t k = work.size();
-            bi.resize(k); bo.resize(k);
-            std::vector<Batch_GPU_t<result_t> *> outs(k);
-            for (size_t i = 0; i < k; i++) {
-                batch_t *b = work[i];
-                b->getSize();
-                Batch_GPU_t<result_t> *o = pool.get(b->original_size * max_out);
-                o->watermarks = b->watermarks;
-                if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
-                bi[i] = wfb_batch_t{b->tuples_gpu, b->ts_gpu, b->getWatermark(), static_cast<uint32_t>(b->size), 0};
-                bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, b->getWatermark(), static_cast<uint32_t>(o->original_size), 0};
-                outs[i] = o;
-            }
-            CountBlock *blk; uint32_t *counts_d;
-            gpuErrChk(counts.acquire(static_cast<uint32_t>(k + 1), blk, counts_d));
-            {   // the replicas of the operator share the state table: one launch sequence at a time
-                std::lock_guard<std::mutex> lock(ks->mu);
-                wfbErrChk(wfb_flatmap_stateful(ks->h, reinterpret_cast<const wfb_functors_t *>(&prm), bi.data(), bo.data(), static_cast<uint32_t>(k),
-                                               max_out, counts_d, stream));
-                gpuErrChk(cudaStreamSynchronize(stream)); // another replica's launches on its own stream must see this call's state
-            }
-            gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * (k + 1), cudaMemcpyDeviceToHost, stream));
-            cudaEvent_t e = next_event();
-            gpuErrChk(cudaEventRecord(e, stream));
-            drops.add(blk, k, e);
-            for (size_t i = 0; i < k; i++) {
-                outs[i]->defer(work[i]->size * max_out, blk, i, e);
-                work[i]->reuse_after = e; recycleBatch(work[i]);
-                this->ff_send_out(outs[i]);
-            }
-            work.clear();
-        }
     };
+    typename prog_t::params_t params() const
+    {
+        if constexpr (KIND == Stateful_Kind_t::MAP) return {func, {}, key_extr};
+        else if constexpr (KIND == Stateful_Kind_t::FILTER) return {{}, func, key_extr};
+        else return {func, key_extr};
+    }
     std::shared_ptr<SharedKState> kstate;
     Replica *make_replica()
     {
         if (!kstate) { kstate = std::make_shared<SharedKState>(); wfbErrChk(wfb_kstate_create(&kstate->h, wfb::register_program<prog_t>(), max_keys, grow_keys ? WFB_KEYS_GROW : 0u)); }
-        return new Replica(name, kstate, func, key_extr, max_outputs, parallelism > 1 ? 1 : maxk);
+        return new Replica(name, kstate, params(), max_outputs, parallelism > 1 ? 1 : maxk);
     }
 };
+template <class F, class K> using Map_GPU_KB = Stateful_GPU<F, K, Stateful_Kind_t::MAP>;
+template <class F, class K> using Filter_GPU_KB = Stateful_GPU<F, K, Stateful_Kind_t::FILTER>;
+template <class F, class K> using FlatMap_GPU_KB = Stateful_GPU<F, K, Stateful_Kind_t::FLATMAP>;
 
 // Reduce_GPU (wf/reduce_gpu.hpp:109-289): per batch, one item per distinct key (ascending) or one item for the batch.
 template <class reduce_func_gpu_t, class keyextr_func_gpu_t>
@@ -1041,15 +923,11 @@ public:
     reduce_func_gpu_t func; keyextr_func_gpu_t key_extr; uint32_t key_bits = 64; size_t maxk = WF_MAX_BATCHES_PER_CALL;
     Reduce_GPU(reduce_func_gpu_t f, keyextr_func_gpu_t k, size_t p, std::string n, Routing_Mode_t r): Basic_Operator(std::move(n), p, r, 1), func(f), key_extr(k) {}
     std::string getType() const override { return "Reduce_GPU"; }
-    class Replica: public Basic_Replica {
-        using batch_t = Batch_GPU_t<tuple_t>;
-        wfb_engine_t *eng = nullptr; typename prog_t::params_t prm; uint32_t key_bits; size_t maxk;
-        DeferredCounts counts;
-        BatchPool<tuple_t> pool{4 * WF_MAX_BATCHES_PER_CALL};
-        std::vector<batch_t *> in;
-        std::vector<wfb_batch_t> bi, bo;
+    class Replica: public Batch_Replica<tuple_t> {
+        using base_t = Batch_Replica<tuple_t>; using base_t::in; using base_t::bi; using base_t::bo; using base_t::outs; using base_t::stream;
+        wfb_engine_t *eng = nullptr; typename prog_t::params_t prm; uint32_t key_bits;
     public:
-        Replica(std::string n, reduce_func_gpu_t f, keyextr_func_gpu_t k, uint32_t kb, size_t mk): Basic_Replica(std::move(n)), prm{{}, {}, k, {}, {}, f}, key_bits(kb), maxk(mk ? mk : 1) {}
+        Replica(std::string n, reduce_func_gpu_t f, keyextr_func_gpu_t k, uint32_t kb, size_t mk): base_t(std::move(n), mk), prm{{}, {}, k, {}, {}, f}, key_bits(kb) {}
         ~Replica() override { if (eng) wfb_engine_destroy(eng); }
         int svc_init() override
         {
@@ -1057,54 +935,34 @@ public:
             wfbErrChk(wfb_engine_create(&eng, wfb::register_program<prog_t>()));
             wfbErrChk(wfb_engine_set_params(eng, &prm, sizeof(prm)));
             if (key_bits != 64) wfbErrChk(wfb_engine_set_key_bits(eng, key_bits)); // (integral keys: ReduceGPU_Builder::build checks)
-            if (isKeyed) gpuErrChk(counts.init(maxk));
+            if (isKeyed) gpuErrChk(this->counts.init(this->maxk));
             return 0;
         }
         void *svc(void *msg) override
         {
-            drain(msg, maxk, in);
-            std::vector<batch_t *> work;
-            for (auto *b : in) { if (b->isPunct()) { run(work); this->ff_send_out(b); } else if (b->getSize() == 0) recycleBatch(b); else work.push_back(b); }
-            run(work);
-            return this->GO_ON;
-        }
-    private:
-        void run(std::vector<batch_t *> &work)
-        {
-            if (work.empty()) return;
-            wait_inputs(work);
-            const size_t k = work.size();
-            bi.resize(k); bo.resize(k);
-            std::vector<batch_t *> outs(k);
-            CountBlock *blk = nullptr; uint32_t *counts_d = nullptr;
-            if (isKeyed) gpuErrChk(counts.acquire(static_cast<uint32_t>(k), blk, counts_d));
-            uint32_t kbits = 0; while ((1ull << kbits) < k) kbits++;
-            for (size_t i = 0; i < k; i++) {
-                batch_t *o = pool.get(isKeyed ? work[i]->original_size : 1);
-                o->watermarks = work[i]->watermarks;
-                if (o->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, o->reuse_after, 0));
-                bi[i] = wfb_batch_t{work[i]->tuples_gpu, work[i]->ts_gpu, work[i]->getWatermark(), static_cast<uint32_t>(work[i]->size), 0};
-                bo[i] = wfb_batch_t{o->tuples_gpu, o->ts_gpu, work[i]->getWatermark(), bi[i].n, 0};
-                outs[i] = o;
-            }
+            if (!this->take(msg, true)) return this->GO_ON;
+            const size_t k = in.size();
             if constexpr (isKeyed) {
+                uint32_t kbits = 0; while ((1ull << kbits) < k) kbits++;
                 const uint32_t sort_bits = integral_key_v<keyextr_func_gpu_t> ? key_bits : 32u; // other keys are sorted by their 32-bit rank
-                if (k > 1 && sort_bits + kbits <= 64) { wfbErrChk(wfb_reduce_by_key_batches(eng, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream)); }
-                else for (size_t i = 0; i < k; i++)
-                    wfbErrChk(wfb_reduce_by_key(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), counts_d + i, stream));
-                gpuErrChk(cudaMemcpyAsync(blk->h, counts_d, sizeof(uint32_t) * k, cudaMemcpyDeviceToHost, stream));
-            } else {
-                for (size_t i = 0; i < k; i++) wfbErrChk(wfb_reduce_all(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), stream));
+                this->send_deferred(1, 0, [&](uint32_t *counts_d) {
+                    if (k > 1 && sort_bits + kbits <= 64) { wfbErrChk(wfb_reduce_by_key_batches(eng, bi.data(), bo.data(), static_cast<uint32_t>(k), counts_d, stream)); }
+                    else for (size_t i = 0; i < k; i++)
+                        wfbErrChk(wfb_reduce_by_key(eng, bi[i].tuples, bi[i].ts, bi[i].n, const_cast<void *>(bo[i].tuples), const_cast<uint64_t *>(bo[i].ts), counts_d + i, stream));
+                });
+            } else { // one item per batch: the output's size, 1, is known on the host
+                outs.resize(k);
+                for (size_t i = 0; i < k; i++) outs[i] = this->output_for(in[i], 1);
+                for (size_t i = 0; i < k; i++) wfbErrChk(wfb_reduce_all(eng, bi[i].tuples, bi[i].ts, bi[i].n, outs[i]->tuples_gpu, outs[i]->ts_gpu, stream));
+                cudaEvent_t e = this->next_event();
+                gpuErrChk(cudaEventRecord(e, stream));
+                for (size_t i = 0; i < k; i++) {
+                    outs[i]->valid_after = e;
+                    in[i]->reuse_after = e; recycleBatch(in[i]);
+                    this->ff_send_out(outs[i]);
+                }
             }
-            cudaEvent_t e = next_event();
-            gpuErrChk(cudaEventRecord(e, stream));
-            for (size_t i = 0; i < k; i++) {
-                if (isKeyed) outs[i]->defer(work[i]->size, blk, i, e);
-                else { outs[i]->size = 1; outs[i]->valid_after = e; }
-                work[i]->reuse_after = e; recycleBatch(work[i]);
-                this->ff_send_out(outs[i]);
-            }
-            work.clear();
+            return this->GO_ON;
         }
     };
     Replica *make_replica() { return new Replica(name, func, key_extr, key_bits, maxk); }
@@ -1143,17 +1001,15 @@ public:
     }
     std::string getType() const override { return "Ffat_Windows_GPU"; }
     keyextr_func_gpu_t getKeyExtractor() const { return key_extr; }
-    class Replica: public Basic_Replica {
-        using batch_t = Batch_GPU_t<tuple_t>;
+    class Replica: public Batch_Replica<tuple_t, result_t> {
+        using base_t = Batch_Replica<tuple_t, result_t>; using base_t::in; using base_t::bi; using base_t::stream;
         Ffat_Windows_GPU op;
         wfb_ffat_t *ffat = nullptr; typename prog_t::params_t prm;
-        DeferredCounts counts; // (one word per call)
-        BatchPool<result_t> pool{64};
         const bool tb; uint64_t last_wm = 0; size_t cap_hint = 0;
-        std::vector<batch_t *> in;
-        std::vector<wfb_batch_t> bi;
     public:
-        explicit Replica(const Ffat_Windows_GPU &o): Basic_Replica(o.name), op(o), prm{{}, o.pre, o.key_extr, o.lift, o.comb, {}}, tb(o.winType == Win_Type_t::TB) {}
+        // (time-based windows fire per batch watermark: one batch per call)
+        explicit Replica(const Ffat_Windows_GPU &o): base_t(o.name, o.winType == Win_Type_t::TB ? 1 : o.maxk, 64), op(o), prm{{}, o.pre, o.key_extr, o.lift, o.comb, {}},
+            tb(o.winType == Win_Type_t::TB) {}
         ~Replica() override { if (ffat) wfb_ffat_destroy(ffat); }
         int svc_init() override
         {
@@ -1161,25 +1017,20 @@ public:
             wfbErrChk(wfb_ffat_create(&ffat, wfb::register_program<prog_t>(), op.win_len, op.slide_len, static_cast<uint32_t>(op.numWinPerBatch),
                                       op.max_keys, tb ? 1 : 0, op.lateness, (op.dense_keys ? WFB_FFAT_DENSE_KEYS : 0u) | (op.grow_keys ? WFB_KEYS_GROW : 0u)));
             wfbErrChk(wfb_ffat_set_params(ffat, &prm, sizeof(prm)));
-            gpuErrChk(counts.init(1));
+            gpuErrChk(this->counts.init(1)); // (one word per call)
             return 0;
         }
         void *svc(void *msg) override
         {
-            drain(msg, tb ? 1 : op.maxk, in); // (time-based windows fire per batch watermark: one batch per call)
-            std::vector<batch_t *> work;
-            for (auto *b : in) { if (b->isPunct()) recycleBatch(b); else if (b->getSize() == 0) recycleBatch(b); else work.push_back(b); }
-            if (work.empty()) return this->GO_ON;
-            wait_inputs(work);
-            const size_t k = work.size();
-            bi.resize(k);
+            if (!this->take(msg, true)) return this->GO_ON;
+            const size_t k = in.size();
             uint64_t total = 0;
-            for (size_t i = 0; i < k; i++) { bi[i] = wfb_batch_t{work[i]->tuples_gpu, work[i]->ts_gpu, work[i]->getWatermark(), static_cast<uint32_t>(work[i]->size), 0}; total += work[i]->size; }
+            for (auto *b : in) total += b->size;
             // every group that can fire in this call: per key, count-based one per slide*Nb items (+1: the first group); time-based one
             // per slide*Nb time units the watermark advanced since the key was last seen -- bounded here by the whole advance. A growing
             // key table may take new keys in the call: count-based, a new key fires its first group after B = (Nb-1)*slide+win of its
             // items; time-based, one item may be enough, so every item counts as a key
-            const uint64_t wm = work.back()->getWatermark();
+            const uint64_t wm = in.back()->getWatermark();
             const uint64_t nb = op.numWinPerBatch, per = op.slide_len * nb, B = (nb - 1) * op.slide_len + op.win_len;
             const uint64_t keys = wfb_ffat_key_capacity(ffat) + (op.grow_keys ? (tb ? total : total / B) : 0);
             const uint64_t groups = tb ? keys * ((wm > last_wm ? wm - last_wm : 0) / per + 2) + (wm / per + 2)
@@ -1188,19 +1039,18 @@ public:
             cap_hint = std::max(cap_hint, static_cast<size_t>(std::min<uint64_t>(groups * nb, 0x7fffffffull))); // (never shrinks: recycled batches keep fitting)
             const size_t cap = cap_hint;
             if (tb) last_wm = wm;
-            Batch_GPU_t<result_t> *out = pool.get(cap);
-            if (out->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, out->reuse_after, 0));
+            Batch_GPU_t<result_t> *out = this->output_for(in.back(), cap); // (with the watermark of the call's last batch)
             CountBlock *blk; uint32_t *count_d;
-            gpuErrChk(counts.acquire(1, blk, count_d));
+            gpuErrChk(this->counts.acquire(1, blk, count_d));
             const wfb_functors_t *pre = op.has_pre() ? reinterpret_cast<const wfb_functors_t *>(&prm) : nullptr;
             if (tb) { wfbErrChk(wfb_ffat_process_tb(ffat, pre, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), count_d, stream)); }
             else { wfbErrChk(wfb_ffat_process_cb(ffat, pre, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), count_d, stream)); }
             if (tb) check_errors(); // (the time-based path synchronises per batch anyway: a result that did not fit is reported, not lost silently)
             gpuErrChk(cudaMemcpyAsync(blk->h, count_d, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-            cudaEvent_t e = next_event();
+            cudaEvent_t e = this->next_event();
             gpuErrChk(cudaEventRecord(e, stream));
-            out->defer(cap, blk, 0, e); out->setWatermark(wm);
-            for (auto *b : work) { b->reuse_after = e; recycleBatch(b); }
+            out->defer(cap, blk, 0, e);
+            for (auto *b : in) { b->reuse_after = e; recycleBatch(b); }
             this->ff_send_out(out);
             return this->GO_ON;
         }
@@ -1208,8 +1058,8 @@ public:
         {
             uint32_t nkeys = 0, err = 0;
             if (ffat) wfbErrChk(wfb_ffat_stats(ffat, &nkeys, &err, stream));
-            if (err & 1u) wf_fatal("Ffat_Windows_GPU [" + opName + "]: more distinct keys than withMaxKeys(" + std::to_string(op.max_keys) + ")");
-            if (err & ~1u) wf_fatal("Ffat_Windows_GPU [" + opName + "]: more window results in one call than the output batch holds");
+            if (err & 1u) wf_fatal("Ffat_Windows_GPU [" + this->opName + "]: more distinct keys than withMaxKeys(" + std::to_string(op.max_keys) + ")");
+            if (err & ~1u) wf_fatal("Ffat_Windows_GPU [" + this->opName + "]: more window results in one call than the output batch holds");
         }
         void eosnotify(ssize_t id) override
         {   // nothing is flushed at end of stream (wf/ffat_replica_gpu.hpp:1050-1056); errors raised on the device surface here
@@ -1221,16 +1071,29 @@ public:
 };
 
 // ---- builders (wf/builders_gpu.hpp) ----------------------------------------------------------------------------------------
-template <class map_func_gpu_t, class keyextr_func_gpu_t>
-class MapGPU_KB_Builder { // MapGPU_Builder(func).withKeyBy(key_extr): the keyed-stateful operator
-    map_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
+// MapGPU_Builder / FilterGPU_Builder / FlatMapGPU_Builder(func).withKeyBy(key_extr): the keyed-stateful operator
+template <class func_t, class keyextr_func_gpu_t, Stateful_Kind_t KIND>
+class StatefulGPU_Builder {
+    func_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
+    uint32_t max_outputs; // (FlatMap)
 public:
-    MapGPU_KB_Builder(map_func_gpu_t f, keyextr_func_gpu_t k, std::string n, size_t p): func(f), key(k), name(std::move(n)), parallelism(p) {}
+    StatefulGPU_Builder(func_t f, keyextr_func_gpu_t k, std::string n, size_t p, uint32_t m = 0): func(f), key(k), name(std::move(n)), parallelism(p), max_outputs(m) {}
     auto &withName(std::string n) { name = std::move(n); return *this; }
     auto &withParallelism(size_t p) { parallelism = p; return *this; }
     auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; } // capacity of the device key -> state table (the initial one withKeyGrowth())
     auto &withKeyGrowth() { grow = true; return *this; } // extension: the table grows with the keys, as the reference's map does on the host
-    auto build() { Map_GPU_KB<map_func_gpu_t, keyextr_func_gpu_t> m(func, key, parallelism, name, max_keys); m.grow_keys = grow; return m; }
+    auto &withMaxOutputsPerTuple(uint32_t m) // required by a FlatMap: the output batches hold original_size * m records
+    {
+        static_assert(KIND == Stateful_Kind_t::FLATMAP, "WindFlow Compilation Error - withMaxOutputsPerTuple() belongs to FlatMapGPU_Builder");
+        max_outputs = m; return *this;
+    }
+    auto build()
+    {
+        if (KIND == Stateful_Kind_t::FLATMAP && max_outputs == 0) wf_fatal("FlatMapGPU_Builder [" + name + "]: withMaxOutputsPerTuple(m >= 1) is required");
+        Stateful_GPU<func_t, keyextr_func_gpu_t, KIND> op(func, key, parallelism, name, max_keys, max_outputs);
+        op.grow_keys = grow;
+        return op;
+    }
 };
 
 template <class map_func_gpu_t>
@@ -1249,25 +1112,13 @@ public:
     template <class keyextr_t> auto withKeyBy(keyextr_t k)
     {
         static_assert(arity == 2, "WindFlow Compilation Error - MapGPU_Builder: withKeyBy() needs the stateful signature void(tuple_t &, state_t &)");
-        return MapGPU_KB_Builder<map_func_gpu_t, keyextr_t>(func, k, name, parallelism);
+        return StatefulGPU_Builder<map_func_gpu_t, keyextr_t, Stateful_Kind_t::MAP>(func, k, name, parallelism);
     }
     auto build()
     {
         static_assert(arity == 1, "WindFlow Compilation Error - MapGPU_Builder: a stateful functor needs withKeyBy()");
         return Map_GPU<map_func_gpu_t>(func, parallelism, name, mode);
     }
-};
-
-template <class filter_func_gpu_t, class keyextr_func_gpu_t>
-class FilterGPU_KB_Builder {
-    filter_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
-public:
-    FilterGPU_KB_Builder(filter_func_gpu_t f, keyextr_func_gpu_t k, std::string n, size_t p): func(f), key(k), name(std::move(n)), parallelism(p) {}
-    auto &withName(std::string n) { name = std::move(n); return *this; }
-    auto &withParallelism(size_t p) { parallelism = p; return *this; }
-    auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; }
-    auto &withKeyGrowth() { grow = true; return *this; } // extension: the key -> state table grows with the keys
-    auto build() { Filter_GPU_KB<filter_func_gpu_t, keyextr_func_gpu_t> m(func, key, parallelism, name, max_keys); m.grow_keys = grow; return m; }
 };
 
 template <class filter_func_gpu_t>
@@ -1286,33 +1137,12 @@ public:
     template <class keyextr_t> auto withKeyBy(keyextr_t k)
     {
         static_assert(arity == 2, "WindFlow Compilation Error - FilterGPU_Builder: withKeyBy() needs the stateful signature bool(tuple_t &, state_t &)");
-        return FilterGPU_KB_Builder<filter_func_gpu_t, keyextr_t>(func, k, name, parallelism);
+        return StatefulGPU_Builder<filter_func_gpu_t, keyextr_t, Stateful_Kind_t::FILTER>(func, k, name, parallelism);
     }
     auto build()
     {
         static_assert(arity == 1, "WindFlow Compilation Error - FilterGPU_Builder: a stateful functor needs withKeyBy()");
         return Filter_GPU<filter_func_gpu_t>(func, parallelism, name, mode);
-    }
-};
-
-template <class flatmap_func_gpu_t, class keyextr_func_gpu_t>
-class FlatMapGPU_KB_Builder { // FlatMapGPU_Builder(func).withKeyBy(key_extr): the keyed-stateful operator
-    flatmap_func_gpu_t func; keyextr_func_gpu_t key; std::string name; size_t parallelism; uint32_t max_keys = 1u << 16; bool grow = false;
-    uint32_t max_outputs;
-public:
-    FlatMapGPU_KB_Builder(flatmap_func_gpu_t f, keyextr_func_gpu_t k, std::string n, size_t p, uint32_t m)
-        : func(f), key(k), name(std::move(n)), parallelism(p), max_outputs(m) {}
-    auto &withName(std::string n) { name = std::move(n); return *this; }
-    auto &withParallelism(size_t p) { parallelism = p; return *this; }
-    auto &withMaxKeys(uint32_t mk) { max_keys = mk; return *this; } // capacity of the device key -> state table (the initial one withKeyGrowth())
-    auto &withKeyGrowth() { grow = true; return *this; } // extension: the table grows with the keys
-    auto &withMaxOutputsPerTuple(uint32_t m) { max_outputs = m; return *this; } // required: the output batches hold original_size * m records
-    auto build()
-    {
-        if (max_outputs == 0) wf_fatal("FlatMapGPU_Builder [" + name + "]: withMaxOutputsPerTuple(m >= 1) is required");
-        FlatMap_GPU_KB<flatmap_func_gpu_t, keyextr_func_gpu_t> op(func, key, parallelism, name, max_keys, max_outputs);
-        op.grow_keys = grow;
-        return op;
     }
 };
 
@@ -1344,7 +1174,7 @@ public:
     {
         static_assert(arity == 3, "WindFlow Compilation Error - FlatMapGPU_Builder: withKeyBy() needs the stateful signature "
                                   "void(const tuple_t &, Shipper_GPU<result_t> &, state_t &)");
-        return FlatMapGPU_KB_Builder<flatmap_func_gpu_t, keyextr_t>(func, k, name, parallelism, max_outputs);
+        return StatefulGPU_Builder<flatmap_func_gpu_t, keyextr_t, Stateful_Kind_t::FLATMAP>(func, k, name, parallelism, max_outputs);
     }
     auto build()
     {
@@ -1477,9 +1307,7 @@ public:
     // can fill while it works (the replica then takes everything queued in one call)
     // (stateless operators return a proxy that remembers the functor types while the expression goes on: FusedPipe below)
     template <class F, bool IS> FusedPipe<Stateless_GPU<F, IS>> chain(Stateless_GPU<F, IS> op);
-    template <class F, class K> MultiPipe &chain(Map_GPU_KB<F, K> op) { return add_replicated(op); }
-    template <class F, class K> MultiPipe &chain(Filter_GPU_KB<F, K> op) { return add_replicated(op); }
-    template <class F, class K> MultiPipe &chain(FlatMap_GPU_KB<F, K> op) { return add_replicated(op); }
+    template <class F, class K, Stateful_Kind_t KIND> MultiPipe &chain(Stateful_GPU<F, K, KIND> op) { return add_replicated(op); }
     template <class F, class K> MultiPipe &chain(Reduce_GPU<F, K> op) { return add_replicated(op); }
     template <class F> MultiPipe &chain(FlatMap_GPU<F> op)
     {
