@@ -232,6 +232,30 @@ struct FacadeStatefulFlatMapProgram {
         FlatF f = p.fm; f(t, sh, st);
     }
 };
+// The program of a Keyed_Windows_GPU: func(const Iterable_GPU<tuple_t> &, result_t &) over each count-based window of a key
+// (wf/keyed_windows.hpp, non-incremental and non-riched); the result starts as result_t(key, gwid) when that constructor exists
+template <class T> using Iterable_GPU = wfb::Iterable_GPU<T>; // size(), operator[], at(), front(), back(), begin() / end() (wf/iterable.hpp)
+template <class T, class R, class WinF, class KeyF, bool KEYED>
+struct FacadeKeyedWindowsProgram {
+    using tuple_t = T; using result_t = R; using key_t = key_of_t<KeyF>;
+    struct params_t { WinF win; KeyF key; };
+    static_assert(std::is_trivially_copyable<T>::value && std::is_trivially_copyable<R>::value, "tuple_t / result_t must be trivially copyable");
+    static_assert(sizeof(T) % 8 == 0 && sizeof(R) % 8 == 0, "tuple_t / result_t sizes must be multiples of 8 bytes");
+    __host__ __device__ static void map(tuple_t &, const params_t &) {}
+    __host__ __device__ static bool filter(tuple_t &, const params_t &) { return true; }
+    __host__ __device__ static key_t key(const tuple_t &t, const params_t &p) { KeyF f = p.key; return f(t); }
+    __host__ __device__ static void lift(const tuple_t &, result_t &, const params_t &) {}
+    __host__ __device__ static void comb(const result_t &, const result_t &, result_t &, const params_t &) {}
+    __host__ __device__ static result_t make_result(key_t k, uint64_t gwid, const params_t &p)
+    {
+        return FacadeProgram<T, R, KeyF, NoLift<T, R>, NoComb<R>, NoReduce<T>, KEYED>::make_result(k, gwid, {{}, {}, p.key, {}, {}, {}});
+    }
+    __host__ __device__ static tuple_t reduce(const tuple_t &a, const tuple_t &, const params_t &) { return a; }
+    __host__ __device__ static void win_func(const Iterable_GPU<tuple_t> &w, result_t &r, const params_t &p) { WinF f = p.win; f(w, r); }
+};
+template <class X> struct iterable_tuple;
+template <class T> struct iterable_tuple<wfb::Iterable_GPU<T>> { using type = T; };
+
 template <class T, class S> struct StatefulIdMap { __host__ __device__ void operator()(T &, S &) const {} };
 template <class T, class S> struct StatefulKeepAll { __host__ __device__ bool operator()(T &, S &) const { return true; } };
 
@@ -1070,7 +1094,102 @@ public:
     Replica *make_replica() { return new Replica(*this); }
 };
 
-// ---- builders (wf/builders_gpu.hpp) ----------------------------------------------------------------------------------------
+// Keyed_Windows_GPU, count-based (wf/keyed_windows.hpp, wf/window_replica.hpp): func(const Iterable_GPU<tuple_t> &, result_t &) over
+// every window of every key, the key's last pow2ceil(win) tuples kept on the device. svc(): the K batches found queued go to ONE
+// wfb_kwin_process_cb call, whose results form one output batch whose size stays on the device; at end of stream the windows that
+// opened and did not fire are evaluated on the tuples they have (wf/window_replica.hpp:356-407) and sent as one more batch.
+template <class win_func_gpu_t, class keyextr_func_gpu_t>
+class Keyed_Windows_GPU: public Basic_Operator {
+public:
+    using tuple_t = typename iterable_tuple<fn_arg_t<win_func_gpu_t, 0>>::type;
+    using result_t = fn_arg_t<win_func_gpu_t, 1>;
+    static constexpr bool isKeyed = !std::is_same<keyextr_func_gpu_t, NoKey<tuple_t>>::value;
+    using prog_t = FacadeKeyedWindowsProgram<tuple_t, result_t, win_func_gpu_t, keyextr_func_gpu_t, isKeyed>;
+    static constexpr op_type_t op_type = op_type_t::WIN_GPU;
+    win_func_gpu_t func; keyextr_func_gpu_t key_extr; uint64_t win_len, slide_len; uint32_t max_keys; size_t maxk;
+    Keyed_Windows_GPU(win_func_gpu_t f, keyextr_func_gpu_t k, std::string n, uint64_t w, uint64_t s, uint32_t mk, size_t mbpc):
+        Basic_Operator(std::move(n), 1, isKeyed ? Routing_Mode_t::KEYBY : Routing_Mode_t::FORWARD, 1), func(f), key_extr(k),
+        win_len(w), slide_len(s), max_keys(mk), maxk(mbpc ? mbpc : 1)
+    {
+        static_assert(std::is_trivially_copyable<win_func_gpu_t>::value, "GPU functors must be trivially copyable");
+        if (win_len == 0 || slide_len == 0) wf_fatal("Keyed_Windows_GPU used with window length or slide equal to zero");
+    }
+    std::string getType() const override { return "Keyed_Windows_GPU"; }
+    keyextr_func_gpu_t getKeyExtractor() const { return key_extr; }
+    class Replica: public Batch_Replica<tuple_t, result_t> {
+        using base_t = Batch_Replica<tuple_t, result_t>; using base_t::in; using base_t::bi; using base_t::stream;
+        Keyed_Windows_GPU op;
+        wfb_kwin_t *kw = nullptr; typename prog_t::params_t prm;
+        size_t cap_hint = 0, eos_seen = 0; uint64_t last_wm = 0;
+        // one output batch of capacity `cap` whose size `call(count_d)` leaves on the device
+        template <class Call> void send_results(size_t cap, uint64_t wm, Call &&call)
+        {
+            Batch_GPU_t<result_t> *out = this->pool.get(cap);
+            out->setWatermark(wm);
+            if (out->reuse_after) gpuErrChk(cudaStreamWaitEvent(stream, out->reuse_after, 0));
+            CountBlock *blk; uint32_t *count_d;
+            gpuErrChk(this->counts.acquire(1, blk, count_d));
+            wfbErrChk(call(out, count_d));
+            gpuErrChk(cudaMemcpyAsync(blk->h, count_d, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+            cudaEvent_t e = this->next_event();
+            gpuErrChk(cudaEventRecord(e, stream));
+            out->defer(cap, blk, 0, e);
+            for (auto *b : in) { b->reuse_after = e; recycleBatch(b); }
+            in.clear();
+            this->ff_send_out(out);
+        }
+    public:
+        explicit Replica(const Keyed_Windows_GPU &o): base_t(o.name, o.maxk, 64), op(o), prm{o.func, o.key_extr} {}
+        ~Replica() override { if (kw) wfb_kwin_destroy(kw); }
+        int svc_init() override
+        {
+            Basic_Replica::svc_init();
+            wfbErrChk(wfb_kwin_create(&kw, wfb::register_program<prog_t>(), op.win_len, op.slide_len, op.max_keys, 0));
+            wfbErrChk(wfb_kwin_set_params(kw, &prm, sizeof(prm)));
+            gpuErrChk(this->counts.init(1)); // (one word per call)
+            return 0;
+        }
+        void *svc(void *msg) override
+        {
+            if (!this->take(msg, true)) return this->GO_ON;
+            uint64_t total = 0;
+            for (auto *b : in) total += b->size;
+            // every window the call can fire: per key, at most one per slide items of its run, plus one
+            const uint64_t groups = total / op.slide_len + wfb_kwin_key_capacity(kw) + 1;
+            cap_hint = std::max(cap_hint, static_cast<size_t>(std::min<uint64_t>(groups, 0x7fffffffull))); // (never shrinks: recycled batches keep fitting)
+            const size_t cap = cap_hint, k = in.size();
+            last_wm = in.back()->getWatermark();
+            send_results(cap, last_wm, [&](Batch_GPU_t<result_t> *out, uint32_t *count_d) {
+                return wfb_kwin_process_cb(kw, bi.data(), static_cast<uint32_t>(k), out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), count_d, stream);
+            });
+            return this->GO_ON;
+        }
+        void check_errors()
+        {
+            uint32_t nkeys = 0, err = 0;
+            if (kw) wfbErrChk(wfb_kwin_stats(kw, &nkeys, &err, stream));
+            if (err & 1u) wf_fatal("Keyed_Windows_GPU [" + this->opName + "]: more distinct keys than withMaxKeys(" + std::to_string(op.max_keys) + ")");
+            if (err & ~1u) wf_fatal("Keyed_Windows_GPU [" + this->opName + "]: more window results in one call than the output batch holds");
+        }
+        void eosnotify(ssize_t id) override
+        {   // once every input has ended: the open windows of every key (at most ceil(win / slide) each), then the errors raised on the device
+            const size_t nin = this->worker_ ? this->worker_->in.size() : 1;
+            if (id >= 0 && ++eos_seen < nin) return;
+            uint32_t nkeys = 0, err = 0;
+            wfbErrChk(wfb_kwin_stats(kw, &nkeys, &err, stream));
+            const size_t cap = std::max<size_t>(1, static_cast<size_t>(nkeys) * ((op.win_len + op.slide_len - 1) / op.slide_len));
+            in.clear();
+            send_results(cap, last_wm, [&](Batch_GPU_t<result_t> *out, uint32_t *count_d) {
+                return wfb_kwin_flush(kw, out->tuples_gpu, out->ts_gpu, static_cast<uint32_t>(cap), count_d, stream);
+            });
+            check_errors();
+            Basic_Replica::eosnotify(id);
+        }
+    };
+    Replica *make_replica() { return new Replica(*this); }
+};
+
+// ---- builders (wf/builders_gpu.hpp)----------------------------------------------------------------------------------------
 // MapGPU_Builder / FilterGPU_Builder / FlatMapGPU_Builder(func).withKeyBy(key_extr): the keyed-stateful operator
 template <class func_t, class keyextr_func_gpu_t, Stateful_Kind_t KIND>
 class StatefulGPU_Builder {
@@ -1247,6 +1366,41 @@ public:
     }
 };
 
+// Keyed_WindowsGPU_Builder(win_func).withKeyBy(k).withCBWindows(w, s): win_func is __host__ __device__
+// void(const Iterable_GPU<tuple_t> &, result_t &) (wf/builders.hpp, Keyed_Windows_Builder); without withKeyBy every tuple has one key
+// (and withMaxKeys is ignored)
+template <class win_func_gpu_t, class keyextr_func_gpu_t = NoKey<typename iterable_tuple<fn_arg_t<win_func_gpu_t, 0>>::type>>
+class Keyed_WindowsGPU_Builder {
+    template <class A, class B> friend class Keyed_WindowsGPU_Builder;
+    win_func_gpu_t func; keyextr_func_gpu_t key_extr; std::string name = "keyed_windows_gpu";
+    uint64_t win_len = 0, slide_len = 0; uint32_t max_keys = 65536; size_t max_batches = WF_MAX_BATCHES_PER_CALL;
+    Keyed_WindowsGPU_Builder(win_func_gpu_t f, keyextr_func_gpu_t k): func(f), key_extr(k) {}
+    using args_t = typename fn_sig<win_func_gpu_t>::args;
+public:
+    explicit Keyed_WindowsGPU_Builder(win_func_gpu_t f): func(f), key_extr()
+    {
+        static_assert(std::tuple_size<args_t>::value == 2 && std::is_same<fn_ret_t<win_func_gpu_t>, void>::value &&
+                      std::is_same<std::tuple_element_t<0, args_t>, const Iterable_GPU<typename iterable_tuple<fn_arg_t<win_func_gpu_t, 0>>::type> &>::value &&
+                      std::is_same<std::tuple_element_t<1, args_t>, fn_arg_t<win_func_gpu_t, 1> &>::value,
+                      "WindFlow Compilation Error - Keyed_WindowsGPU_Builder: __host__ __device__ void(const Iterable_GPU<tuple_t> &, result_t &)");
+    }
+    auto &withName(std::string n) { name = std::move(n); return *this; }
+    template <class new_keyextr_t> auto withKeyBy(new_keyextr_t k)
+    {
+        Keyed_WindowsGPU_Builder<win_func_gpu_t, new_keyextr_t> nb(func, k);
+        nb.name = name; nb.win_len = win_len; nb.slide_len = slide_len; nb.max_keys = max_keys; nb.max_batches = max_batches;
+        return nb;
+    }
+    auto &withCBWindows(uint64_t w, uint64_t s) { win_len = w; slide_len = s; return *this; }
+    auto &withMaxKeys(uint32_t n) { max_keys = n; return *this; }            // extension: capacity of the device key table and archive
+    auto &withMaxBatchesPerCall(size_t k) { max_batches = k; return *this; } // extension: queued batches one svc() hands to one launch sequence
+    auto build()
+    {   // (without withKeyBy every tuple has the one key: a table, a ring and an output bound for one key)
+        using op_t = Keyed_Windows_GPU<win_func_gpu_t, keyextr_func_gpu_t>;
+        return op_t(func, key_extr, name, win_len, slide_len, op_t::isKeyed ? max_keys : 1u, max_batches);
+    }
+};
+
 // ---- MultiPipe / PipeGraph (wf/multipipe.hpp, wf/pipegraph.hpp) ------------------------------------------------------------------------
 // A MultiPipe is a sequence of stages; a stage is the group of replicas of one operator (ff_group), consecutive stages are connected
 // all-to-all by the runtime (a producer sends a batch to ONE consumer replica, round-robin: batches are the unit of routing on the
@@ -1309,6 +1463,7 @@ public:
     template <class F, bool IS> FusedPipe<Stateless_GPU<F, IS>> chain(Stateless_GPU<F, IS> op);
     template <class F, class K, Stateful_Kind_t KIND> MultiPipe &chain(Stateful_GPU<F, K, KIND> op) { return add_replicated(op); }
     template <class F, class K> MultiPipe &chain(Reduce_GPU<F, K> op) { return add_replicated(op); }
+    template <class F, class K> MultiPipe &chain(Keyed_Windows_GPU<F, K> op) { return add_replicated(op); } // (a pending stateless run is materialised in front)
     template <class F> MultiPipe &chain(FlatMap_GPU<F> op)
     {
         using T = typename FlatMap_GPU<F>::tuple_t;

@@ -183,6 +183,37 @@ int wfb_filter_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batc
 int wfb_flatmap_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h,
                          uint32_t nbatches, uint32_t max_per_tuple, uint32_t *n_out_dev, void *stream);
 
+/* ---- Keyed_Windows_GPU, count-based: a window function that iterates every tuple of the window --------------------------------
+ * The program's win_func(const Iterable_GPU<tuple_t> &, result_t &, const params_t &) (wfb_kernels.cuh) sees the window's tuples in
+ * arrival order. Per key, tuples get ids 0, 1, 2, ... in arrival order (batch order, then index order); window g holds ids
+ * [g*slide, g*slide + win) and fires when the first tuple after it, id g*slide + win, arrives (sliding, tumbling and hopping windows
+ * alike, wf/window_structure.hpp:69-80). Its result starts as make_result(key, g) and carries the timestamp of the tuple that fired it
+ * (the DETERMINISTIC-mode rule, wf/window_replica.hpp:331).
+ * The handle keeps, per key, its count and a ring of its last pow2ceil(win) tuples on the device. A key's results come out in window
+ * order; the order across keys is unspecified. max_keys up to 2^30, win up to 2^24, slide up to 2^40, max_keys * pow2ceil(win) * sizeof(tuple_t) bytes
+ * of ring (WFB_E_UNSUPPORTED above; a failed allocation returns the CUDA error). flags: 0 or WFB_FFAT_DENSE_KEYS (integral keys).
+ * A key that finds no slot raises error bit 0 and its tuples are dropped; every other key's windows stay exact.
+ * Programs without win_func: WFB_E_UNSUPPORTED; win or slide 0: WFB_E_BADARG.
+ * replaces Keyed_Windows + Window_Replica's key descriptors, archives and triggerers, wf/keyed_windows.hpp, wf/window_replica.hpp:84-112. */
+typedef struct wfb_kwin wfb_kwin_t;
+int wfb_kwin_create(wfb_kwin_t **h, int prog, uint64_t win, uint64_t slide, uint32_t max_keys, uint32_t flags);
+int wfb_kwin_destroy(wfb_kwin_t *h);
+/* params_t of a registered program (its key extractor and window function; see wfb_engine_set_params). Until set: all-zero params. */
+int wfb_kwin_set_params(wfb_kwin_t *h, const void *params, size_t bytes);
+/* K queued batches (at most 2^31 - 1 tuples per call; ts may be NULL: timestamps 0): every window fired by them is evaluated; results
+ * and timestamps go to out_results / out_ts (out_ts may be NULL), *n_out_dev = min(results, out_capacity); more results than
+ * out_capacity raise error bit 1 and nothing is written beyond it. K batches per call give the results of K single-batch calls.
+ * replaces Window_Replica::svc / process_input, wf/window_replica.hpp:175-352. */
+int wfb_kwin_process_cb(wfb_kwin_t *h, const wfb_batch_t *batches_h, uint32_t nbatches, void *out_results, uint64_t *out_ts,
+                        uint32_t out_capacity, uint32_t *n_out_dev, void *stream);
+/* End of stream: every window of every key that opened (its first tuple arrived) and has not fired -- a complete window whose firing
+ * tuple never came included -- is evaluated on the tuples of it that arrived, with the largest timestamp the handle has seen (wf/window_replica.hpp:356-407). Call once, after the last batch. */
+int wfb_kwin_flush(wfb_kwin_t *h, void *out_results, uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, void *stream);
+/* Distinct keys holding a slot (0 on a WFB_FFAT_DENSE_KEYS handle, whose slot is the key) / error flags (bit 0 a key found no slot, bit 1 more results than out_capacity); synchronises the stream. */
+int wfb_kwin_stats(wfb_kwin_t *h, uint32_t *n_keys_h, uint32_t *err_flags_h, void *stream);
+uint32_t wfb_kwin_key_capacity(const wfb_kwin_t *h);
+uint64_t wfb_kwin_launches(const wfb_kwin_t *h);
+
 /* ---- Reduce_GPU, per batch -------------------------------------------------------------------------
  * keyed: one output item per distinct key, ascending key order (floating-point keys: numeric, NaN last; other keys that are not
  * integers: their bytes read as a little-endian unsigned integer), tuple = fold of the program's reduce functor

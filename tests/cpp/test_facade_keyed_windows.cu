@@ -1,0 +1,104 @@
+// Application-level test of Keyed_Windows_GPU in the builder API (include/wf/windflow_gpu.hpp): Source -> Map_GPU -> Filter_GPU ->
+// Keyed_Windows_GPU (count-based, an order-sensitive window function that iterates every tuple of the window) -> Sink, run as
+//   K128  K = 128 batches per call
+//   K1    one batch per call
+//   KS    a keyed-stateful Map_GPU in front of the windows (the pending stateless run is materialised before it)
+// and writes the source's tuples and every run's results, in Sink order, to the directory argv[1]; tests/test_facade_keyed_windows.py
+// folds the tuples with its Python model and compares. Prints KEYED_WINDOWS_OK on success.
+#include <cstdio>
+#include <cstdlib>
+#include <optional>
+#include <string>
+#include <vector>
+#include <wf/windflow_gpu.hpp>
+
+using namespace wf;
+
+constexpr uint64_t N = 40000, BATCH = 500, KEYS = 50, WIN = 12, SLIDE = 5;
+constexpr uint64_t MIX = 0x9E3779B97F4A7C15ull, MUL = 0x100000001B3ull;
+
+struct tup_t { uint64_t key, id; int64_t ivalue; double fvalue; uint64_t pad[4]; };
+struct res_t {
+    uint64_t key, id, hash, size, mid, front, back, distinct; double fsum;
+    __host__ __device__ res_t(): key(0), id(0), hash(0), size(0), mid(0), front(0), back(0), distinct(0), fsum(0) {}
+    __host__ __device__ res_t(uint64_t k, uint64_t g): key(k), id(g), hash(0), size(0), mid(0), front(0), back(0), distinct(0), fsum(0) {}
+};
+struct kstate_t { int64_t c; };
+static_assert(sizeof(tup_t) == 64 && sizeof(res_t) == 72, "record sizes");
+
+static uint64_t mix(uint64_t x) { x ^= x >> 31; x *= 0x7fb5d329728ea185ull; x ^= x >> 27; x *= 0x81dadef4bc2dd44dull; x ^= x >> 33; return x; }
+static tup_t make_tuple(uint64_t i)
+{
+    tup_t t{};
+    t.key = mix(i) % KEYS; t.id = i;
+    t.ivalue = static_cast<int64_t>(mix(i + 99) % 2000) - 1000;
+    t.fvalue = static_cast<double>(mix(i + 7) >> 11) * (1.0 / 9007199254740992.0);
+    return t;
+}
+
+struct Source_Functor {
+    void operator()(Source_Shipper<tup_t> &sh)
+    {
+        for (uint64_t i = 0; i < N; i++) { sh.setNextWatermark(i); sh.pushWithTimestamp(make_tuple(i), i * 3); }
+    }
+};
+struct AddTwo { __host__ __device__ void operator()(tup_t &t) const { t.ivalue += 2; } };
+struct KeepSome { __host__ __device__ bool operator()(tup_t &t) const { return (t.ivalue & 3) != 0; } };
+struct Counter { __host__ __device__ void operator()(tup_t &t, kstate_t &s) const { s.c++; t.ivalue += s.c; } };
+struct Key { __host__ __device__ uint64_t operator()(const tup_t &t) const { return t.key; } };
+// the window function: a polynomial hash over (id, ivalue) through the iterators, size(), the middle tuple, front(), back(), the
+// number of distinct ivalue % 16 and the in-order sum of fvalue
+struct WinF {
+    __host__ __device__ void operator()(const Iterable_GPU<tup_t> &w, res_t &r) const
+    {
+        uint64_t h = 0; double s = 0.0; uint32_t seen = 0;
+        for (auto it = w.begin(); it != w.end(); ++it) {
+            h = h * MUL + (it->id * MIX ^ static_cast<uint64_t>(it->ivalue));
+            s += it->fvalue;
+            seen |= 1u << (static_cast<uint64_t>(it->ivalue) & 15u);
+        }
+        r.hash = h; r.fsum = s; r.size = w.size(); r.mid = w[w.size() / 2].id; r.front = w.front().id; r.back = w.at(w.size() - 1).id;
+        r.distinct = static_cast<uint64_t>(__builtin_popcount(seen));
+    }
+};
+
+static std::vector<res_t> got;
+struct ResSink { void operator()(std::optional<res_t> &r) { if (r) got.push_back(*r); } };
+
+static void write_file(const std::string &path, const void *p, size_t bytes)
+{
+    FILE *f = std::fopen(path.c_str(), "wb");
+    if (!f || std::fwrite(p, 1, bytes, f) != bytes) { std::printf("FAILED writing %s\n", path.c_str()); std::exit(1); }
+    std::fclose(f);
+}
+
+static void run(const std::string &name, size_t k, bool stateful, const std::string &dir)
+{
+    got.clear();
+    PipeGraph graph(name, Execution_Mode_t::DEFAULT, Time_Policy_t::EVENT_TIME);
+    MultiPipe &mp = graph.add_source(Source_Builder(Source_Functor()).withName("source").withOutputBatchSize(BATCH).build());
+    mp.chain(MapGPU_Builder(AddTwo()).withName("add").build());
+    mp.chain(FilterGPU_Builder(KeepSome()).withName("keep").build());
+    if (stateful) mp.chain(MapGPU_Builder(Counter()).withName("counter").withKeyBy(Key()).withMaxKeys(64).build());
+    mp.add(Keyed_WindowsGPU_Builder(WinF()).withName("windows").withKeyBy(Key()).withCBWindows(WIN, SLIDE).withMaxKeys(64)
+               .withMaxBatchesPerCall(k).build());
+    mp.chain_sink(Sink_Builder(ResSink()).withName("sink").build());
+    graph.run();
+    write_file(dir + "/" + name + ".bin", got.data(), got.size() * sizeof(res_t));
+    std::printf("run %s: %zu windows\n", name.c_str(), got.size());
+    if (got.empty()) { std::printf("FAILED run %s: no windows\n", name.c_str()); std::exit(1); }
+}
+
+int main(int argc, char **argv)
+{
+    if (argc < 2) { std::printf("usage: %s OUTPUT_DIR\n", argv[0]); return 2; }
+    const std::string dir = argv[1];
+    std::vector<tup_t> src(N);
+    for (uint64_t i = 0; i < N; i++) src[i] = make_tuple(i);
+    write_file(dir + "/tuples.bin", src.data(), src.size() * sizeof(tup_t));
+    run("K128", 128, false, dir);
+    run("K1", 1, false, dir);
+    run("KS", 128, true, dir);
+    std::printf("KEYED_WINDOWS_OK\n");
+    return 0;
+}

@@ -53,6 +53,14 @@ SYMBOLS = {
     "wfb_map_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), u32, vp]),
     "wfb_filter_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_flatmap_stateful": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, u32, vp, vp]),
+    "wfb_kwin_create": (C.c_int, [C.POINTER(vp), C.c_int, u64, u64, u32, u32]),
+    "wfb_kwin_destroy": (C.c_int, [vp]),
+    "wfb_kwin_set_params": (C.c_int, [vp, vp, C.c_size_t]),
+    "wfb_kwin_process_cb": (C.c_int, [vp, C.POINTER(Batch), u32, vp, vp, u32, vp, vp]),
+    "wfb_kwin_flush": (C.c_int, [vp, vp, vp, u32, vp, vp]),
+    "wfb_kwin_stats": (C.c_int, [vp, C.POINTER(u32), C.POINTER(u32), vp]),
+    "wfb_kwin_key_capacity": (u32, [vp]),
+    "wfb_kwin_launches": (u64, [vp]),
     "wfb_reduce_by_key_batches": (C.c_int, [vp, C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_map_filter_batches": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, vp, vp]),
     "wfb_flatmap_batches": (C.c_int, [vp, C.POINTER(Functors), C.POINTER(Batch), C.POINTER(Batch), u32, u32, vp, vp]),

@@ -23,6 +23,7 @@
 //   k_extract_keys, k_seg_*, k_reduce_segments*, k_reduce_all, k_gather_tuples   KeyBy_Emitter_GPU grouping, Reduce_GPU
 #pragma once
 #include <type_traits>
+#include <iterator>
 #include <cstdint>
 #include <cstring>
 #include <cuda.h>
@@ -3583,6 +3584,250 @@ static __global__ void __launch_bounds__(256) k_fm_offsets(const uint32_t *__res
         const uint32_t gi = first + r;
         if (gi < n) off[gi] = rank - rank_start[batch_of(boff, nb, gi)];
         rank += c[r];
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------
+// Keyed_Windows_GPU, count-based (wf/keyed_windows.hpp, wf/window_replica.hpp:230-407): a window function that iterates every
+// tuple of the window. Per key, tuple ids 0, 1, 2, ... in arrival order; window g holds ids [g*slide, g*slide + win) and fires with the
+// first tuple after it, id g*slide + win (wf/window_structure.hpp:69-80: that tuple is FIRED, not IN). The key's last C = pow2ceil(win)
+// tuples live in its ring (ring + slot * C, id & (C - 1)): a window that has not fired has at most win of its tuples already. Per call the items come sorted by slot (stable: each key's run in arrival order)
+// and are gathered into a staging buffer in that order, so that a window firing in the call reads its older tuples from the ring and
+// the call's own from the staging buffer. Then: windows per run (k_kw_count) -> exclusive scan -> one thread per fired window
+// (k_kw_eval) -> the last C tuples of every run into the ring and the key's count (k_kw_archive).
+// ------------------------------------------------------------------------------------------------------
+
+// Read-only view of one window (wf/iterable.hpp without the mutating overloads): the older part in the key's ring, ids
+// [first_id, first_id + n_ring), then n_stage contiguous tuples of the current call.
+template <class T>
+class Iterable_GPU {
+public:
+    class const_iterator {
+    public:
+        using iterator_category = std::random_access_iterator_tag;
+        using value_type = T; using difference_type = long long; using reference = const T &; using pointer = const T *;
+        __host__ __device__ const_iterator(const Iterable_GPU *it, size_t i) : it_(it), i_(i) {}
+        __host__ __device__ const T &operator*() const { return (*it_)[i_]; }
+        __host__ __device__ const T *operator->() const { return &(*it_)[i_]; }
+        __host__ __device__ const T &operator[](difference_type d) const { return (*it_)[i_ + d]; }
+        __host__ __device__ const_iterator &operator++() { ++i_; return *this; }
+        __host__ __device__ const_iterator operator++(int) { const_iterator o = *this; ++i_; return o; }
+        __host__ __device__ const_iterator &operator--() { --i_; return *this; }
+        __host__ __device__ const_iterator operator--(int) { const_iterator o = *this; --i_; return o; }
+        __host__ __device__ const_iterator &operator+=(difference_type d) { i_ += d; return *this; }
+        __host__ __device__ const_iterator &operator-=(difference_type d) { i_ -= d; return *this; }
+        __host__ __device__ const_iterator operator+(difference_type d) const { return const_iterator(it_, i_ + d); }
+        __host__ __device__ friend const_iterator operator+(difference_type d, const const_iterator &x) { return x + d; }
+        __host__ __device__ const_iterator operator-(difference_type d) const { return const_iterator(it_, i_ - d); }
+        __host__ __device__ difference_type operator-(const const_iterator &o) const { return static_cast<difference_type>(i_) - static_cast<difference_type>(o.i_); }
+        __host__ __device__ bool operator==(const const_iterator &o) const { return i_ == o.i_; }
+        __host__ __device__ bool operator!=(const const_iterator &o) const { return i_ != o.i_; }
+        __host__ __device__ bool operator<(const const_iterator &o) const { return i_ < o.i_; }
+        __host__ __device__ bool operator<=(const const_iterator &o) const { return i_ <= o.i_; }
+        __host__ __device__ bool operator>(const const_iterator &o) const { return i_ > o.i_; }
+        __host__ __device__ bool operator>=(const const_iterator &o) const { return i_ >= o.i_; }
+    private:
+        const Iterable_GPU *it_; size_t i_;
+    };
+    using iterator = const_iterator;
+
+    __host__ __device__ Iterable_GPU(const T *ring, uint32_t mask, uint64_t first_id, uint32_t n_ring, const T *stage, uint32_t n_stage)
+        : ring_(ring), mask_(mask), first_(first_id), n_ring_(n_ring), stage_(stage), n_stage_(n_stage) {}
+    __host__ __device__ size_t size() const { return static_cast<size_t>(n_ring_) + n_stage_; }
+    __host__ __device__ const T &operator[](size_t i) const
+    {
+        return i < n_ring_ ? ring_[(first_ + i) & mask_] : stage_[i - n_ring_];
+    }
+    __host__ __device__ const T &at(size_t i) const { return (*this)[i < size() ? i : size() - 1]; } // (no exceptions on the device: clamped)
+    __host__ __device__ const T &front() const { return (*this)[0]; }
+    __host__ __device__ const T &back() const { return (*this)[size() - 1]; }
+    __host__ __device__ const_iterator begin() const { return const_iterator(this, 0); }
+    __host__ __device__ const_iterator end() const { return const_iterator(this, size()); }
+
+private:
+    const T *ring_; uint32_t mask_; uint64_t first_; uint32_t n_ring_; const T *stage_; uint32_t n_stage_;
+};
+
+// state and geometry of one Keyed_Windows_GPU handle as its kernels see it
+struct KwinDev {
+    unsigned char *ring;     // max_keys * C tuples
+    uint64_t *cnt;           // tuples of each slot so far
+    uint64_t *last_ts;       // largest timestamp seen (the end-of-stream windows carry it)
+    uint64_t win, slide;
+    uint32_t C;              // ring length (power of two >= win)
+    uint32_t max_keys;
+    uint32_t *err_flags;     // bit 0: a key found no slot, bit 1: more results than the output capacity
+    uint32_t *n_slots;       // slots taken (a dense table takes none: slot = key, every slot may hold a key)
+    uint32_t dense;
+};
+
+// the windows g whose firing id g*slide + win lies in [c, c + m) (fired by a run of m tuples on a key that had c): [*g_lo, *g_lo + count)
+__device__ __forceinline__ uint64_t kw_fired(uint64_t c, uint64_t m, uint64_t win, uint64_t slide, uint64_t *g_lo)
+{
+    const uint64_t lo = c > win ? (c - win + slide - 1) / slide : 0;
+    *g_lo = lo;
+    if (c + m <= win) return 0;
+    const uint64_t hi = (c + m - 1 - win) / slide;
+    return hi >= lo ? hi - lo + 1 : 0;
+}
+
+// first index in [lo, hi) whose sorted slot is >= v
+__device__ __forceinline__ uint32_t kw_lower_bound(const uint32_t *__restrict__ a, uint32_t lo, uint32_t hi, uint32_t v)
+{
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < v) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+// staging: tuple and timestamp of every sorted position; the largest timestamp of the call into last_ts
+template <class P>
+__global__ void __launch_bounds__(256) k_kw_stage(const DevBatch *__restrict__ batches, const uint32_t *__restrict__ boff, uint32_t nb, uint32_t n,
+                                                  const uint32_t *__restrict__ sorted_pos, unsigned char *__restrict__ stage,
+                                                  uint64_t *__restrict__ stage_ts, uint64_t *__restrict__ last_ts)
+{
+    using T = typename P::tuple_t;
+    uint64_t mx = 0;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t gi = sorted_pos[j], b = batch_of(boff, nb, gi), li = gi - boff[b];
+        alignas(16) T t;
+        ld_rec<T>(batches[b].tuples + static_cast<size_t>(li) * sizeof(T), t);
+        st_rec<T>(stage + static_cast<size_t>(j) * sizeof(T), t);
+        const uint64_t ts = batches[b].ts != nullptr ? batches[b].ts[li] : 0;
+        stage_ts[j] = ts;
+        mx = ts > mx ? ts : mx;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const uint64_t v = __shfl_xor_sync(FULL, mx, o); mx = v > mx ? v : mx; }
+    if ((threadIdx.x & 31u) == 0 && mx != 0) atomicMax(reinterpret_cast<unsigned long long *>(last_ts), static_cast<unsigned long long>(mx));
+}
+
+// per sorted position: the windows its run fires (run heads only; 0 elsewhere), and the run's length and starting count at its head
+static __global__ void __launch_bounds__(256) k_kw_count(const KwinDev kw, const uint32_t *__restrict__ sorted_slots, uint32_t n,
+                                                         uint32_t *__restrict__ wcnt, uint32_t *__restrict__ run_m, uint64_t *__restrict__ run_c)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t slot = sorted_slots[j];
+        uint32_t w = 0;
+        if (slot < kw.max_keys && (j == 0 || sorted_slots[j - 1] != slot)) {
+            const uint32_t m = kw_lower_bound(sorted_slots, j, n, slot + 1) - j;
+            const uint64_t c = kw.cnt[slot];
+            uint64_t g_lo;
+            w = static_cast<uint32_t>(kw_fired(c, m, kw.win, kw.slide, &g_lo));
+            run_m[j] = m; run_c[j] = c;
+        }
+        wcnt[j] = w;
+    }
+}
+
+// woff[j] = windows of the positions before j (tile_base: the exclusive scan of the SEGT-position tile sums); total -> *n_total
+static __global__ void __launch_bounds__(256) k_kw_offsets(const uint32_t *__restrict__ cnt, const uint32_t *__restrict__ tile_base, uint32_t n,
+                                                           uint32_t *__restrict__ off)
+{
+    __shared__ uint32_t wsum[8];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t first = blockIdx.x * SEGT + tid * (SEGT / 256);
+    uint32_t c[SEGT / 256];
+    uint32_t mine = 0;
+#pragma unroll
+    for (uint32_t r = 0; r < SEGT / 256; r++) { const uint32_t i = first + r; c[r] = i < n ? cnt[i] : 0u; mine += c[r]; }
+    uint32_t incl = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, o); if (lane >= static_cast<uint32_t>(o)) incl += v; }
+    if (lane == 31) wsum[warp] = incl;
+    __syncthreads();
+    uint32_t rank = tile_base[blockIdx.x] + incl - mine;
+    for (uint32_t w = 0; w < warp; w++) rank += wsum[w];
+#pragma unroll
+    for (uint32_t r = 0; r < SEGT / 256; r++) {
+        const uint32_t i = first + r;
+        if (i < n) off[i] = rank;
+        rank += c[r];
+    }
+}
+
+// *n_out = min(total, cap); bit 1 when the results exceed the capacity
+static __global__ void k_kw_clamp(const uint32_t *__restrict__ total, uint32_t cap, uint32_t *__restrict__ n_out, uint32_t *__restrict__ err_flags)
+{
+    const uint32_t t = *total;
+    *n_out = t < cap ? t : cap;
+    if (t > cap) atomicOr(err_flags, 2u);
+}
+
+// one thread per fired window (the first min(total, cap)): its run by binary search over the offsets, its view, the user's function
+template <class P>
+__global__ void __launch_bounds__(128) k_kw_eval(const KwinDev kw, const uint32_t *__restrict__ sorted_slots, uint32_t n,
+                                                 const uint32_t *__restrict__ woff, const uint32_t *__restrict__ run_m, const uint64_t *__restrict__ run_c,
+                                                 const unsigned char *__restrict__ stage, const uint64_t *__restrict__ stage_ts,
+                                                 const uint32_t *__restrict__ n_out, unsigned char *__restrict__ out, uint64_t *__restrict__ out_ts,
+                                                 const typename P::params_t prm)
+{
+    using T = typename P::tuple_t; using R = typename P::result_t;
+    const uint32_t total = *n_out;
+    const T *st = reinterpret_cast<const T *>(stage);
+    for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < total; w += gridDim.x * blockDim.x) {
+        uint32_t lo = 0, hi = n; // last j with woff[j] <= w: the run head whose windows include w
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (woff[mid] <= w) lo = mid; else hi = mid; }
+        const uint32_t j = lo, slot = sorted_slots[j];
+        const uint64_t c = run_c[j];
+        uint64_t g_lo;
+        kw_fired(c, run_m[j], kw.win, kw.slide, &g_lo);
+        const uint64_t g = g_lo + (w - woff[j]), first = g * kw.slide, last = first + kw.win; // ids [first, last)
+        const uint32_t n_ring = first < c ? static_cast<uint32_t>(c - first) : 0u;
+        const uint32_t s0 = j + static_cast<uint32_t>(first > c ? first - c : 0); // staging index of the window's first id of this call
+        const Iterable_GPU<T> it(reinterpret_cast<const T *>(kw.ring) + static_cast<size_t>(slot) * kw.C, kw.C - 1, first, n_ring,
+                                 st + s0, static_cast<uint32_t>(kw.win) - n_ring);
+        R r = P::make_result(P::key(st[j], prm), g, prm);
+        P::win_func(it, r, prm);
+        st_rec<R>(out + static_cast<size_t>(w) * sizeof(R), r);
+        if (out_ts != nullptr) out_ts[w] = stage_ts[j + static_cast<uint32_t>(last - c)]; // (the firing tuple, id `last`, is of this call)
+    }
+}
+
+// after k_kw_eval: the last C tuples of every run into the key's ring; the run's head stores the key's new count
+template <class P>
+__global__ void __launch_bounds__(256) k_kw_archive(const KwinDev kw, const uint32_t *__restrict__ sorted_slots, uint32_t n,
+                                                    const uint32_t *__restrict__ run_m, const uint64_t *__restrict__ run_c,
+                                                    const unsigned char *__restrict__ stage)
+{
+    using T = typename P::tuple_t;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t slot = sorted_slots[j];
+        if (slot >= kw.max_keys) continue;
+        const uint32_t head = kw_lower_bound(sorted_slots, 0, j, slot), r = j - head, m = run_m[head];
+        const uint64_t c = run_c[head];
+        if (static_cast<uint64_t>(r) + kw.C >= m) {
+            alignas(16) T t;
+            ld_rec<T>(stage + static_cast<size_t>(j) * sizeof(T), t);
+            st_rec<T>(kw.ring + (static_cast<size_t>(slot) * kw.C + ((c + r) & (kw.C - 1))) * sizeof(T), t);
+        }
+        if (r == 0) kw.cnt[slot] = c + m;
+    }
+}
+
+// end of stream (wf/window_replica.hpp:356-407): every window of every key that opened (g*slide < count) and has not fired
+// (g*slide + win >= count: also a complete window whose firing tuple never came), on the tuples of it that arrived, with the largest
+// timestamp seen. One thread per key; a key's windows take consecutive results.
+template <class P>
+__global__ void __launch_bounds__(128) k_kw_flush(const KwinDev kw, uint32_t *__restrict__ total, uint32_t cap, unsigned char *__restrict__ out,
+                                                  uint64_t *__restrict__ out_ts, const typename P::params_t prm)
+{
+    using T = typename P::tuple_t; using R = typename P::result_t;
+    const uint32_t nk = kw.dense ? kw.max_keys : min(*kw.n_slots, kw.max_keys);
+    const uint64_t ts = *kw.last_ts;
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < nk; s += gridDim.x * blockDim.x) {
+        const uint64_t c = kw.cnt[s];
+        if (c == 0) continue;
+        const uint64_t g_lo = c > kw.win ? (c - kw.win + kw.slide - 1) / kw.slide : 0, g_hi = (c - 1) / kw.slide; // g*slide <= c-1
+        if (g_hi < g_lo) continue;
+        const T *ring = reinterpret_cast<const T *>(kw.ring) + static_cast<size_t>(s) * kw.C;
+        const uint32_t k = static_cast<uint32_t>(g_hi - g_lo + 1), base = atomicAdd(total, k);
+        for (uint32_t q = 0; q < k && base + q < cap; q++) {
+            const uint64_t g = g_lo + q, first = g * kw.slide;
+            const Iterable_GPU<T> it(ring, kw.C - 1, first, static_cast<uint32_t>(min(c, first + kw.win) - first), nullptr, 0);
+            R r = P::make_result(P::key(it.front(), prm), g, prm);
+            P::win_func(it, r, prm);
+            st_rec<R>(out + static_cast<size_t>(base + q) * sizeof(R), r);
+            if (out_ts != nullptr) out_ts[base + q] = ts;
+        }
     }
 }
 

@@ -123,6 +123,18 @@ struct ProgramOps {
     int (*flatmap)(TileArgs &a, const void *params, uint32_t want_grid, cudaStream_t s, uint32_t *grid_used, uint64_t span_begin, uint64_t span_end);
     // 1: the program has flatmap_stateful (keyed-stateful FlatMap_GPU: ks_apply / ks_apply_runs take KS_FM_COUNT and KS_FM_EMIT)
     uint32_t has_flatmap_stateful, reserved3;
+    // Keyed_Windows_GPU (null when the program has no win_func): the staging gather, the evaluation of the fired windows, the archive
+    // of every run's last tuples and the end-of-stream evaluation
+    int (*kw_stage)(const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n, const uint32_t *sorted_pos, unsigned char *stage,
+                    uint64_t *stage_ts, uint64_t *last_ts, cudaStream_t s);
+    int (*kw_eval)(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *woff, const uint32_t *run_m, const uint64_t *run_c,
+                   const unsigned char *stage, const uint64_t *stage_ts, const uint32_t *n_out, unsigned char *out, uint64_t *out_ts,
+                   uint32_t max_windows, cudaStream_t s, const void *params);
+    int (*kw_archive)(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *run_m, const uint64_t *run_c,
+                      const unsigned char *stage, cudaStream_t s);
+    int (*kw_flush)(const KwinDev &kw, uint32_t *total, uint32_t cap, unsigned char *out, uint64_t *out_ts, cudaStream_t s, const void *params);
+    // 1: the program has win_func (the kw_* entries are set)
+    uint32_t has_win_func, reserved4;
 };
 
 // P::passthrough (optional): map is a no-op and lift the identity (tuple_t == result_t)
@@ -333,6 +345,44 @@ int flatmap_dispatch(TileArgs &a, const void *params, uint32_t want_grid, cudaSt
     return launch_tile_pass<P, MODE_FLATMAP>(a, params, want_grid, s, grid_used, span_begin, span_end);
 }
 
+// P::win_func(const Iterable_GPU<tuple_t> &, result_t &, const params_t &) (optional: Keyed_Windows_GPU)
+template <class P, class = void> struct program_has_win_func : std::false_type {};
+template <class P> struct program_has_win_func<P, std::void_t<decltype(P::win_func(std::declval<const Iterable_GPU<typename P::tuple_t> &>(),
+    std::declval<typename P::result_t &>(), std::declval<const typename P::params_t &>()))>> : std::true_type {};
+template <class P>
+int kw_stage_dispatch(const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n, const uint32_t *sorted_pos, unsigned char *stage,
+                      uint64_t *stage_ts, uint64_t *last_ts, cudaStream_t s)
+{
+    k_kw_stage<P><<<grid_for(n, 256), 256, 0, s>>>(batches, boff, nb, n, sorted_pos, stage, stage_ts, last_ts);
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+template <class P>
+int kw_eval_dispatch(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *woff, const uint32_t *run_m, const uint64_t *run_c,
+                     const unsigned char *stage, const uint64_t *stage_ts, const uint32_t *n_out, unsigned char *out, uint64_t *out_ts,
+                     uint32_t max_windows, cudaStream_t s, const void *params)
+{
+    k_kw_eval<P><<<grid_for(max_windows, 128), 128, 0, s>>>(kw, sorted_slots, n, woff, run_m, run_c, stage, stage_ts, n_out, out, out_ts,
+                                                           load_params<P>(params));
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+template <class P>
+int kw_archive_dispatch(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *run_m, const uint64_t *run_c,
+                        const unsigned char *stage, cudaStream_t s)
+{
+    k_kw_archive<P><<<grid_for(n, 256), 256, 0, s>>>(kw, sorted_slots, n, run_m, run_c, stage);
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+template <class P>
+int kw_flush_dispatch(const KwinDev &kw, uint32_t *total, uint32_t cap, unsigned char *out, uint64_t *out_ts, cudaStream_t s, const void *params)
+{
+    k_kw_flush<P><<<grid_for(kw.max_keys, 128), 128, 0, s>>>(kw, total, cap, out, out_ts, load_params<P>(params));
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+
 template <class P>
 int tb_lift_dispatch(const unsigned char *tuples, const uint64_t *ts, uint32_t n, const FfatDev &ff, const TbDev &tb, uint64_t first_incomplete,
                      unsigned char *lifted, uint64_t *ckeys, cudaStream_t s, const void *params)
@@ -487,6 +537,11 @@ ProgramOps make_ops()
     if constexpr (program_is_lifted<P>::value) o.lifted_ops = nullptr; else o.lifted_ops = &lifted_ops_of<P>;
     if constexpr (program_has_flatmap<P>::value) o.flatmap = &flatmap_dispatch<P>; else o.flatmap = nullptr;
     o.has_flatmap_stateful = program_has_flatmap_stateful<P>::value ? 1u : 0u; o.reserved3 = 0;
+    if constexpr (program_has_win_func<P>::value) {
+        o.kw_stage = &kw_stage_dispatch<P>; o.kw_eval = &kw_eval_dispatch<P>; o.kw_archive = &kw_archive_dispatch<P>; o.kw_flush = &kw_flush_dispatch<P>;
+        o.has_win_func = 1u;
+    } else { o.kw_stage = nullptr; o.kw_eval = nullptr; o.kw_archive = nullptr; o.kw_flush = nullptr; o.has_win_func = 0u; }
+    o.reserved4 = 0;
     return o;
 }
 

@@ -1065,6 +1065,39 @@ int wfb_kstate_destroy(wfb_kstate_t *h)
 
 uint32_t wfb_kstate_key_capacity(const wfb_kstate_t *h) { return h ? h->ff.max_keys : 0; }
 
+} // extern "C" (the template below is C++)
+// The front half of a keyed call over K batches, shared by the keyed-stateful operators and Keyed_Windows_GPU: the batch table and
+// offsets go to the device, every item gets its key's slot (a growing handle grows its key table through `grow` and looks the slots up
+// again), then the (slot, position) pairs are grouped -- into 1024 buckets of consecutive slots by one wide partition pass when
+// h->buckets (counts = the bucket sizes), else by the full stable sort by slot (sorted_slots / sorted_pos). `extra(batch capacity,
+// item capacity)` sizes the handle's own scratch before the first launch.
+template <class H, class Extra, class Grow>
+static int keyed_front(H *h, const void *f, const std::vector<DevBatch> &hb, const std::vector<uint32_t> &boff, uint32_t nbatches, uint32_t n,
+                       cudaStream_t s, Extra &&extra, Grow &&grow, const uint32_t **counts, const uint32_t **sorted_slots, const uint32_t **sorted_pos)
+{
+    CK(h->d_batches.ensure(nbatches, s));
+    const size_t bcap = h->d_batches.capacity();
+    CK(h->d_boff.ensure(nbatches + 1ull, s, bcap + 1));
+    CK(h->slotsA.ensure(n, s));
+    const size_t cap = h->slotsA.capacity();
+    CK(h->slotsB.ensure(n, s, cap)); CK(h->posA.ensure(n, s, cap)); CK(h->posB.ensure(n, s, cap));
+    int rc = extra(bcap, cap); if (rc) return rc;
+    { int rc_ = h->stage.h2d(h->d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
+    { int rc_ = h->stage.h2d(h->d_boff, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
+    rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc;
+    for (bool grew = h->ff.grow != 0; grew; ) {
+        rc = grow(&grew); if (rc) return rc;
+        if (grew) { rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc; h->launches += 2; }
+    }
+    const uint64_t before = h->sorter.launches;
+    if (h->buckets) rc = h->sorter.template sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, counts, nullptr, nullptr, 0, true);
+    else rc = h->sorter.template sort<uint32_t>(h->slotsA, h->slotsB, h->posA, h->posB, nullptr, n, n, h->sort_passes, s, sorted_slots, sorted_pos);
+    if (rc) return rc;
+    h->launches += 1 + (h->sorter.launches - before);
+    return 0;
+}
+extern "C" {
+
 // mode: KS_MAP (in place), KS_FILTER (survivors into out), KS_FM_COUNT (the flatmap: both of its walks, records into out, m per tuple)
 static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_t *in_h, const wfb_batch_t *out_h, uint32_t nbatches,
                       uint32_t *n_out_dev, int mode, uint32_t m, cudaStream_t s)
@@ -1104,38 +1137,29 @@ static int kstate_run(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_batch_
     if (total == 0) return 0;
     if (total > 0x7fffffffull) return WFB_E_BADARG;
     const uint32_t n = static_cast<uint32_t>(total);
-    CK(h->d_batches.ensure(nbatches, s));
-    const size_t bcap = h->d_batches.capacity();
-    CK(h->d_boff.ensure(nbatches + 1ull, s, bcap + 1)); CK(h->rank_start.ensure(nbatches + 1ull, s, bcap + 1));
-    CK(h->slotsA.ensure(n, s));
-    const size_t cap = h->slotsA.capacity();
-    CK(h->slotsB.ensure(n, s, cap)); CK(h->posA.ensure(n, s, cap)); CK(h->posB.ensure(n, s, cap)); CK(h->keep.ensure(n, s, cap));
-    if (flatmap) { CK(h->fm_cnt.ensure(n, s, cap)); CK(h->fm_off.ensure(n, s, cap)); }
-    const size_t cnt_cap = (cap + SEGT - 1) / SEGT + 1;
-    CK(h->tile_cnt.ensure(cnt_cap, s, cnt_cap));
-    { int rc_ = h->stage.h2d(h->d_batches, hb.data(), sizeof(DevBatch) * nbatches, s); if (rc_) return rc_; }
-    { int rc_ = h->stage.h2d(h->d_boff, boff.data(), sizeof(uint32_t) * (nbatches + 1), s); if (rc_) return rc_; }
     // 1. slots; 2. one wide partition pass into 1024 buckets of consecutive slots; 3. per-bucket CTAs, one thread per key
     // (more than 65536 keys: 2. a stable sort by slot; 3. one thread per run of a slot)
-    rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc;
-    for (bool grew = h->ff.grow != 0; grew; ) { // (a growing handle stops at 65536 keys, the last capacity of the bucket path, on its way up)
-        rc = grow_keys(h->ff, h->ops->key_bytes, h->growc, 1u << (OSW_BITS + 6), 1u << 30, s, &grew,
-                       [h](GrowPlan &plan, uint32_t cap) {
-                           const size_t sb = h->ops->state_bytes;
-                           plan.add(h->states, sb * h->ff.max_keys, sb * cap, true, 0); // state_t(): zero-initialised
-                           return 0;
-                       },
-                       [h](uint32_t cap, const GrowPlan &) { kstate_derive_paths(h, cap); return 0; });
-        if (rc) return rc;
-        if (grew) { rc = h->ops->ks_slots(h->d_batches, h->d_boff, nbatches, n, h->ff, h->slotsA, s, f); if (rc) return rc; h->launches += 2; }
-    }
-    const uint64_t before = h->sorter.launches;
-    KsFlatMap fm{h->fm_cnt, h->fm_off, m, flatmap ? n_out_dev + nbatches : nullptr};
     const uint32_t *counts = nullptr, *sorted_slots = nullptr, *sorted_pos = nullptr;
-    if (h->buckets) rc = h->sorter.sort_wide<uint32_t>(h->slotsA, h->slotsB, h->posB, nullptr, n, n, h->bucket_shift, s, nullptr, &counts, nullptr, nullptr, 0, true);
-    else rc = h->sorter.sort<uint32_t>(h->slotsA, h->slotsB, h->posA, h->posB, nullptr, n, n, h->sort_passes, s, &sorted_slots, &sorted_pos);
+    rc = keyed_front(h, f, hb, boff, nbatches, n, s,
+                     [&](size_t bcap, size_t cap) {
+                         CK(h->rank_start.ensure(nbatches + 1ull, s, bcap + 1)); CK(h->keep.ensure(n, s, cap));
+                         if (flatmap) { CK(h->fm_cnt.ensure(n, s, cap)); CK(h->fm_off.ensure(n, s, cap)); }
+                         const size_t cnt_cap = (cap + SEGT - 1) / SEGT + 1;
+                         CK(h->tile_cnt.ensure(cnt_cap, s, cnt_cap));
+                         return 0;
+                     },
+                     [&](bool *grew) { // (a growing handle stops at 65536 keys, the last capacity of the bucket path, on its way up)
+                         return grow_keys(h->ff, h->ops->key_bytes, h->growc, 1u << (OSW_BITS + 6), 1u << 30, s, grew,
+                                          [h](GrowPlan &plan, uint32_t cap) {
+                                              const size_t sb = h->ops->state_bytes;
+                                              plan.add(h->states, sb * h->ff.max_keys, sb * cap, true, 0); // state_t(): zero-initialised
+                                              return 0;
+                                          },
+                                          [h](uint32_t cap, const GrowPlan &) { kstate_derive_paths(h, cap); return 0; });
+                     },
+                     &counts, &sorted_slots, &sorted_pos);
     if (rc) return rc;
-    h->launches += 1 + (h->sorter.launches - before);
+    KsFlatMap fm{h->fm_cnt, h->fm_off, m, flatmap ? n_out_dev + nbatches : nullptr};
     // the walk of `walk` over the partition (both walks of a flatmap visit every key's items in the same order from the same partition)
     auto apply = [&](int walk) {
         h->launches++;
@@ -1179,6 +1203,175 @@ int wfb_flatmap_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_bat
                          uint32_t max_per_tuple, uint32_t *n_out_dev, void *stream)
 {
     return kstate_run(h, f, in_h, out_h, nbatches, n_out_dev, KS_FM_COUNT, max_per_tuple, static_cast<cudaStream_t>(stream));
+}
+
+// ---- Keyed_Windows_GPU, count-based ------------------------------------------------------------------------------------
+} // extern "C"
+struct wfb_kwin {
+    int prog = 0;
+    const ProgramOps *ops = nullptr;
+    FfatDev ff{};                 // key table only (dense or open addressing), as a keyed-stateful handle's
+    KwinDev kw{};                 // ring, counts, geometry
+    std::vector<unsigned char> params;
+    RadixSorter sorter;
+    const bool buckets = false;   // (keyed_front: always the full stable sort by slot, which gives every key's run contiguous)
+    uint32_t bucket_shift = 0, sort_passes = 0;
+    Scratch<DevBatch> d_batches; Scratch<uint32_t> d_boff;
+    Scratch<uint32_t> slotsA, slotsB, posA, posB, wcnt, woff, run_m, tile_cnt, total; // capacity in tuples per call: slotsA's
+    Scratch<uint64_t> run_c, stage_ts;
+    Scratch<unsigned char> staged;                                                      // the call's tuples in sorted order
+    uint64_t launches = 0;
+    PinnedStage stage;
+    StreamOrder order;            // a call on another stream waits for the previous call: the scratch and the archive are shared
+    std::mutex mu;
+};
+extern "C" {
+
+int wfb_kwin_create(wfb_kwin_t **hh, int prog, uint64_t win, uint64_t slide, uint32_t max_keys, uint32_t flags)
+{
+    if (!hh || max_keys == 0 || win == 0 || slide == 0) return WFB_E_BADARG;
+    const ProgramOps *o = program(prog);
+    if (!o) return WFB_E_NOPROG;
+    if (!o->has_win_func) return WFB_E_UNSUPPORTED;  // the program has no win_func
+    if (flags & ~WFB_FFAT_DENSE_KEYS) return WFB_E_UNSUPPORTED;
+    if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
+    if (max_keys > (1u << 30) || win > (1ull << 24) || slide > (1ull << 40)) return WFB_E_UNSUPPORTED; // (window ids g * slide + win stay far below 2^64)
+    uint32_t C = 1; while (C < win) C <<= 1;
+    const unsigned __int128 ring_bytes = static_cast<unsigned __int128>(max_keys) * C * o->tuple_bytes;
+    if (ring_bytes > static_cast<unsigned __int128>(SIZE_MAX)) return WFB_E_UNSUPPORTED;
+    int rc = device_ready(); if (rc) return rc;
+    wfb_kwin *h = new (std::nothrow) wfb_kwin();
+    if (!h) return WFB_E_BADARG;
+    h->prog = prog; h->ops = o;
+    { uint32_t bits = 0; while ((1ull << bits) < max_keys) bits++; h->sort_passes = bits / 8 + 1; } // 8·passes > log2(capacity): INVALID_SLOT sorts last
+    FfatDev &ff = h->ff;
+    ff.max_keys = max_keys; ff.dense = (flags & WFB_FFAT_DENSE_KEYS) ? 1u : 0u;
+    rc = h->order.init(); if (rc) { wfb_kwin_destroy(h); return rc; }
+    uint32_t cap = 1; while (cap < 2ull * max_keys) cap <<= 1;
+    ff.ht_mask = cap - 1;
+#define ALLOC(ptr, bytes) do { cudaError_t e_ = cudaMalloc(reinterpret_cast<void **>(&(ptr)), (bytes)); if (e_ != cudaSuccess) { cudaGetLastError(); wfb_kwin_destroy(h); return static_cast<int>(e_); } } while (0)
+    if (!ff.dense) {
+        ALLOC(ff.ht_keys, static_cast<size_t>(o->key_bytes) * cap); ALLOC(ff.ht_slots, sizeof(uint32_t) * cap);
+        CK(cudaMemset(ff.ht_keys, 0xff, static_cast<size_t>(o->key_bytes) * cap)); CK(cudaMemset(ff.ht_slots, 0xff, sizeof(uint32_t) * cap));
+    }
+    ALLOC(ff.n_slots, sizeof(uint32_t) * 4); ff.err_flags = ff.n_slots + 1;
+    CK(cudaMemset(ff.n_slots, 0, sizeof(uint32_t) * 4));
+    ALLOC(ff.slot_key, static_cast<size_t>(o->key_bytes) * max_keys);
+    KwinDev &kw = h->kw;
+    kw.win = win; kw.slide = slide; kw.C = C; kw.max_keys = max_keys; kw.err_flags = ff.err_flags; kw.n_slots = ff.n_slots; kw.dense = ff.dense;
+    ALLOC(kw.ring, static_cast<size_t>(ring_bytes));
+    ALLOC(kw.cnt, sizeof(uint64_t) * (max_keys + 1ull)); kw.last_ts = kw.cnt + max_keys;
+    CK(cudaMemset(kw.cnt, 0, sizeof(uint64_t) * (max_keys + 1ull)));
+#undef ALLOC
+    *hh = h;
+    return 0;
+}
+
+int wfb_kwin_destroy(wfb_kwin_t *h)
+{
+    if (!h) return 0;
+    cudaDeviceSynchronize();
+    cudaFree(h->ff.ht_keys); cudaFree(h->ff.ht_slots); cudaFree(h->ff.n_slots); cudaFree(h->ff.slot_key); cudaFree(h->kw.ring); cudaFree(h->kw.cnt);
+    h->stage.destroy(); h->order.destroy();
+    delete h;
+    cudaGetLastError();
+    return 0;
+}
+
+uint32_t wfb_kwin_key_capacity(const wfb_kwin_t *h) { return h ? h->ff.max_keys : 0; }
+uint64_t wfb_kwin_launches(const wfb_kwin_t *h) { return h ? h->launches : 0; }
+
+int wfb_kwin_set_params(wfb_kwin_t *h, const void *params, size_t bytes)
+{
+    if (!h || !params || bytes != h->ops->params_bytes) return WFB_E_BADARG;
+    std::lock_guard<std::mutex> lock(h->mu);
+    h->params.assign(static_cast<const unsigned char *>(params), static_cast<const unsigned char *>(params) + bytes);
+    return 0;
+}
+
+int wfb_kwin_process_cb(wfb_kwin_t *h, const wfb_batch_t *batches_h, uint32_t nbatches, void *out_results, uint64_t *out_ts,
+                        uint32_t out_capacity, uint32_t *n_out_dev, void *stream)
+{
+    if (!h || !n_out_dev || (nbatches && !batches_h)) return WFB_E_BADARG;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    std::lock_guard<std::mutex> lock(h->mu);
+    int rc = h->order.enter(s); if (rc) return rc;
+    CK(cudaMemsetAsync(n_out_dev, 0, sizeof(uint32_t), s));
+    std::vector<DevBatch> hb(nbatches);
+    std::vector<uint32_t> boff(nbatches + 1);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < nbatches; i++) {
+        if (batches_h[i].n && !batches_h[i].tuples) return WFB_E_BADARG;
+        DevBatch b; std::memset(&b, 0, sizeof(b));
+        b.tuples = static_cast<const unsigned char *>(batches_h[i].tuples); b.ts = batches_h[i].ts; b.n = batches_h[i].n;
+        hb[i] = b; boff[i] = static_cast<uint32_t>(total); total += b.n;
+    }
+    boff[nbatches] = static_cast<uint32_t>(total);
+    if (total == 0) return 0;
+    if (total > 0x7fffffffull) return WFB_E_BADARG;
+    if (out_capacity && !out_results) return WFB_E_BADARG;
+    const uint32_t n = static_cast<uint32_t>(total);
+    const void *f = h->params.empty() ? nullptr : h->params.data();
+    const uint32_t *counts = nullptr, *sorted_slots = nullptr, *sorted_pos = nullptr;
+    const size_t TB = h->ops->tuple_bytes;
+    // 1. slots; 2. the stable sort by slot: every key's items contiguous, in arrival order
+    rc = keyed_front(h, f, hb, boff, nbatches, n, s,
+                     [&](size_t, size_t cap) {
+                         CK(h->wcnt.ensure(n, s, cap)); CK(h->woff.ensure(n, s, cap)); CK(h->run_m.ensure(n, s, cap)); CK(h->run_c.ensure(n, s, cap));
+                         CK(h->stage_ts.ensure(n, s, cap)); CK(h->staged.ensure(n * TB, s, cap * TB));
+                         const size_t cnt_cap = (cap + SEGT - 1) / SEGT + 1;
+                         CK(h->tile_cnt.ensure(cnt_cap, s, cnt_cap)); CK(h->total.ensure(1, s));
+                         return 0;
+                     },
+                     [](bool *) { return WFB_E_UNSUPPORTED; }, // (the key table does not grow)
+                     &counts, &sorted_slots, &sorted_pos);
+    if (rc) return rc;
+    (void)counts;
+    // 3. gather into the staging buffer; 4. windows per run, their offsets and the call's count; 5. evaluation; 6. archive
+    rc = h->ops->kw_stage(h->d_batches, h->d_boff, nbatches, n, sorted_pos, h->staged, h->stage_ts, h->kw.last_ts, s); if (rc) return rc;
+    const uint32_t tiles = (n + SEGT - 1) / SEGT;
+    k_kw_count<<<grid_for(n, 256), 256, 0, s>>>(h->kw, sorted_slots, n, h->wcnt, h->run_m, h->run_c);
+    k_flag_tile_counts<uint32_t><<<tiles, 256, 0, s>>>(h->wcnt, n, h->tile_cnt);
+    k_scan_u32<<<1, 1024, 0, s>>>(h->tile_cnt, h->tile_cnt, tiles, h->total);
+    k_kw_offsets<<<tiles, 256, 0, s>>>(h->wcnt, h->tile_cnt, n, h->woff);
+    k_kw_clamp<<<1, 1, 0, s>>>(h->total, out_capacity, n_out_dev, h->ff.err_flags);
+    CK(cudaGetLastError());
+    rc = h->ops->kw_eval(h->kw, sorted_slots, n, h->woff, h->run_m, h->run_c, h->staged, h->stage_ts, n_out_dev, static_cast<unsigned char *>(out_results),
+                         out_ts, std::min(n, out_capacity), s, f);
+    if (rc) return rc;
+    rc = h->ops->kw_archive(h->kw, sorted_slots, n, h->run_m, h->run_c, h->staged, s); if (rc) return rc;
+    h->launches += 8;
+    return 0;
+}
+
+int wfb_kwin_flush(wfb_kwin_t *h, void *out_results, uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, void *stream)
+{
+    if (!h || !n_out_dev || (out_capacity && !out_results)) return WFB_E_BADARG;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    std::lock_guard<std::mutex> lock(h->mu);
+    int rc = h->order.enter(s); if (rc) return rc;
+    CK(h->total.ensure(1, s));
+    CK(cudaMemsetAsync(h->total, 0, sizeof(uint32_t), s));
+    rc = h->ops->kw_flush(h->kw, h->total, out_capacity, static_cast<unsigned char *>(out_results), out_ts, s, h->params.empty() ? nullptr : h->params.data());
+    if (rc) return rc;
+    k_kw_clamp<<<1, 1, 0, s>>>(h->total, out_capacity, n_out_dev, h->ff.err_flags);
+    CK(cudaGetLastError());
+    h->launches += 2;
+    return 0;
+}
+
+int wfb_kwin_stats(wfb_kwin_t *h, uint32_t *n_keys_h, uint32_t *err_flags_h, void *stream)
+{
+    if (!h) return WFB_E_BADARG;
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    std::lock_guard<std::mutex> lock(h->mu);
+    uint32_t v[2] = {0, 0};
+    int rc = h->order.enter(s); if (rc) return rc; // (the counters of a call issued on another stream)
+    CK(cudaMemcpyAsync(v, h->ff.n_slots, sizeof(v), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (n_keys_h) *n_keys_h = std::min(v[0], h->ff.max_keys);
+    if (err_flags_h) *err_flags_h = v[1];
+    return 0;
 }
 
 static int ffat_process_cb_impl(wfb_ffat_t *h, const void *pre, const wfb_batch_t *batches_h, uint32_t nbatches, void *out_results, uint64_t *out_ts,

@@ -248,6 +248,72 @@ class KeyedState:
         return outs, n_out
 
 
+class KeyedWindowsGPU:
+    """Keyed_Windows_GPU replica state (wf/keyed_windows.hpp, wf/window_replica.hpp): count-based windows whose win_func iterates
+    every tuple of the window, with each key's last pow2ceil(win) tuples in a ring on the device. `prog` must define win_func."""
+
+    def __init__(self, prog, win, slide, max_keys, dense_keys=False, params=None):
+        self.L = _lib.lib()
+        if self.L.wfb_device_count() <= 0:
+            raise RuntimeError("windflow_b200: no CUDA device (there is no CPU fallback)")
+        self.h = C.c_void_p()
+        self.result_bytes = 0
+        check(self.L.wfb_kwin_create(C.byref(self.h), prog, win, slide, max_keys, 1 if dense_keys else 0), "wfb_kwin_create")
+        info = _lib.ProgramInfo()
+        check(self.L.wfb_program_info(prog, C.byref(info)), "wfb_program_info")
+        self.result_bytes = info.result_bytes
+        if params is not None:
+            check(self.L.wfb_kwin_set_params(self.h, C.byref(params), C.sizeof(params)), "wfb_kwin_set_params")
+
+    @property
+    def key_capacity(self):
+        return int(self.L.wfb_kwin_key_capacity(self.h))
+
+    @property
+    def launches(self):
+        return int(self.L.wfb_kwin_launches(self.h))
+
+    def close(self):
+        if self.h:
+            self.L.wfb_kwin_destroy(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _out(self, cap, out, out_ts, n_out, device="cuda"):
+        if out is None:
+            out = torch.empty(max(1, cap) * self.result_bytes, dtype=torch.uint8, device=device)
+        if out_ts is None:
+            out_ts = torch.empty(max(1, cap), dtype=torch.int64, device=device)
+        if n_out is None:
+            n_out = torch.zeros(1, dtype=torch.int32, device=device)
+        return out, out_ts, n_out
+
+    def process(self, batches, capacity=None, out=None, out_ts=None, n_out=None, stream=None):
+        """The windows the queued batches fire: (out, out_ts, n_out). capacity defaults to the call's tuples (a bound on its windows)."""
+        cap = sum(b.n for b in batches) if capacity is None else capacity
+        out, out_ts, n_out = self._out(cap, out, out_ts, n_out)
+        check(self.L.wfb_kwin_process_cb(self.h, _cbatches(batches), len(batches), _ptr(out), _ptr(out_ts), cap, _ptr(n_out),
+                                         _stream_ptr(stream)), "wfb_kwin_process_cb")
+        return out, out_ts, n_out
+
+    def flush(self, capacity, out=None, out_ts=None, n_out=None, stream=None):
+        """End of stream: every opened window that has not fired, on its tuples so far (at most ceil(win / slide) per key)."""
+        out, out_ts, n_out = self._out(capacity, out, out_ts, n_out)
+        check(self.L.wfb_kwin_flush(self.h, _ptr(out), _ptr(out_ts), capacity, _ptr(n_out), _stream_ptr(stream)), "wfb_kwin_flush")
+        return out, out_ts, n_out
+
+    def stats(self, stream=None):
+        """(distinct keys, error flags): bit 0 a key found no slot, bit 1 more results than the capacity."""
+        nk, ef = C.c_uint32(), C.c_uint32()
+        check(self.L.wfb_kwin_stats(self.h, C.byref(nk), C.byref(ef), _stream_ptr(stream)), "wfb_kwin_stats")
+        return nk.value, ef.value
+
+
 class Segment(list):
     """A list of DeviceBatch whose C descriptor array is built once: a replica that re-submits the same device buffers
     (a ring of input segments) does not pay the per-batch Python / ctypes cost on every call. Immutable by convention."""
