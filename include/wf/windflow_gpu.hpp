@@ -232,10 +232,12 @@ struct FacadeStatefulFlatMapProgram {
         FlatF f = p.fm; f(t, sh, st);
     }
 };
-// The program of a Keyed_Windows_GPU: func(const Iterable_GPU<tuple_t> &, result_t &) over each count-based window of a key
-// (wf/keyed_windows.hpp, non-incremental and non-riched); the result starts as result_t(key, gwid) when that constructor exists
+// The program of a Keyed_Windows_GPU: func(const Iterable_GPU<tuple_t> &, result_t &) over each count-based window of a key, or,
+// INC, func(const tuple_t &, result_t &) folding each tuple into every open window it is IN (wf/keyed_windows.hpp, non-riched); the
+// result starts as result_t(key, gwid) when that constructor exists. Only the member matching the functor is defined (win_func or
+// win_func_inc), so that the launch table takes the matching path.
 template <class T> using Iterable_GPU = wfb::Iterable_GPU<T>; // size(), operator[], at(), front(), back(), begin() / end() (wf/iterable.hpp)
-template <class T, class R, class WinF, class KeyF, bool KEYED>
+template <class T, class R, class WinF, class KeyF, bool KEYED, bool INC>
 struct FacadeKeyedWindowsProgram {
     using tuple_t = T; using result_t = R; using key_t = key_of_t<KeyF>;
     struct params_t { WinF win; KeyF key; };
@@ -251,10 +253,14 @@ struct FacadeKeyedWindowsProgram {
         return FacadeProgram<T, R, KeyF, NoLift<T, R>, NoComb<R>, NoReduce<T>, KEYED>::make_result(k, gwid, {{}, {}, p.key, {}, {}, {}});
     }
     __host__ __device__ static tuple_t reduce(const tuple_t &a, const tuple_t &, const params_t &) { return a; }
+    template <bool I = INC, std::enable_if_t<!I, int> = 0>
     __host__ __device__ static void win_func(const Iterable_GPU<tuple_t> &w, result_t &r, const params_t &p) { WinF f = p.win; f(w, r); }
+    template <bool I = INC, std::enable_if_t<I, int> = 0>
+    __host__ __device__ static void win_func_inc(const tuple_t &t, result_t &r, const params_t &p) { WinF f = p.win; f(t, r); }
 };
-template <class X> struct iterable_tuple;
-template <class T> struct iterable_tuple<wfb::Iterable_GPU<T>> { using type = T; };
+// the tuple type of a window function's first argument: T from const Iterable_GPU<T> & (non-incremental) or from const T & (incremental)
+template <class X> struct window_tuple { using type = X; static constexpr bool incremental = true; };
+template <class T> struct window_tuple<wfb::Iterable_GPU<T>> { using type = T; static constexpr bool incremental = false; };
 
 template <class T, class S> struct StatefulIdMap { __host__ __device__ void operator()(T &, S &) const {} };
 template <class T, class S> struct StatefulKeepAll { __host__ __device__ bool operator()(T &, S &) const { return true; } };
@@ -1095,16 +1101,19 @@ public:
 };
 
 // Keyed_Windows_GPU, count-based (wf/keyed_windows.hpp, wf/window_replica.hpp): func(const Iterable_GPU<tuple_t> &, result_t &) over
-// every window of every key, the key's last pow2ceil(win) tuples kept on the device. svc(): the K batches found queued go to ONE
+// every window of every key, the key's last pow2ceil(win) tuples kept on the device; or func(const tuple_t &, result_t &) folding each
+// tuple into the accumulator of every open window it is IN, the key's open accumulators kept on the device (a WFB_KWIN_INCREMENTAL
+// handle). svc(): the K batches found queued go to ONE
 // wfb_kwin_process_cb call, whose results form one output batch whose size stays on the device; at end of stream the windows that
 // opened and did not fire are evaluated on the tuples they have (wf/window_replica.hpp:356-407) and sent as one more batch.
 template <class win_func_gpu_t, class keyextr_func_gpu_t>
 class Keyed_Windows_GPU: public Basic_Operator {
 public:
-    using tuple_t = typename iterable_tuple<fn_arg_t<win_func_gpu_t, 0>>::type;
+    using tuple_t = typename window_tuple<fn_arg_t<win_func_gpu_t, 0>>::type;
     using result_t = fn_arg_t<win_func_gpu_t, 1>;
     static constexpr bool isKeyed = !std::is_same<keyextr_func_gpu_t, NoKey<tuple_t>>::value;
-    using prog_t = FacadeKeyedWindowsProgram<tuple_t, result_t, win_func_gpu_t, keyextr_func_gpu_t, isKeyed>;
+    static constexpr bool isIncremental = window_tuple<fn_arg_t<win_func_gpu_t, 0>>::incremental;
+    using prog_t = FacadeKeyedWindowsProgram<tuple_t, result_t, win_func_gpu_t, keyextr_func_gpu_t, isKeyed, isIncremental>;
     static constexpr op_type_t op_type = op_type_t::WIN_GPU;
     win_func_gpu_t func; keyextr_func_gpu_t key_extr; uint64_t win_len, slide_len; uint32_t max_keys; size_t maxk;
     Keyed_Windows_GPU(win_func_gpu_t f, keyextr_func_gpu_t k, std::string n, uint64_t w, uint64_t s, uint32_t mk, size_t mbpc):
@@ -1144,7 +1153,7 @@ public:
         int svc_init() override
         {
             Basic_Replica::svc_init();
-            wfbErrChk(wfb_kwin_create(&kw, wfb::register_program<prog_t>(), op.win_len, op.slide_len, op.max_keys, 0));
+            wfbErrChk(wfb_kwin_create(&kw, wfb::register_program<prog_t>(), op.win_len, op.slide_len, op.max_keys, isIncremental ? WFB_KWIN_INCREMENTAL : 0u));
             wfbErrChk(wfb_kwin_set_params(kw, &prm, sizeof(prm)));
             gpuErrChk(this->counts.init(1)); // (one word per call)
             return 0;
@@ -1367,9 +1376,9 @@ public:
 };
 
 // Keyed_WindowsGPU_Builder(win_func).withKeyBy(k).withCBWindows(w, s): win_func is __host__ __device__
-// void(const Iterable_GPU<tuple_t> &, result_t &) (wf/builders.hpp, Keyed_Windows_Builder); without withKeyBy every tuple has one key
-// (and withMaxKeys is ignored)
-template <class win_func_gpu_t, class keyextr_func_gpu_t = NoKey<typename iterable_tuple<fn_arg_t<win_func_gpu_t, 0>>::type>>
+// void(const Iterable_GPU<tuple_t> &, result_t &) or, incremental, __host__ __device__ void(const tuple_t &, result_t &)
+// (wf/builders.hpp, Keyed_Windows_Builder); without withKeyBy every tuple has one key (and withMaxKeys is ignored)
+template <class win_func_gpu_t, class keyextr_func_gpu_t = NoKey<typename window_tuple<fn_arg_t<win_func_gpu_t, 0>>::type>>
 class Keyed_WindowsGPU_Builder {
     template <class A, class B> friend class Keyed_WindowsGPU_Builder;
     win_func_gpu_t func; keyextr_func_gpu_t key_extr; std::string name = "keyed_windows_gpu";
@@ -1379,10 +1388,14 @@ class Keyed_WindowsGPU_Builder {
 public:
     explicit Keyed_WindowsGPU_Builder(win_func_gpu_t f): func(f), key_extr()
     {
+        using T = typename window_tuple<fn_arg_t<win_func_gpu_t, 0>>::type;
         static_assert(std::tuple_size<args_t>::value == 2 && std::is_same<fn_ret_t<win_func_gpu_t>, void>::value &&
-                      std::is_same<std::tuple_element_t<0, args_t>, const Iterable_GPU<typename iterable_tuple<fn_arg_t<win_func_gpu_t, 0>>::type> &>::value &&
+                      (std::is_same<std::tuple_element_t<0, args_t>, const Iterable_GPU<T> &>::value ||
+                       std::is_same<std::tuple_element_t<0, args_t>, const T &>::value) &&
                       std::is_same<std::tuple_element_t<1, args_t>, fn_arg_t<win_func_gpu_t, 1> &>::value,
-                      "WindFlow Compilation Error - Keyed_WindowsGPU_Builder: __host__ __device__ void(const Iterable_GPU<tuple_t> &, result_t &)");
+                      "WindFlow Compilation Error - unknown signature passed to the Keyed_WindowsGPU_Builder:\n"
+                      "  Candidate 1 : __host__ __device__ void(const Iterable_GPU<tuple_t> &, result_t &)\n"
+                      "  Candidate 2 : __host__ __device__ void(const tuple_t &, result_t &)\n");
     }
     auto &withName(std::string n) { name = std::move(n); return *this; }
     template <class new_keyextr_t> auto withKeyBy(new_keyextr_t k)

@@ -194,7 +194,16 @@ int wfb_flatmap_stateful(wfb_kstate_t *h, const wfb_functors_t *f, const wfb_bat
  * of ring (WFB_E_UNSUPPORTED above; a failed allocation returns the CUDA error). flags: 0 or WFB_FFAT_DENSE_KEYS (integral keys).
  * A key that finds no slot raises error bit 0 and its tuples are dropped; every other key's windows stay exact.
  * Programs without win_func: WFB_E_UNSUPPORTED; win or slide 0: WFB_E_BADARG.
- * replaces Keyed_Windows + Window_Replica's key descriptors, archives and triggerers, wf/keyed_windows.hpp, wf/window_replica.hpp:84-112. */
+ * replaces Keyed_Windows + Window_Replica's key descriptors, archives and triggerers, wf/keyed_windows.hpp, wf/window_replica.hpp:84-112.
+ *
+ * Incremental (flags | WFB_KWIN_INCREMENTAL, combinable with WFB_FFAT_DENSE_KEYS): the program's
+ * win_func_inc(const tuple_t &t, result_t &acc, const params_t &) folds, in arrival order, every tuple that is IN window g into the
+ * window's accumulator, which starts as make_result(key, g) when the window's first tuple arrives (wf/window_replica.hpp:293-303,
+ * wf/window_structure.hpp:151); the firing tuple is not folded. Same windows, timestamps, flush and error bits as above. No tuple is
+ * kept: per key, the handle holds its count and a ring of R = pow2ceil(ceil(win / slide)) accumulators (R = 1 for tumbling and hopping
+ * windows), max_keys * R * sizeof(result_t) bytes (WFB_E_UNSUPPORTED when that does not fit size_t). A call whose
+ * min(tuples, max_keys) * ceil(win / slide) exceeds 2^31 - 1 returns WFB_E_UNSUPPORTED. Programs without win_func_inc: WFB_E_UNSUPPORTED. */
+#define WFB_KWIN_INCREMENTAL 8u
 typedef struct wfb_kwin wfb_kwin_t;
 int wfb_kwin_create(wfb_kwin_t **h, int prog, uint64_t win, uint64_t slide, uint32_t max_keys, uint32_t flags);
 int wfb_kwin_destroy(wfb_kwin_t *h);

@@ -4,14 +4,17 @@
 //     SourceGPU (a ring of batches resident in HBM) -> Map_GPU -> Filter_GPU -> Keyed_Windows_GPU (count-based, hashed keys) -> Sink
 //
 // 64-byte tuples of the seeded synthetic stream (batch 65536, uniform keys), map ivalue += 2 / fvalue *= 1.0000001, filter
-// (ivalue & 1) == 0, and a window function that reads every tuple of its window (the one of tests/cpp/kwin_programs.cu).
-// tools/keyed_windows_bench.py runs it as the builder arm.
-//   usage: keyed_windows_bench.bin [K=128] [timed_batches=2048] [keys=65536] [win=1024] [slide=64] [ring_batches=256]
+// (ivalue & 1) == 0, and a window function that reads every tuple of its window (the one of tests/cpp/kwin_programs.cu), or with
+// inc=1 the incremental function of tests/cpp/kwin_inc_programs.cu, void(const tuple64_t &, result80_t &).
+// tools/keyed_windows_bench.py runs it as the builder arms.
+//   usage: keyed_windows_bench.bin [K=128] [timed_batches=2048] [keys=65536] [win=1024] [slide=64] [ring_batches=256] [inc=0]
 // prints one JSON line.
 #include <atomic>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
+#include <functional>
 #include <optional>
 #include <thread>
 #include <wf/windflow_gpu.hpp>
@@ -23,6 +26,11 @@ struct result72_t {
     uint64_t key, id, hash, size, mid, front, back, distinct; double fsum;
     __host__ __device__ result72_t(): key(0), id(0), hash(0), size(0), mid(0), front(0), back(0), distinct(0), fsum(0) {}
     __host__ __device__ result72_t(uint64_t k, uint64_t g): key(k), id(g), hash(0), size(0), mid(0), front(0), back(0), distinct(0), fsum(0) {}
+};
+struct result80_t {
+    uint64_t key, id, hash, size, front, back, mask; double fsum; uint64_t argmax; int64_t maxiv;
+    __host__ __device__ result80_t(): key(0), id(0), hash(0), size(0), front(0), back(0), mask(0), fsum(0), argmax(0), maxiv(0) {}
+    __host__ __device__ result80_t(uint64_t k, uint64_t g): result80_t() { key = k; id = g; }
 };
 struct MapF { __host__ __device__ void operator()(tuple64_t &t) { t.ivalue += 2; t.fvalue *= 1.0000001; } };
 struct FiltF { __host__ __device__ bool operator()(tuple64_t &t) { return (t.ivalue & 1) == 0; } };
@@ -42,12 +50,40 @@ struct WinF {
     }
 };
 
+struct WinIncF {
+    __host__ __device__ void operator()(const tuple64_t &t, result80_t &r) const
+    {
+        constexpr uint64_t MIX = 0x9E3779B97F4A7C15ull, MUL = 0x100000001B3ull;
+        if (r.size == 0 || t.ivalue > r.maxiv) { r.maxiv = t.ivalue; r.argmax = t.id; }
+        if (r.size == 0) r.front = t.id;
+        r.hash = r.hash * MUL + (t.id * MIX ^ static_cast<uint64_t>(t.ivalue));
+        r.size++; r.back = t.id;
+        r.mask |= 1ull << (static_cast<uint64_t>(t.ivalue) & 15u);
+        r.fsum += t.fvalue;
+    }
+};
+
 static std::atomic<uint64_t> g_seen_wm{0}; // watermark (= index of the last input batch) of the newest result batch the sink has seen
 static std::atomic<uint64_t> g_windows{0};
-struct SinkF {
+template <class R> struct SinkF {
     uint64_t windows = 0;
-    void operator()(std::optional<result72_t> &r) { if (r) windows++; else g_windows.fetch_add(windows); }
+    void operator()(std::optional<R> &r) { if (r) windows++; else g_windows.fetch_add(windows); }
 };
+
+template <class Win, class R>
+static size_t run_graph(Win winf, size_t K, uint64_t nkeys, uint64_t win, uint64_t slide, std::function<void(SourceGPU_Shipper<tuple64_t> &)> source)
+{
+    PipeGraph graph("keyed_windows_bench", Execution_Mode_t::DEFAULT, Time_Policy_t::EVENT_TIME);
+    MultiPipe &mp = graph.add_source(SourceGPU_Builder(source).withName("source").build());
+    mp.chain(MapGPU_Builder(MapF()).withName("map").build());
+    mp.chain(FilterGPU_Builder(FiltF()).withName("filter").build());
+    mp.add(Keyed_WindowsGPU_Builder(winf).withName("keyed_windows").withKeyBy(KeyF()).withCBWindows(win, slide)
+               .withMaxKeys(static_cast<uint32_t>(nkeys)).withMaxBatchesPerCall(K).build());
+    mp.chain_sink(Sink_Builder(SinkF<R>()).withName("sink").withWatermarkProbe(&g_seen_wm).build());
+    const size_t threads = graph.getNumThreads();
+    graph.run();
+    return threads;
+}
 
 int main(int argc, char **argv)
 {
@@ -57,9 +93,11 @@ int main(int argc, char **argv)
     const uint64_t win = argc > 4 ? std::strtoull(argv[4], nullptr, 10) : 1024;
     const uint64_t slide = argc > 5 ? std::strtoull(argv[5], nullptr, 10) : 64;
     const uint64_t ring = argc > 6 ? std::strtoull(argv[6], nullptr, 10) : 256;
+    const bool inc = argc > 7 && std::strtoull(argv[7], nullptr, 10) != 0;
     const uint64_t BATCH = 65536;
-    // every key past its first window before the clock starts: win + 1 surviving tuples per key at selectivity 0.5
-    const uint64_t prime = (2 * (win + 1) * nkeys + BATCH - 1) / BATCH + ring;
+    // every key past its first window before the clock starts: win + 1 surviving tuples per key at selectivity 0.5 (at most 8192
+    // batches: with longer windows the timed batches mostly fold into windows that stay open)
+    const uint64_t prime = std::min<uint64_t>((2 * (win + 1) * nkeys + BATCH - 1) / BATCH, 8192) + ring;
 
     tuple64_t *d_tuples = nullptr; uint64_t *d_ts = nullptr;
     gpuErrChk(cudaMalloc(&d_tuples, ring * BATCH * sizeof(tuple64_t)));
@@ -79,22 +117,13 @@ int main(int argc, char **argv)
         drained(prime + timed);
         t1 = std::chrono::steady_clock::now();
     };
-    size_t threads = 0;
-    {
-        PipeGraph graph("keyed_windows_bench", Execution_Mode_t::DEFAULT, Time_Policy_t::EVENT_TIME);
-        MultiPipe &mp = graph.add_source(SourceGPU_Builder(source).withName("source").build());
-        mp.chain(MapGPU_Builder(MapF()).withName("map").build());
-        mp.chain(FilterGPU_Builder(FiltF()).withName("filter").build());
-        mp.add(Keyed_WindowsGPU_Builder(WinF()).withName("keyed_windows").withKeyBy(KeyF()).withCBWindows(win, slide)
-                   .withMaxKeys(static_cast<uint32_t>(nkeys)).withMaxBatchesPerCall(K).build());
-        mp.chain_sink(Sink_Builder(SinkF()).withName("sink").withWatermarkProbe(&g_seen_wm).build());
-        threads = graph.getNumThreads();
-        graph.run();
-    }
+    const size_t threads = inc ? run_graph<WinIncF, result80_t>(WinIncF(), K, nkeys, win, slide, source)
+                               : run_graph<WinF, result72_t>(WinF(), K, nkeys, win, slide, source);
     const double sec = std::chrono::duration<double>(t1 - t0).count();
-    std::printf("{\"arm\": \"builder\", \"max_batches_per_call\": %zu, \"tuples\": %llu, \"seconds\": %.6f, \"tuples_per_s\": %.1f, \"windows\": %llu, "
+    std::printf("{\"arm\": \"%s\", \"max_batches_per_call\": %zu, \"tuples\": %llu, \"seconds\": %.6f, \"tuples_per_s\": %.1f, \"windows\": %llu, "
                 "\"threads\": %zu, \"keys\": %llu, \"win\": %llu, \"slide\": %llu, \"primed_batches\": %llu}\n",
-                K, static_cast<unsigned long long>(timed * BATCH), sec, timed * BATCH / sec, static_cast<unsigned long long>(g_windows.load()), threads,
+                inc ? "builder_inc" : "builder", K, static_cast<unsigned long long>(timed * BATCH), sec, timed * BATCH / sec,
+                static_cast<unsigned long long>(g_windows.load()), threads,
                 static_cast<unsigned long long>(nkeys), static_cast<unsigned long long>(win), static_cast<unsigned long long>(slide),
                 static_cast<unsigned long long>(prime));
     cudaFree(d_tuples); cudaFree(d_ts);

@@ -3650,11 +3650,11 @@ private:
 
 // state and geometry of one Keyed_Windows_GPU handle as its kernels see it
 struct KwinDev {
-    unsigned char *ring;     // max_keys * C tuples
+    unsigned char *ring;     // max_keys * C tuples (incremental: max_keys * C accumulators)
     uint64_t *cnt;           // tuples of each slot so far
     uint64_t *last_ts;       // largest timestamp seen (the end-of-stream windows carry it)
     uint64_t win, slide;
-    uint32_t C;              // ring length (power of two >= win)
+    uint32_t C;              // ring length (power of two >= win; incremental: >= ceil(win / slide))
     uint32_t max_keys;
     uint32_t *err_flags;     // bit 0: a key found no slot, bit 1: more results than the output capacity
     uint32_t *n_slots;       // slots taken (a dense table takes none: slot = key, every slot may hold a key)
@@ -3826,6 +3826,139 @@ __global__ void __launch_bounds__(128) k_kw_flush(const KwinDev kw, uint32_t *__
             R r = P::make_result(P::key(it.front(), prm), g, prm);
             P::win_func(it, r, prm);
             st_rec<R>(out + static_cast<size_t>(base + q) * sizeof(R), r);
+            if (out_ts != nullptr) out_ts[base + q] = ts;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------
+// Keyed_Windows_GPU, incremental (WFB_KWIN_INCREMENTAL; wf/window_replica.hpp:293-303): win_func_inc(t, acc, params) folds every tuple
+// that is IN window g into its accumulator, in arrival order. Per key the handle keeps its count and a ring of C = pow2ceil(ceil(win /
+// slide)) accumulators (kw.ring + slot * C results, entry g & (C - 1)): at most ceil(win / slide) windows are open at once, and windows
+// open together never share an entry. A call reuses the staging gather, then per run (a key's m tuples of the call, count c before it)
+// the windows it touches, g with g*slide <= c + m - 1 and g*slide + win >= c, are [g_lo, g_lo + fired + open): the fired ones first
+// (k_kwi_count), each count scanned on its own (fired -> output index, open -> pending index, their sum -> the run of a thread). Then
+// one thread per touched window (k_kwi_eval) and the copy of the windows opened in the call that stay open into the ring (k_kwi_writeback).
+// The ring hazard: a window open before the call can fire in it while a window opened in the same call stays open in the same entry, so
+// the latter is written to the pending buffer and copied after every read of the call. A window open before the call that stays open
+// is written in place: no other window open before the call, and none open after it, shares its entry.
+// ------------------------------------------------------------------------------------------------------
+
+// one record from src to dst, both aligned as ld_rec / st_rec require
+template <class R>
+__device__ __forceinline__ void copy_rec(unsigned char *__restrict__ dst, const unsigned char *__restrict__ src)
+{
+    if constexpr (sizeof(R) % 16 == 0) {
+#pragma unroll
+        for (uint32_t k = 0; k < sizeof(R) / 16; k++) reinterpret_cast<uint4 *>(dst)[k] = reinterpret_cast<const uint4 *>(src)[k];
+    } else {
+#pragma unroll
+        for (uint32_t k = 0; k < sizeof(R) / 8; k++) reinterpret_cast<uint64_t *>(dst)[k] = reinterpret_cast<const uint64_t *>(src)[k];
+    }
+}
+
+// per sorted position: the windows its run fires and those it leaves open (run heads only; 0 elsewhere), the run's length and starting
+// count at its head; the head also stores the key's new count (the call's later kernels read the starting count from run_c)
+static __global__ void __launch_bounds__(256) k_kwi_count(const KwinDev kw, const uint32_t *__restrict__ sorted_slots, uint32_t n,
+                                                          uint32_t *__restrict__ wcnt, uint32_t *__restrict__ ocnt, uint32_t *__restrict__ run_m,
+                                                          uint64_t *__restrict__ run_c)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        const uint32_t slot = sorted_slots[j];
+        uint32_t w = 0, o = 0;
+        if (slot < kw.max_keys && (j == 0 || sorted_slots[j - 1] != slot)) {
+            const uint32_t m = kw_lower_bound(sorted_slots, j, n, slot + 1) - j;
+            const uint64_t c = kw.cnt[slot];
+            uint64_t g_lo;
+            w = static_cast<uint32_t>(kw_fired(c, m, kw.win, kw.slide, &g_lo));
+            const uint64_t g_hi = (c + m - 1) / kw.slide; // the last window whose first id is of this call or earlier
+            o = g_hi + 1 >= g_lo + w ? static_cast<uint32_t>(g_hi + 1 - g_lo - w) : 0u;
+            run_m[j] = m; run_c[j] = c;
+            kw.cnt[slot] = c + m;
+        }
+        wcnt[j] = w; ocnt[j] = o;
+    }
+}
+
+// one thread per touched window: its run by binary search over the summed offsets, its accumulator (the ring entry when it opened before
+// the call, else make_result(key, g)), the fold of the call's tuples IN it; then the result (fired, among the first *n_out) or the
+// accumulator (open: in place, or to the pending buffer when it opened in this call)
+template <class P>
+__global__ void __launch_bounds__(128) k_kwi_eval(const KwinDev kw, const uint32_t *__restrict__ sorted_slots, uint32_t n,
+                                                  const uint32_t *__restrict__ woff, const uint32_t *__restrict__ ooff, const uint32_t *__restrict__ n_open,
+                                                  const uint32_t *__restrict__ run_m, const uint64_t *__restrict__ run_c,
+                                                  const unsigned char *__restrict__ stage, const uint64_t *__restrict__ stage_ts,
+                                                  const uint32_t *__restrict__ n_fired, const uint32_t *__restrict__ n_out, unsigned char *__restrict__ out,
+                                                  uint64_t *__restrict__ out_ts, unsigned char *__restrict__ pending, const typename P::params_t prm)
+{
+    using T = typename P::tuple_t; using R = typename P::result_t;
+    const uint32_t total = *n_fired + *n_open, cap = *n_out; // (the host keeps fired + open below 2^32)
+    const T *st = reinterpret_cast<const T *>(stage);
+    for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < total; w += gridDim.x * blockDim.x) {
+        uint32_t lo = 0, hi = n; // last j with woff[j] + ooff[j] <= w: the run head whose windows include w
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (woff[mid] + ooff[mid] <= w) lo = mid; else hi = mid; }
+        const uint32_t j = lo, slot = sorted_slots[j], q = w - (woff[j] + ooff[j]);
+        const uint64_t c = run_c[j], m = run_m[j];
+        uint64_t g_lo;
+        const uint32_t nf = static_cast<uint32_t>(kw_fired(c, m, kw.win, kw.slide, &g_lo));
+        const bool fired = q < nf;
+        if (fired && woff[j] + q >= cap) continue; // (beyond the output capacity: error bit 1; a fired window keeps no state)
+        const uint64_t g = g_lo + q, first = g * kw.slide, last = first + kw.win; // ids [first, last)
+        unsigned char *entry = kw.ring + (static_cast<size_t>(slot) * kw.C + (g & (kw.C - 1))) * sizeof(R);
+        alignas(16) R r = P::make_result(P::key(st[j], prm), g, prm);
+        if (first < c) ld_rec<R>(entry, r);
+        const uint64_t a = first > c ? first : c, b = last < c + m ? last : c + m;
+        for (uint64_t id = a; id < b; id++) P::win_func_inc(st[j + static_cast<uint32_t>(id - c)], r, prm);
+        if (fired) {
+            st_rec<R>(out + static_cast<size_t>(woff[j] + q) * sizeof(R), r);
+            if (out_ts != nullptr) out_ts[woff[j] + q] = stage_ts[j + static_cast<uint32_t>(last - c)]; // (the firing tuple, id `last`, is of this call)
+        } else if (first < c) {
+            st_rec<R>(entry, r);
+        } else {
+            st_rec<R>(pending + static_cast<size_t>(ooff[j] + (q - nf)) * sizeof(R), r);
+        }
+    }
+}
+
+// after k_kwi_eval: the accumulators of the windows opened in the call that stay open, from the pending buffer into their ring entries
+template <class P>
+__global__ void __launch_bounds__(256) k_kwi_writeback(const KwinDev kw, const uint32_t *__restrict__ sorted_slots, uint32_t n,
+                                                       const uint32_t *__restrict__ ooff, const uint32_t *__restrict__ n_open,
+                                                       const uint32_t *__restrict__ run_m, const uint64_t *__restrict__ run_c,
+                                                       const unsigned char *__restrict__ pending)
+{
+    using R = typename P::result_t;
+    const uint32_t total = *n_open;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        uint32_t lo = 0, hi = n; // last j with ooff[j] <= i
+        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (ooff[mid] <= i) lo = mid; else hi = mid; }
+        const uint32_t j = lo;
+        const uint64_t c = run_c[j];
+        uint64_t g_lo;
+        const uint64_t nf = kw_fired(c, run_m[j], kw.win, kw.slide, &g_lo), g = g_lo + nf + (i - ooff[j]);
+        if (g * kw.slide < c) continue; // (opened before the call: k_kwi_eval wrote it in place)
+        copy_rec<R>(kw.ring + (static_cast<size_t>(sorted_slots[j]) * kw.C + (g & (kw.C - 1))) * sizeof(R), pending + static_cast<size_t>(i) * sizeof(R));
+    }
+}
+
+// end of stream: the accumulator of every window of every key that opened and has not fired, in window order, with the largest
+// timestamp seen (the window set of k_kw_flush). One thread per key; a key's windows take consecutive results.
+template <class P>
+__global__ void __launch_bounds__(128) k_kwi_flush(const KwinDev kw, uint32_t *__restrict__ total, uint32_t cap, unsigned char *__restrict__ out,
+                                                   uint64_t *__restrict__ out_ts)
+{
+    using R = typename P::result_t;
+    const uint32_t nk = kw.dense ? kw.max_keys : min(*kw.n_slots, kw.max_keys);
+    const uint64_t ts = *kw.last_ts;
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < nk; s += gridDim.x * blockDim.x) {
+        const uint64_t c = kw.cnt[s];
+        if (c == 0) continue;
+        const uint64_t g_lo = c > kw.win ? (c - kw.win + kw.slide - 1) / kw.slide : 0, g_hi = (c - 1) / kw.slide;
+        if (g_hi < g_lo) continue;
+        const uint32_t k = static_cast<uint32_t>(g_hi - g_lo + 1), base = atomicAdd(total, k);
+        for (uint32_t q = 0; q < k && base + q < cap; q++) {
+            const uint64_t g = g_lo + q;
+            copy_rec<R>(out + static_cast<size_t>(base + q) * sizeof(R), kw.ring + (static_cast<size_t>(s) * kw.C + (g & (kw.C - 1))) * sizeof(R));
             if (out_ts != nullptr) out_ts[base + q] = ts;
         }
     }

@@ -123,8 +123,8 @@ struct ProgramOps {
     int (*flatmap)(TileArgs &a, const void *params, uint32_t want_grid, cudaStream_t s, uint32_t *grid_used, uint64_t span_begin, uint64_t span_end);
     // 1: the program has flatmap_stateful (keyed-stateful FlatMap_GPU: ks_apply / ks_apply_runs take KS_FM_COUNT and KS_FM_EMIT)
     uint32_t has_flatmap_stateful, reserved3;
-    // Keyed_Windows_GPU (null when the program has no win_func): the staging gather, the evaluation of the fired windows, the archive
-    // of every run's last tuples and the end-of-stream evaluation
+    // Keyed_Windows_GPU (null when the program has no win_func; kw_stage is also set when it has win_func_inc): the staging gather, the
+    // evaluation of the fired windows, the archive of every run's last tuples and the end-of-stream evaluation
     int (*kw_stage)(const DevBatch *batches, const uint32_t *boff, uint32_t nb, uint32_t n, const uint32_t *sorted_pos, unsigned char *stage,
                     uint64_t *stage_ts, uint64_t *last_ts, cudaStream_t s);
     int (*kw_eval)(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *woff, const uint32_t *run_m, const uint64_t *run_c,
@@ -135,6 +135,17 @@ struct ProgramOps {
     int (*kw_flush)(const KwinDev &kw, uint32_t *total, uint32_t cap, unsigned char *out, uint64_t *out_ts, cudaStream_t s, const void *params);
     // 1: the program has win_func (the kw_* entries are set)
     uint32_t has_win_func, reserved4;
+    // incremental Keyed_Windows_GPU (null when the program has no win_func_inc): one thread per window the call touches, the copy of the
+    // windows opened in the call that stay open into the ring, and the end-of-stream emission of the open accumulators
+    int (*kwi_eval)(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *woff, const uint32_t *ooff, const uint32_t *n_open,
+                    const uint32_t *run_m, const uint64_t *run_c, const unsigned char *stage, const uint64_t *stage_ts, const uint32_t *n_fired,
+                    const uint32_t *n_out, unsigned char *out, uint64_t *out_ts, unsigned char *pending, uint32_t max_windows, cudaStream_t s,
+                    const void *params);
+    int (*kwi_writeback)(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *ooff, const uint32_t *n_open,
+                         const uint32_t *run_m, const uint64_t *run_c, const unsigned char *pending, uint32_t max_open, cudaStream_t s);
+    int (*kwi_flush)(const KwinDev &kw, uint32_t *total, uint32_t cap, unsigned char *out, uint64_t *out_ts, cudaStream_t s);
+    // 1: the program has win_func_inc (the kwi_* entries and kw_stage are set)
+    uint32_t has_win_func_inc, reserved5;
 };
 
 // P::passthrough (optional): map is a no-op and lift the identity (tuple_t == result_t)
@@ -383,6 +394,37 @@ int kw_flush_dispatch(const KwinDev &kw, uint32_t *total, uint32_t cap, unsigned
     return 0;
 }
 
+// P::win_func_inc(const tuple_t &, result_t &, const params_t &) (optional: incremental Keyed_Windows_GPU)
+template <class P, class = void> struct program_has_win_func_inc : std::false_type {};
+template <class P> struct program_has_win_func_inc<P, std::void_t<decltype(P::win_func_inc(std::declval<const typename P::tuple_t &>(),
+    std::declval<typename P::result_t &>(), std::declval<const typename P::params_t &>()))>> : std::true_type {};
+template <class P>
+int kwi_eval_dispatch(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *woff, const uint32_t *ooff, const uint32_t *n_open,
+                      const uint32_t *run_m, const uint64_t *run_c, const unsigned char *stage, const uint64_t *stage_ts, const uint32_t *n_fired,
+                      const uint32_t *n_out, unsigned char *out, uint64_t *out_ts, unsigned char *pending, uint32_t max_windows, cudaStream_t s,
+                      const void *params)
+{
+    k_kwi_eval<P><<<grid_for(max_windows, 128), 128, 0, s>>>(kw, sorted_slots, n, woff, ooff, n_open, run_m, run_c, stage, stage_ts, n_fired, n_out,
+                                                            out, out_ts, pending, load_params<P>(params));
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+template <class P>
+int kwi_writeback_dispatch(const KwinDev &kw, const uint32_t *sorted_slots, uint32_t n, const uint32_t *ooff, const uint32_t *n_open,
+                           const uint32_t *run_m, const uint64_t *run_c, const unsigned char *pending, uint32_t max_open, cudaStream_t s)
+{
+    k_kwi_writeback<P><<<grid_for(max_open, 256), 256, 0, s>>>(kw, sorted_slots, n, ooff, n_open, run_m, run_c, pending);
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+template <class P>
+int kwi_flush_dispatch(const KwinDev &kw, uint32_t *total, uint32_t cap, unsigned char *out, uint64_t *out_ts, cudaStream_t s)
+{
+    k_kwi_flush<P><<<grid_for(kw.max_keys, 128), 128, 0, s>>>(kw, total, cap, out, out_ts);
+    WFB_CK(cudaGetLastError());
+    return 0;
+}
+
 template <class P>
 int tb_lift_dispatch(const unsigned char *tuples, const uint64_t *ts, uint32_t n, const FfatDev &ff, const TbDev &tb, uint64_t first_incomplete,
                      unsigned char *lifted, uint64_t *ckeys, cudaStream_t s, const void *params)
@@ -542,6 +584,11 @@ ProgramOps make_ops()
         o.has_win_func = 1u;
     } else { o.kw_stage = nullptr; o.kw_eval = nullptr; o.kw_archive = nullptr; o.kw_flush = nullptr; o.has_win_func = 0u; }
     o.reserved4 = 0;
+    if constexpr (program_has_win_func_inc<P>::value) {
+        o.kw_stage = &kw_stage_dispatch<P>; o.kwi_eval = &kwi_eval_dispatch<P>; o.kwi_writeback = &kwi_writeback_dispatch<P>; o.kwi_flush = &kwi_flush_dispatch<P>;
+        o.has_win_func_inc = 1u;
+    } else { o.kwi_eval = nullptr; o.kwi_writeback = nullptr; o.kwi_flush = nullptr; o.has_win_func_inc = 0u; }
+    o.reserved5 = 0;
     return o;
 }
 

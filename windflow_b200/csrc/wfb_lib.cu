@@ -1220,6 +1220,10 @@ struct wfb_kwin {
     Scratch<uint32_t> slotsA, slotsB, posA, posB, wcnt, woff, run_m, tile_cnt, total; // capacity in tuples per call: slotsA's
     Scratch<uint64_t> run_c, stage_ts;
     Scratch<unsigned char> staged;                                                      // the call's tuples in sorted order
+    bool inc = false;             // WFB_KWIN_INCREMENTAL: kw.ring holds accumulators, C of them per key
+    uint32_t open_per_key = 0;    // incremental: ceil(win / slide), the most windows of one key open at once
+    Scratch<uint32_t> ocnt, ooff, otile_cnt, n_open;                                    // incremental: the open windows per run, scanned
+    Scratch<unsigned char> pending;                                                     // incremental: windows opened in the call that stay open
     uint64_t launches = 0;
     PinnedStage stage;
     StreamOrder order;            // a call on another stream waits for the previous call: the scratch and the archive are shared
@@ -1232,17 +1236,20 @@ int wfb_kwin_create(wfb_kwin_t **hh, int prog, uint64_t win, uint64_t slide, uin
     if (!hh || max_keys == 0 || win == 0 || slide == 0) return WFB_E_BADARG;
     const ProgramOps *o = program(prog);
     if (!o) return WFB_E_NOPROG;
-    if (!o->has_win_func) return WFB_E_UNSUPPORTED;  // the program has no win_func
-    if (flags & ~WFB_FFAT_DENSE_KEYS) return WFB_E_UNSUPPORTED;
+    const bool inc = (flags & WFB_KWIN_INCREMENTAL) != 0;
+    if (!(inc ? o->has_win_func_inc : o->has_win_func)) return WFB_E_UNSUPPORTED;  // the program has no win_func_inc / win_func
+    if (flags & ~(WFB_FFAT_DENSE_KEYS | WFB_KWIN_INCREMENTAL)) return WFB_E_UNSUPPORTED;
     if ((flags & WFB_FFAT_DENSE_KEYS) && o->key_kind != KEY_KIND_INTEGRAL) return WFB_E_BADARG; // dense keys are integers
     if (max_keys > (1u << 30) || win > (1ull << 24) || slide > (1ull << 40)) return WFB_E_UNSUPPORTED; // (window ids g * slide + win stay far below 2^64)
-    uint32_t C = 1; while (C < win) C <<= 1;
-    const unsigned __int128 ring_bytes = static_cast<unsigned __int128>(max_keys) * C * o->tuple_bytes;
+    // the ring: pow2ceil(win) tuples per key, or pow2ceil(ceil(win / slide)) accumulators per key for an incremental handle
+    const uint64_t open_per_key = (win + slide - 1) / slide;
+    uint32_t C = 1; while (C < (inc ? open_per_key : win)) C <<= 1;
+    const unsigned __int128 ring_bytes = static_cast<unsigned __int128>(max_keys) * C * (inc ? o->result_bytes : o->tuple_bytes);
     if (ring_bytes > static_cast<unsigned __int128>(SIZE_MAX)) return WFB_E_UNSUPPORTED;
     int rc = device_ready(); if (rc) return rc;
     wfb_kwin *h = new (std::nothrow) wfb_kwin();
     if (!h) return WFB_E_BADARG;
-    h->prog = prog; h->ops = o;
+    h->prog = prog; h->ops = o; h->inc = inc; h->open_per_key = static_cast<uint32_t>(open_per_key);
     { uint32_t bits = 0; while ((1ull << bits) < max_keys) bits++; h->sort_passes = bits / 8 + 1; } // 8·passes > log2(capacity): INVALID_SLOT sorts last
     FfatDev &ff = h->ff;
     ff.max_keys = max_keys; ff.dense = (flags & WFB_FFAT_DENSE_KEYS) ? 1u : 0u;
@@ -1289,6 +1296,28 @@ int wfb_kwin_set_params(wfb_kwin_t *h, const void *params, size_t bytes)
     return 0;
 }
 
+// incremental handle, after the staging gather: 4. the windows every run fires and leaves open, each count scanned into offsets, and the
+// call's count of fired windows; 5. one thread per touched window; 6. the windows opened in the call that stay open into the ring
+static int kwin_inc_windows(wfb_kwin_t *h, const uint32_t *sorted_slots, uint32_t n, uint32_t tiles, uint32_t max_open, void *out_results,
+                            uint64_t *out_ts, uint32_t out_capacity, uint32_t *n_out_dev, cudaStream_t s, const void *f)
+{
+    k_kwi_count<<<grid_for(n, 256), 256, 0, s>>>(h->kw, sorted_slots, n, h->wcnt, h->ocnt, h->run_m, h->run_c);
+    k_flag_tile_counts<uint32_t><<<tiles, 256, 0, s>>>(h->wcnt, n, h->tile_cnt);
+    k_scan_u32<<<1, 1024, 0, s>>>(h->tile_cnt, h->tile_cnt, tiles, h->total);
+    k_kw_offsets<<<tiles, 256, 0, s>>>(h->wcnt, h->tile_cnt, n, h->woff);
+    k_flag_tile_counts<uint32_t><<<tiles, 256, 0, s>>>(h->ocnt, n, h->otile_cnt);
+    k_scan_u32<<<1, 1024, 0, s>>>(h->otile_cnt, h->otile_cnt, tiles, h->n_open);
+    k_kw_offsets<<<tiles, 256, 0, s>>>(h->ocnt, h->otile_cnt, n, h->ooff);
+    k_kw_clamp<<<1, 1, 0, s>>>(h->total, out_capacity, n_out_dev, h->ff.err_flags);
+    CK(cudaGetLastError());
+    int rc = h->ops->kwi_eval(h->kw, sorted_slots, n, h->woff, h->ooff, h->n_open, h->run_m, h->run_c, h->staged, h->stage_ts, h->total, n_out_dev,
+                              static_cast<unsigned char *>(out_results), out_ts, h->pending, std::min(n, out_capacity) + max_open, s, f);
+    if (rc) return rc;
+    rc = h->ops->kwi_writeback(h->kw, sorted_slots, n, h->ooff, h->n_open, h->run_m, h->run_c, h->pending, max_open, s); if (rc) return rc;
+    h->launches += 11;
+    return 0;
+}
+
 int wfb_kwin_process_cb(wfb_kwin_t *h, const wfb_batch_t *batches_h, uint32_t nbatches, void *out_results, uint64_t *out_ts,
                         uint32_t out_capacity, uint32_t *n_out_dev, void *stream)
 {
@@ -1314,6 +1343,9 @@ int wfb_kwin_process_cb(wfb_kwin_t *h, const wfb_batch_t *batches_h, uint32_t nb
     const void *f = h->params.empty() ? nullptr : h->params.data();
     const uint32_t *counts = nullptr, *sorted_slots = nullptr, *sorted_pos = nullptr;
     const size_t TB = h->ops->tuple_bytes;
+    // incremental: the windows the call leaves open, at most open_per_key per key of the call (fired + open stay below 2^32)
+    const uint64_t max_open = h->inc ? std::min<uint64_t>(n, h->ff.max_keys) * h->open_per_key : 0;
+    if (max_open > 0x7fffffffull) return WFB_E_UNSUPPORTED;
     // 1. slots; 2. the stable sort by slot: every key's items contiguous, in arrival order
     rc = keyed_front(h, f, hb, boff, nbatches, n, s,
                      [&](size_t, size_t cap) {
@@ -1321,6 +1353,10 @@ int wfb_kwin_process_cb(wfb_kwin_t *h, const wfb_batch_t *batches_h, uint32_t nb
                          CK(h->stage_ts.ensure(n, s, cap)); CK(h->staged.ensure(n * TB, s, cap * TB));
                          const size_t cnt_cap = (cap + SEGT - 1) / SEGT + 1;
                          CK(h->tile_cnt.ensure(cnt_cap, s, cnt_cap)); CK(h->total.ensure(1, s));
+                         if (h->inc) {
+                             CK(h->ocnt.ensure(n, s, cap)); CK(h->ooff.ensure(n, s, cap)); CK(h->otile_cnt.ensure(cnt_cap, s, cnt_cap));
+                             CK(h->n_open.ensure(1, s)); CK(h->pending.ensure(max_open * h->ops->result_bytes, s));
+                         }
                          return 0;
                      },
                      [](bool *) { return WFB_E_UNSUPPORTED; }, // (the key table does not grow)
@@ -1330,6 +1366,7 @@ int wfb_kwin_process_cb(wfb_kwin_t *h, const wfb_batch_t *batches_h, uint32_t nb
     // 3. gather into the staging buffer; 4. windows per run, their offsets and the call's count; 5. evaluation; 6. archive
     rc = h->ops->kw_stage(h->d_batches, h->d_boff, nbatches, n, sorted_pos, h->staged, h->stage_ts, h->kw.last_ts, s); if (rc) return rc;
     const uint32_t tiles = (n + SEGT - 1) / SEGT;
+    if (h->inc) return kwin_inc_windows(h, sorted_slots, n, tiles, static_cast<uint32_t>(max_open), out_results, out_ts, out_capacity, n_out_dev, s, f);
     k_kw_count<<<grid_for(n, 256), 256, 0, s>>>(h->kw, sorted_slots, n, h->wcnt, h->run_m, h->run_c);
     k_flag_tile_counts<uint32_t><<<tiles, 256, 0, s>>>(h->wcnt, n, h->tile_cnt);
     k_scan_u32<<<1, 1024, 0, s>>>(h->tile_cnt, h->tile_cnt, tiles, h->total);
@@ -1352,7 +1389,8 @@ int wfb_kwin_flush(wfb_kwin_t *h, void *out_results, uint64_t *out_ts, uint32_t 
     int rc = h->order.enter(s); if (rc) return rc;
     CK(h->total.ensure(1, s));
     CK(cudaMemsetAsync(h->total, 0, sizeof(uint32_t), s));
-    rc = h->ops->kw_flush(h->kw, h->total, out_capacity, static_cast<unsigned char *>(out_results), out_ts, s, h->params.empty() ? nullptr : h->params.data());
+    if (h->inc) rc = h->ops->kwi_flush(h->kw, h->total, out_capacity, static_cast<unsigned char *>(out_results), out_ts, s);
+    else rc = h->ops->kw_flush(h->kw, h->total, out_capacity, static_cast<unsigned char *>(out_results), out_ts, s, h->params.empty() ? nullptr : h->params.data());
     if (rc) return rc;
     k_kw_clamp<<<1, 1, 0, s>>>(h->total, out_capacity, n_out_dev, h->ff.err_flags);
     CK(cudaGetLastError());

@@ -248,17 +248,23 @@ class KeyedState:
         return outs, n_out
 
 
+KWIN_INCREMENTAL = 8  # WFB_KWIN_INCREMENTAL
+
+
 class KeyedWindowsGPU:
     """Keyed_Windows_GPU replica state (wf/keyed_windows.hpp, wf/window_replica.hpp): count-based windows whose win_func iterates
-    every tuple of the window, with each key's last pow2ceil(win) tuples in a ring on the device. `prog` must define win_func."""
+    every tuple of the window, with each key's last pow2ceil(win) tuples in a ring on the device. `prog` must define win_func.
+    incremental=True: the program's win_func_inc folds each tuple into every open window it is in, and each key keeps only the
+    accumulators of its open windows (pow2ceil(ceil(win / slide)) of them) on the device."""
 
-    def __init__(self, prog, win, slide, max_keys, dense_keys=False, params=None):
+    def __init__(self, prog, win, slide, max_keys, dense_keys=False, params=None, incremental=False):
         self.L = _lib.lib()
         if self.L.wfb_device_count() <= 0:
             raise RuntimeError("windflow_b200: no CUDA device (there is no CPU fallback)")
         self.h = C.c_void_p()
         self.result_bytes = 0
-        check(self.L.wfb_kwin_create(C.byref(self.h), prog, win, slide, max_keys, 1 if dense_keys else 0), "wfb_kwin_create")
+        flags = (1 if dense_keys else 0) | (KWIN_INCREMENTAL if incremental else 0)
+        check(self.L.wfb_kwin_create(C.byref(self.h), prog, win, slide, max_keys, flags), "wfb_kwin_create")
         info = _lib.ProgramInfo()
         check(self.L.wfb_program_info(prog, C.byref(info)), "wfb_program_info")
         self.result_bytes = info.result_bytes
